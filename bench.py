@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Benchmark of the C2-Matching restoration-forward hot path on B200.
+"""Benchmark of the C2-Matching restoration-forward hot path on H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     (N > 1: python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...)
 
 Metric (BASELINE.json): SR images/s, LR 160x160 -> 640x640 with a 500x500 Ref (zero-padded to
@@ -17,6 +17,9 @@ RestorationPipeline.run_host call), roofline of the dominant kernel class (per-l
 the library on the launching stream in a SEPARATE pass), cpu_baseline (the oracle port of the reference's CPU
 path on this box's physical host cores, bounded sample), parity (image 0 of the timed batch: GPU pipeline vs
 that same oracle run), micro (BASELINE configs 3 and 4), clocks, gpu_launches.
+--dump-outputs DIR writes the SR images of the last timed step as DIR/sr.npy (float32; one sr_rank<r>.npy per rank
+with several GPUs; with --impl reference the CPU oracle's images); the inputs are seeded, so two builds run with the
+same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -139,6 +142,15 @@ def cpu_baseline(pair, timed_runs=3, b4_budget_s=120.0):
     return rec, want
 
 
+def dump_sr(out_dir, sr, rank, world):
+    """SR images of the last timed step -> out_dir/sr.npy (float32); with several ranks each writes its own shard
+    as sr_rank<r>.npy."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    name = 'sr.npy' if world == 1 else f'sr_rank{rank}.npy'
+    np.save(os.path.join(out_dir, name), sr.detach().float().cpu().numpy())
+
+
 # ------------------------------------------------------------------------------- reference arm
 def run_reference(args, rank):
     if rank != 0:
@@ -149,19 +161,17 @@ def run_reference(args, rank):
     torch.set_num_threads(threads)
     sd_e, sd_m, sd_g = seeded_weights()
     img_lq, img_up, img_ref = [t[:1] for t in synthetic_pair(1234, BATCH, LR, REF)]     # bounded sample: image 0, 1 image per step
-    budget_s = 200.0
-    t_est = None
     for _ in range(max(1, min(args.warmup, 1))):
-        t0 = time.perf_counter()
         ref_path.full_forward(sd_e, sd_m, sd_g, img_lq, img_up, img_ref)
-        t_est = time.perf_counter() - t0
-    steps = max(1, min(args.steps, int(budget_s / max(t_est, 1e-3))))
+    steps = max(1, args.steps)
     t0 = time.perf_counter()
     for _ in range(steps):
-        ref_path.full_forward(sd_e, sd_m, sd_g, img_lq, img_up, img_ref)
+        sr = ref_path.full_forward(sd_e, sd_m, sd_g, img_lq, img_up, img_ref)
     dt = time.perf_counter() - t0
+    if args.dump_outputs:
+        dump_sr(args.dump_outputs, sr, rank, 1)
     v = steps / dt
-    sample = (f'1 image per step (config-2 shapes), {steps} timed steps of {args.steps} requested, '
+    sample = (f'1 image per step (config-2 shapes), {steps} timed steps, '
               f'torch-CPU oracle port of the reference path, {threads} threads = physical cores ({logical} logical)')
     print(json.dumps({
         'impl': 'reference', 'metric': 'SR images/sec (160x160->640x640, 500x500 Ref)', 'value': v, 'unit': 'images/s',
@@ -202,7 +212,7 @@ def run_ours(args, rank, world, local_rank):
     host = [t.pin_memory() for t in (img_lq, img_up, img_ref)]
     devt = [t.to(dev) for t in host]
     out_host = torch.empty(BATCH, 3, 4 * LR, 4 * LR, dtype=torch.float32).pin_memory()
-    flush = torch.empty(192 * 1024 * 1024, dtype=torch.uint8, device=dev)       # > 126 MB L2
+    flush = torch.empty(192 * 1024 * 1024, dtype=torch.uint8, device=dev)       # > 50 MB L2
     h2d = sum(t.numel() * t.element_size() for t in host)
     d2h = out_host.numel() * out_host.element_size()
 
@@ -212,17 +222,19 @@ def run_ours(args, rank, world, local_rank):
         torch.cuda.synchronize(dev)
 
     def timed(fn, steps):
-        """K steps, each bracketed by events on the current stream, L2 flushed (untimed) between them."""
+        """K steps, each bracketed by events on the current stream, L2 flushed (untimed) between them.
+        Returns (ms, what the last step returned)."""
         evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(steps)]
+        out = None
         barrier()
         for e0, e1 in evs:
             flush.fill_(1)
             e0.record()
-            fn()
+            out = fn()
             e1.record()
         barrier()
         ms = sum(e0.elapsed_time(e1) for e0, e1 in evs)
-        return max_over_ranks(ms, dev)
+        return max_over_ranks(ms, dev), out
 
     step_eager = lambda: pipe.forward(*devt)
     step_dev = (lambda: pipe.forward_graphed(*devt)) if args.cuda_graph else step_eager
@@ -245,16 +257,18 @@ def run_ours(args, rank, world, local_rank):
         sampler.start()
     # (1) the headline numbers: library profiling hook OFF, nothing but the step inside the events
     ops.profile_enable(False)
-    ms_dev = timed(step_dev, args.steps)
+    ms_dev, last_sr = timed(step_dev, args.steps)
+    if args.dump_outputs:
+        dump_sr(args.dump_outputs, last_sr, rank, world)
     launches = launches_per_step * args.steps
-    ms_e2e = timed(step_e2e, args.steps)
+    ms_e2e, _ = timed(step_e2e, args.steps)
     clocks = sampler.stop() if sampler else None
     # (2) separate pass for the per-kernel-class device times (2 cudaEventRecord per launch: not part of `value`)
     prof_steps = max(1, min(args.steps, 5))
     ops.profile_enable(True)
     for k in ops.PROF_KERNELS:
         ops.profile_collect(k)
-    ms_prof = timed(step_eager, prof_steps)
+    ms_prof, _ = timed(step_eager, prof_steps)
     prof = {k: ops.profile_collect(k) for k in ops.PROF_KERNELS}
     ops.profile_enable(False)
 
@@ -271,7 +285,7 @@ def run_ours(args, rank, world, local_rank):
         peak = peaks.get('bf16_tflops_sustained')       # kernel timed inside a long step -> sustained figure
         peak_src = 'measured (MEASURED_PEAKS.json bf16_tflops_sustained)'
         if not peak:
-            peak, peak_src = 1400.0, 'fallback (B200_PROFILING.md: ~1.4 PFLOP/s sustained)'
+            peak, peak_src = 989.0, 'data sheet (H100 SXM, dense fp16, 700 W), not a measured figure'
         # per kernel class: device time inside the timed steps (CUDA events on the launching stream,
         # recorded by the library), algorithmic flops / bytes per SURVEY.md §8(d)
         classes = {}
@@ -283,21 +297,13 @@ def run_ours(args, rank, world, local_rank):
                               'algorithmic_gbps': r['bytes'] / (r['ms'] / 1e3) / 1e9}
         dom = max(prof, key=lambda k: prof[k]['ms'])
         r = prof[dom]
-        name = {'corr_search': 'corr_umma_kernel', 'conv3x3': 'conv3x3_umma_kernel', 'dcn': 'dcn_umma_kernel'}[dom]
+        name = {'corr_search': 'corr_umma_kernel', 'conv3x3': 'conv3x3_wgmma_kernel', 'dcn': 'dcn_wgmma_kernel'}[dom]
         achieved = r['flops'] / (r['ms'] / 1e3) / 1e12
-        traffic, traffic_shape = None, None
-        try:
-            tj = json.load(open(os.path.join(ROOT, 'profiles', 'dominant_kernel_traffic.json')))
-            traffic = tj.get(name)                      # ncu dram read+write per launch (null if shapes vary)
-            if (tj.get('dominant_shape') or {}).get('kernel') == name:
-                traffic_shape = tj['dominant_shape']
-        except Exception:
-            pass
         # conv / dcn: three split products per algorithmic product.  corr: only the three ROW taps are MMAs (1/3 of the
         # nine-tap flops), x2 products ((q_hi + q_lo) * r_hi), x(16/14)^2 for the halo columns of the 16-px blocks = 0.87
         issued = {'conv3x3': 3.0, 'corr_search': 2.0 / 3.0 * (16.0 / 14.0) ** 2, 'dcn': 3.0}[dom]
         roofline = {'bound': 'tensor', 'kernel': name, 'achieved': achieved, 'peak': peak, 'unit': 'TFLOP/s',
-                    'frac': achieved / peak, 'traffic': traffic, 'traffic_dominant_shape': traffic_shape,
+                    'frac': achieved / peak,
                     'peak_source': peak_src,
                     'ms_per_launch': r['ms'] / r['launches'], 'launches_timed': r['launches'],
                     'algorithmic_flops_per_launch': r['flops'] / r['launches'],
@@ -317,17 +323,18 @@ def run_ours(args, rank, world, local_rank):
             cpu, want = cpu_baseline((img_lq, img_up, img_ref))
             parity = full_forward_parity(pipe, seeded_weights(), img_lq[:1], img_up[:1], img_ref[:1], want=want)
             parity['note'] = ('image 0 of the timed batch vs oracle/ref_path.full_forward on the same inputs: idx_flips = '
-                              'queries whose index differs from the oracle end to end (features from tcgen05 convs vs '
+                              'queries whose index differs from the oracle end to end (features from tensor-core convs vs '
                               'oneDNN), max_gap64_of_flips = largest fp64 score difference between the two candidates of '
                               'a flipped query, sr_max_rel_err = SR vs the oracle restoration evaluated on this run\'s own '
                               'index map, psnr_delta_db = |PSNR(ours) - PSNR(oracle end to end)| with the reference metric')
         if world == 1 and not args.no_micro:
             sys.path.insert(0, os.path.join(ROOT, 'tools'))
             import microbench
-            micro = {'peak_tflops': peaks.get('bf16_tflops') or 1590.0, 'peak_hbm_gbs': peaks.get('hbm_gbs') or 6650.0,
-                     'peaks': 'MEASURED_PEAKS.json burst figures (kernels timed alone)' if peaks else 'fallback',
-                     'rows': microbench.run_config3(dev, flush, peaks.get('bf16_tflops') or 1590.0) +
-                             microbench.run_config4(dev, flush, peaks.get('hbm_gbs') or 6650.0)}
+            micro = {'peak_tflops': peaks.get('bf16_tflops') or 989.0, 'peak_hbm_gbs': peaks.get('hbm_gbs') or 3350.0,
+                     'peaks': 'MEASURED_PEAKS.json burst figures (kernels timed alone)' if peaks else
+                              'H100 SXM data sheet (dense fp16, HBM3), not measured',
+                     'rows': microbench.run_config3(dev, flush, peaks.get('bf16_tflops') or 989.0) +
+                             microbench.run_config4(dev, flush, peaks.get('hbm_gbs') or 3350.0)}
         print(json.dumps({
             'metric': 'SR images/sec (160x160->640x640, 500x500 Ref)', 'value': value, 'unit': 'images/s',
             'n_gpus': world, 'steps': args.steps, 'warmup': max(args.warmup, 3),
@@ -335,7 +342,7 @@ def run_ours(args, rank, world, local_rank):
             'dtype': 'f32', 'data': 'synthetic',
             'config': {'workload': WORKLOAD, 'global_batch': BATCH * world, 'parallelism': f'dp{world} (batch-sharded pairs, no data-path collective)',
                        'l2': 'flushed between timed steps (192 MiB fill)', 'profiling_hook': 'off while `value` / `e2e` are timed', 'cuda_graph': bool(args.cuda_graph), 'weights': 'random-init (seeded), real architecture',
-                       'convs': 'hand-written tcgen05 3x3 kernel, split-fp16 operands, fp32 accumulate (fp32-grade); '
+                       'convs': 'hand-written wgmma 3x3 kernel, split-fp16 operands, fp32 accumulate (fp32-grade); '
                                 'cuDNN is not on the path', 'cudnn_tf32_allowed': bool(args.tf32)},
             'e2e': {'value': e2e, 'unit': 'images/s', 'h2d_bytes_per_step': h2d, 'd2h_bytes_per_step': d2h,
                     'ms_per_step': ms_e2e / args.steps, 'api': 'c2m_b200.pipeline.RestorationPipeline.run_host'},
@@ -446,8 +453,7 @@ def main():
     ap.add_argument('--tf32', type=int, default=0, help='allow cuDNN TF32 for the plain convolutions (default: exact fp32)')
     ap.add_argument('--channels-last', type=int, default=0)
     ap.add_argument('--cuda-graph', type=int, default=0,
-                    help='replay the forward from a CUDA graph captured per input shape (same kernels, bit-identical results; measured: no '
-                         'gain, 100.7 vs 101.1 images/s — the step runs at the power cap, not at the launch rate)')
+                    help='replay the forward from a CUDA graph captured per input shape (same kernels, bit-identical results)')
     ap.add_argument('--no-cpu-baseline', action='store_true', help='skip the CPU oracle leg (cpu_baseline + parity)')
     ap.add_argument('--no-micro', action='store_true', help='skip the config-3 / config-4 microbenchmarks')
     ap.add_argument('--workload', choices=['config2', 'config5'], default='config2',
@@ -459,7 +465,12 @@ def main():
     ap.add_argument('--metrics-device', choices=['cuda', 'cpu'], default='cuda',
                     help="config5: where PSNR/SSIM run ('cpu' = the reference's numpy/cv2 arithmetic on a thread pool)")
     ap.add_argument('--per-batch-workers', action='store_true', help='config5: one BATCH per loader-worker task')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the SR images of the last timed step as DIR/sr.npy (float32; sr_rank<r>.npy per rank '
+                         'when --gpus > 1); config2 only')
     args = ap.parse_args()
+    if args.dump_outputs and args.workload != 'config2':
+        ap.error('--dump-outputs applies to the config2 workload (config5 reports metrics, not images)')
     rank = int(os.environ.get('RANK', 0))
     world = int(os.environ.get('WORLD_SIZE', 1))
     local_rank = int(os.environ.get('LOCAL_RANK', 0))

@@ -1,4 +1,4 @@
-"""c2m_b200 — host side of the B200-native C2-Matching restoration-forward hot path.
+"""c2m_b200 — host side of the H100-native C2-Matching restoration-forward hot path.
 
 Python/PyTorch is plumbing (device memory, streams, torch.distributed); the arithmetic lives in
 libc2m_sm100.so (csrc/, C ABI in include/c2m_sm100.h)."""

@@ -96,7 +96,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise C2MError(
                 f'{LIB_PATH} not built: run `python -c "import __graft_entry__ as g; g.build()"` '
-                '(no CPU/PyTorch fallback exists for the B200 hot path)')
+                '(no CPU/PyTorch fallback exists for the H100 hot path)')
         l = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in SYMBOLS.items():
             fn = getattr(l, name)          # AttributeError if the .so does not export it

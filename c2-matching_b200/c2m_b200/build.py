@@ -1,4 +1,4 @@
-"""Build libc2m_sm100.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Build libc2m_sm100.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
 import os
 import subprocess
 
@@ -7,7 +7,7 @@ CSRC = os.path.join(PKG_ROOT, 'csrc')
 LIB_DIR = os.path.join(PKG_ROOT, 'lib')
 LIB_PATH = os.path.join(LIB_DIR, 'libc2m_sm100.so')
 SOURCES = ['c_abi.cu', 'corr_aux.cu', 'corr_umma.cu', 'dcn_v2.cu', 'offsets.cu', 'conv3x3_umma.cu', 'dcn_umma.cu', 'dcn_bwd.cu']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-shared', '-Xcompiler', '-fPIC']
 
 

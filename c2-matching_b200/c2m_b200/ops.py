@@ -200,7 +200,7 @@ def dcn_v2_fused_forward(x, om, weight, bias, deformable_group, pre_offset=None,
 
 
 # ------------------------------------------------------------------------------------------------
-# Packed-split activations ("PSA") and the tcgen05 3x3 convolution (include/c2m_sm100.h)
+# Packed-split activations ("PSA") and the tensor-core 3x3 convolution (include/c2m_sm100.h)
 class PSA:
     """fp16 hi/lo planes [B][ceil(C/8)][H][W][8]; value = (hi + lo) * 2^-sa."""
     __slots__ = ('hi', 'lo', 'B', 'C', 'H', 'W', 'sa')
@@ -301,7 +301,7 @@ def psa_maxpool2(p):
 
 
 def conv3x3_supported(cin, cout, H=None, W=None):
-    """The tcgen05 kernel takes any channel counts; maps must hold one halo tile (18 x 10)."""
+    """The tensor-core kernel takes any channel counts; maps must hold one halo tile (18 x 10)."""
     return H is None or (H >= 18 and W >= 10)
 
 

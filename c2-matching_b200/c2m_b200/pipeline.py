@@ -26,7 +26,7 @@ class RestorationPipeline:
     def __init__(self, device, ngf=64, n_blocks=16, groups=8, channels_last=False, allow_tf32=False, cuda_graph=False):
         self.device = torch.device(device)
         if self.device.type != 'cuda':
-            raise RuntimeError('RestorationPipeline needs a CUDA device (no CPU fallback for the B200 hot path)')
+            raise RuntimeError('RestorationPipeline needs a CUDA device (no CPU fallback for the H100 hot path)')
         self.net_extractor = ContrasExtractorSep()
         self.net_map = CorrespondenceGenerationArch(3, 1, ['relu1_1', 'relu2_1', 'relu3_1'], 'vgg19')
         self.net_g = RestorationNet(ngf=ngf, n_blocks=n_blocks, groups=groups)

@@ -1,5 +1,5 @@
-// Shared helpers for libc2m_sm100: error plumbing, launch accounting and the sm_100a PTX
-// wrappers (mbarrier, TMA, tcgen05/TMEM) used by the kernels.  sm_100a only.
+// Shared helpers for libc2m_sm100: error plumbing, launch accounting and the sm_90a PTX
+// wrappers (mbarrier, TMA, wgmma) used by the kernels.  sm_90a only.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -8,6 +8,7 @@
 #include <stdio.h>
 
 #include "../../include/c2m_sm100.h"
+#include "wgmma_f16.cuh"
 
 namespace c2m {
 
@@ -121,198 +122,42 @@ __device__ __forceinline__ void tma_load_4d(void *dst, const void *tmap, uint64_
         : "memory");
 }
 
-// ---- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t *smem_result, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(smem_result)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], fp16/bf16 inputs, fp32 accumulate; issued by ONE thread.
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                         uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// Single-thread issue with split descriptor words (inside `if (elect_one())`).
-__device__ __forceinline__ void umma_f16_1(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                           uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-        "mov.b64 da, {%1, %2};\n\t"
-        "mov.b64 db, {%3, %4};\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}"
-        ::"r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// Warp-uniform issue: called by ALL 32 lanes of the issuing warp under uniform control flow; one lane, elected inside
-// the asm, issues.  With `if (lane == 0) { ... umma_f16(...) }` ptxas wraps every MMA in an ELECT / R2UR.BROADCAST /
-// BRA.U.ANY loop (~11 SASS instructions, ~80 cycles per MMA measured) — longer than a 128x64x16 MMA occupies the pipe.
-// Descriptors are passed as (low word, high word): the low word is `base + constant` in 32-bit arithmetic, which ptxas
-// keeps on the uniform datapath; a 64-bit descriptor value is computed in vector registers and costs R2UR moves.
-__device__ __forceinline__ void umma_f16_w(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                           uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p, q;\n\t.reg .b64 da, db;\n\t"
-        "mov.b64 da, {%1, %2};\n\t"
-        "mov.b64 db, {%3, %4};\n\t"
-        "elect.sync _|q, 0xffffffff;\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "@q tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}"
-        ::"r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_f16_w(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                           uint32_t accumulate) {
-    umma_f16_w(d_tmem, (uint32_t)a_desc, (uint32_t)(a_desc >> 32), (uint32_t)b_desc, (uint32_t)(b_desc >> 32), idesc, accumulate);
-}
-__device__ __forceinline__ void umma_commit_w(uint64_t *bar) {
-    asm volatile(
-        "{\n\t.reg .pred q;\n\t"
-        "elect.sync _|q, 0xffffffff;\n\t"
-        "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}"
-        ::"r"(smem_u32(bar))
-        : "memory");
-}
-// mbarrier arrives once all tcgen05 ops issued so far by this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                     smem_u32(bar))
-                 : "memory");
-}
-// 32 lanes x 32 consecutive 32-bit columns -> 32 registers per thread (thread i <-> lane base+i)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]),
-          "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]),
-          "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]),
-          "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// ---- wgmma (warpgroup MMA, sm_90a): issued by all 128 threads of a warpgroup, accumulator in registers
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-// Shared-memory matrix descriptor, K-major, SWIZZLE_NONE ("interleave"): core matrix = 8 rows
-// x 16 bytes, rows 16 B apart; `lbo` = byte distance between the two K core matrices of one
-// UMMA_K=16 step, `sbo` = byte distance between consecutive 8-row groups along M/N.
-// Field layout: cute/arch/mma_sm100_desc.hpp (SmemDescriptor): start[0,14) lbo[16,30) sbo[32,46)
-// version[46,48)=1 layout_type[61,64)=0.
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
-    return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32) |
-           (1ull << 46);
+// Shared-memory matrix descriptor, K-major, no swizzle ("interleave"): core matrix = 8 rows x 16 bytes, rows 16 B
+// apart; `lbo` = byte distance between the two K core matrices of one K=16 step, `sbo` = byte distance between
+// consecutive 8-row groups along M/N.  Fields: start[0,14) lbo[16,30) sbo[32,46), layout type [62,64) = 0.
+__device__ __forceinline__ uint64_t wg_smem_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
+    return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32);
 }
-// Same descriptor advanced by `byte_off` (multiple of 16; the 14-bit start-address field cannot
-// carry: shared memory is < 2^18 bytes) — one 32-bit add on the low word.
-__device__ __forceinline__ uint64_t umma_desc_advance(uint64_t desc, uint32_t byte_off) {
+// Same descriptor advanced by `byte_off` (multiple of 16; the 14-bit start-address field cannot carry: shared
+// memory is < 2^18 bytes) — one 32-bit add on the low word.
+__device__ __forceinline__ uint64_t wg_desc_advance(uint64_t desc, uint32_t byte_off) {
     const uint32_t lo = (uint32_t)desc + (byte_off >> 4);
     return (desc & 0xFFFFFFFF00000000ull) | lo;
 }
-// Instruction descriptor for kind::f16: D fp32, A/B fp16 (0) or bf16 (1), both K-major.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N, int ab_fmt) {
-    return (1u << 4) | ((uint32_t)ab_fmt << 7) | ((uint32_t)ab_fmt << 10) | ((uint32_t)(N >> 3) << 17) |
-           ((uint32_t)(M >> 4) << 24);
-}
 
-// ---- CTA pairs (cta_group::2): cluster of two CTAs on one TPC sharing one UMMA of M = 256.  Only the leader
-// (cluster rank 0) issues MMAs; each CTA feeds its own 128 A rows and HALF of the B rows from its own shared memory
-// (same offsets in both CTAs) and receives its own 128 accumulator lanes in its own TMEM.
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of `local_smem_addr` (a shared::cta address of THIS CTA) in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t local_smem_addr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_smem_addr), "r"(rank));
-    return r;
-}
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t *smem_result, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish2() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma2_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma2_f16_w(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                            uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p, q;\n\t.reg .b64 da, db;\n\t"
-        "mov.b64 da, {%1, %2};\n\t"
-        "mov.b64 db, {%3, %4};\n\t"
-        "elect.sync _|q, 0xffffffff;\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "@q tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %5, p;\n\t}"
-        ::"r"(d_tmem), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit2_w(uint64_t *bar) {
-    const uint16_t mask = 3;
-    asm volatile(
-        "{\n\t.reg .pred q;\n\t"
-        "elect.sync _|q, 0xffffffff;\n\t"
-        "@q tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n\t}"
-        ::"r"(smem_u32(bar)), "h"(mask)
-        : "memory");
-}
-// arrive (once all tcgen05 ops issued so far by this thread have completed) on the barrier at this shared-memory
-// offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma_commit2(uint64_t *bar) {
-    const uint16_t mask = 3;
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                     smem_u32(bar)),
-                 "h"(mask)
-                 : "memory");
-}
+// ---- accumulator staging: the epilogues read a finished tile from shared memory as [column][row] fp32 with
+// ACC_PITCH floats per column (row fastest: one thread per row reads a column without bank conflicts, and the
+// fragment stores below hit 32 distinct banks because 2 * ACC_PITCH = 8 mod 32).
+constexpr int ACC_PITCH = 132;
+__host__ __device__ constexpr int acc_stage_bytes(int cols) { return cols * ACC_PITCH * 4; }
 
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "elect.sync _|p, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(pred));
-    return pred != 0;
+// Store the calling warpgroup's 64 x (2R) wgmma fragment as rows [row0, row0 + 64) of the staging buffer.
+template <int R>
+__device__ __forceinline__ void acc_store(float *acc_s, int row0, const float (&d)[R]) {
+    const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+    float *base = acc_s + row0 + 16 * w + (l >> 2) + 2 * (l & 3) * ACC_PITCH;
+#pragma unroll
+    for (int i = 0; i < R; ++i) base[(8 * (i >> 2) + (i & 1)) * ACC_PITCH + 8 * ((i >> 1) & 1)] = d[i];
+}
+// Columns [c0, c0 + 32) of one row (`acc_row` = staging buffer + row); columns at or beyond `ncol` read as 0.
+__device__ __forceinline__ void acc_ld32(const float *acc_row, int c0, int ncol, uint32_t (&r)[32]) {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) r[j] = c0 + j < ncol ? __float_as_uint(acc_row[(c0 + j) * ACC_PITCH]) : 0u;
 }
 #endif  // __CUDACC__
 

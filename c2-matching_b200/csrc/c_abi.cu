@@ -132,21 +132,24 @@ extern "C" int c2m_corr_argmax_f32(const float *fin, const float *fref, int B, i
         C2M_CUDA(cudaGetDevice(&dev));
         C2M_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
         C2M_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-        if (major != 10) {
-            set_error("corr_argmax: tcgen05 path needs an sm_100 device (found sm_%d*)", major);
+        if (major != 9) {
+            set_error("corr_argmax: wgmma path needs an sm_90 device (found sm_%d*)", major);
             return C2M_ERR_UNSUPPORTED;
         }
         ws.nchunk = corr_umma_pick_nchunk(g, sms);
         if (const char *ev = getenv("C2M_CORR_NCHUNK")) { const int n = atoi(ev); if (n >= 1 && n <= CORR_MAX_CHUNKS) ws.nchunk = n; }   // experiments
         corr_umma_chunk_geom(g, ws.nchunk, cg);
         // DESIGN.md K2: the search scores (q_hi + q_lo) . r_hi.  |approx - exact| <= E = [2^-11 + 2^-22 (K/16 + 3)] ||P_q||
-        // ||P_r|| rinv_r: 2^-11 = fp16 rounding of the Ref operand (Cauchy-Schwarz over the patch), K/16 tcgen05
+        // ||P_r|| rinv_r: 2^-11 = fp16 rounding of the Ref operand (Cauchy-Schwarz over the patch), K/16 wgmma
         // instructions feed each score with 1 fp32 ulp of (|acc| + sum|products|) each, + the query's 2^-22 split.
         // Window = 2E for the rounding part (best and candidate both err; 1 % margin for the fp16 subnormal range) and 4E
         // for the accumulation part (x2 of slack for the tensor core's internal alignment).
         window_coef = 1.01f * ldexpf(1.f, -10) + ldexpf(1.f, -20) * (float)((K + 15) / 16 + 3);
     } else {
-        int n = ceil_div(4 * 148, g.B * ceil_div(g.NQ, 64));
+        int dev = 0, sms = 0;
+        C2M_CUDA(cudaGetDevice(&dev));
+        C2M_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+        int n = ceil_div(4 * sms, g.B * ceil_div(g.NQ, 64));
         const int ntile = ceil_div(g.NR, 64);
         if (n > CORR_MAX_CHUNKS) n = CORR_MAX_CHUNKS;
         if (n > ntile) n = ntile;

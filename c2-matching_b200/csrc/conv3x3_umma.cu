@@ -1,22 +1,21 @@
-// 3x3 / stride 1 / pad 1 convolution on the sm_100a tensor cores with fp32-grade accuracy
-// ("fp16 x 3": split operands hi + lo, hi*hi + hi*lo + lo*hi accumulated in fp32 TMEM).
+// 3x3 / stride 1 / pad 1 convolution on the sm_90a tensor cores (wgmma) with fp32-grade accuracy
+// ("fp16 x 3": split operands hi + lo, hi*hi + hi*lo + lo*hi accumulated in fp32).
 //
 // SURVEY.md §8(f) N3: once the correlation and DCN are fused, the 128 plain 3x3 convolutions of
 // RestorationNet (ResidualBlockNoBN chains, mmsr/models/archs/arch_util.py:80-136;
-// ref_restoration_arch.py:22-27,92-95,...) are ~80 % of the step when run as exact-fp32 cuDNN
-// SIMT kernels (profiles/r01_launches_step_fp32.md).  This kernel keeps fp32-grade results
-// (<= 2^-21 relative per product) at tensor-core speed.
+// ref_restoration_arch.py:22-27,92-95,...) dominate the step when run as exact-fp32 cuDNN
+// SIMT kernels.  This kernel keeps fp32-grade results (<= 2^-21 relative per product) at
+// tensor-core speed.
 //
 // Same trick as corr_umma.cu: activations live in the packed-split layout ("PSA")
 //      hi, lo : fp16 [B][C/8][H][W][8]
 // so ONE TMA box (10 cols x 18 rows x 4 channel octets, origin (x0-1, y0-1): padding = TMA
-// out-of-bounds zero fill) per operand half stages a halo'd 16x8-pixel tile in the tcgen05
-// K-major no-swizzle layout, and the 9 filter taps are 9 MMAs whose A descriptors differ only
+// out-of-bounds zero fill) per operand half stages a halo'd 16x8-pixel tile in the wgmma
+// K-major no-swizzle layout, and the 9 filter taps are MMAs whose A descriptors differ only
 // in start address.  The B operand is the weight matrix [Cout x Cin] of the tap, pre-packed
-// (c2m_conv3x3_pack_weights_f32) as split fp16 [Cin/32][tap][octet][Cout][8] and kept RESIDENT in
-// shared memory for the whole persistent CTA (<= 147 KB for 64 -> 64), so the only streaming
-// traffic is the activation tile: the kernel is HBM-bound on its own input/output, not L2-bound
-// on weights.  Epilogue (4 warps, one output pixel per thread): *2^-(sa+sw) + bias, ReLU /
+// (c2m_conv3x3_pack_weights_f32) as split fp16 [Cin/32][tap][octet][hi | lo][Cout][8] and kept RESIDENT in
+// shared memory for the whole persistent CTA when it fits (<= 147 KB for 64 -> 64), so the only streaming
+// traffic is the activation tile.  Epilogue (one output pixel per thread): *2^-(sa+sw) + bias, ReLU /
 // LeakyReLU, optional residual add (a second PSA tensor), re-split to hi/lo and store — the
 // output is directly the next convolution's operand, no fp32 round trip through HBM.
 #include <cstdlib>
@@ -26,51 +25,55 @@
 namespace c2m {
 
 namespace {
-constexpr int T_R = 16, T_C = 8;          // output pixel tile -> UMMA M = 128
+constexpr int T_R = 16, T_C = 8;          // output pixel tile -> M = 128 (two m64 warpgroups)
 constexpr int A_R = T_R + 2, A_C = T_C + 2;
 constexpr int KOCT = 4;                   // channel octets per K chunk (32 channels)
 constexpr int ROW_B = A_C * 16;           // 160 B  (SBO of A)
 constexpr int A_OCT_B = A_R * ROW_B;      // 2880 B (LBO of A)
 constexpr int A_HALF = KOCT * A_OCT_B;    // 11520 B (hi or lo of one stage)
 constexpr int A_STAGE = 2 * A_HALF;       // 23040 B
-constexpr int NSTAGE = 3;                 // activation ring
 constexpr int NBST = 2;                   // weight-chunk double buffer
-constexpr int MAXT = 8;                   // pixel tiles per work item (one TMEM accumulator each)
+constexpr int MAXT = 8;                   // pixel tiles per work item
 constexpr int NMAX = 64;                  // output channels per CTA slice
 constexpr int W_HDR = 256;                // packed-weight blob header bytes
+// activation ring depth: what is left of the 227 KB next to two weight slots and the accumulator staging
+__host__ __device__ constexpr int conv_nstage(int N) { return N >= 64 ? 2 : 4; }
+constexpr size_t conv_smem_bytes(int N) {
+    return (size_t)NBST * 2 * 9 * KOCT * N * 16 + (size_t)conv_nstage(N) * A_STAGE + acc_stage_bytes(N) + 2048;
+}
 
 }  // namespace
 
 // ------------------------------------------------------------------------------------------
-// Work item = (image, super-tile of up to 8 consecutive 16x8 pixel tiles, 64-wide Cout slice).
-// K loop: for each 32-channel chunk kc the slice's weight chunk (9 taps, hi+lo, N*1152 B) is
-// bulk-copied ONCE into a double-buffered smem slot and used by all T pixel tiles of the item
-// (T TMEM accumulators of N columns), so weight traffic per MMA is 1/T of a per-tile stream and
-// any Cin/Cout fits; 64->64 degenerates to 2 chunks per item.  Activation stages stream
-// through a 3-deep TMA ring exactly as in the correlation kernel.
+// Work item = (image, super-tile of up to MAXT consecutive 16x8 pixel tiles, 64-wide Cout slice).
+// Warpgroup 0 produces: warp 0 streams the activation stages (one per (tile, kc), tile-major) through the TMA ring,
+// warp 3 bulk-copies the slice's weight chunks (9 taps, hi+lo, N*1152 B per 32-channel chunk kc).  When all chunks
+// of the slice fit the two slots (nslice == 1, nkc <= 2) they are loaded once per CTA and stay resident; otherwise
+// they are streamed per (item, kc) and the host gives every item a single tile.
+// Warpgroups 1 and 2 consume: warpgroup c issues the wgmmas of output rows [64c, 64c + 64) (pixel rows 8c..8c+7)
+// of every tile, stages its accumulator in shared memory and runs the epilogue of those 64 pixels.
+// Per K step: x_hi * [W_hi | W_lo] (B = the 2N stacked weight rows, n = 2N) + x_lo * W_hi (n = N, into the first
+// N columns of the same accumulator); the two halves are summed before staging.
 // ------------------------------------------------------------------------------------------
+template <int N>
 __global__ void __launch_bounds__(384, 1)
-conv3x3_umma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo,
-                    const __grid_constant__ CUtensorMap tm2_hi, const __grid_constant__ CUtensorMap tm2_lo,
-                    const ConvPtrs q, const ConvParams p) {
+conv3x3_wgmma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo,
+                     const __grid_constant__ CUtensorMap tm2_hi, const __grid_constant__ CUtensorMap tm2_lo,
+                     const ConvPtrs q, const ConvParams p) {
+    constexpr int NST = conv_nstage(N);
+    constexpr uint32_t w_chunk = 2u * 9 * KOCT * N * 16;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    const uint32_t w_half = 9u * KOCT * p.N * 16;                        // bytes of one chunk half
-    const uint32_t w_chunk = 2 * w_half;
-    uint8_t *sW = smem;                                                  // [NBST][hi | lo]
+    uint8_t *sW = smem;                                                  // [NBST][w_chunk]
     uint8_t *sA = smem + NBST * w_chunk;                                 // multiple of 128 already
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sA + NSTAGE * A_STAGE);
-    uint64_t *full = bars, *empty = full + NSTAGE, *bfull = empty + NSTAGE, *bempty = bfull + NBST,
-             *tfull = bempty + NBST, *tempty = tfull + MAXT;
-    uint32_t *tmem_base_p = reinterpret_cast<uint32_t *>(tempty + MAXT);
-    float *sbias = reinterpret_cast<float *>(tmem_base_p + 4);           // [N], 16 B aligned (float4 reads)
+    float *acc_s = reinterpret_cast<float *>(sA + NST * A_STAGE);        // [N][ACC_PITCH]
+    uint64_t *bars = reinterpret_cast<uint64_t *>(reinterpret_cast<uint8_t *>(acc_s) + acc_stage_bytes(N));
+    uint64_t *full = bars, *empty = full + NST, *bfull = empty + NST, *bempty = bfull + NBST;
+    float *sbias = reinterpret_cast<float *>(bempty + NBST);             // [2][UC_NMAX], 16 B aligned (float4 reads)
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tiles_img = p.tiles_x * p.tiles_y;
     const int n_items = p.B * p.n_st * p.nslice;
-    const uint32_t need_cols = 2u * p.N * p.T;            // stacked accumulators: 2N columns per tile
-    const uint32_t tmem_cols = need_cols <= 32 ? 32 : need_cols <= 64 ? 64 : need_cols <= 128 ? 128
-                               : need_cols <= 256 ? 256 : 512;
 
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tm_hi);
@@ -79,19 +82,11 @@ conv3x3_umma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_cons
         tma_prefetch_desc(&tm2_lo);
     }
     if (warp == 1 && lane == 0) {
-        for (int i = 0; i < NSTAGE; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-        for (int i = 0; i < NBST; ++i) { mbar_init(&bfull[i], 1); mbar_init(&bempty[i], 1); }
-        for (int i = 0; i < MAXT; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], 8); }
+        for (int i = 0; i < NST; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 256); }
+        for (int i = 0; i < NBST; ++i) { mbar_init(&bfull[i], 1); mbar_init(&bempty[i], 256); }
         fence_mbar_init();
     }
-    if (warp == 2) {
-        tmem_alloc(tmem_base_p, tmem_cols);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_base_p;
     const int sw = *reinterpret_cast<const int *>(q.wblob);              // weight scale exponent
     // all weight chunks of the (single) slice fit the chunk slots: load them once per CTA, not per item
     const bool w_resident = p.nslice == 1 && p.nkc <= NBST;
@@ -106,514 +101,143 @@ conv3x3_umma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_cons
         nt = min(p.T, tiles_img - t0);
     };
 
-    // Register budget per warpgroup; the CTA's pool is what it was launched with (168 x 384 = 64512):
-    // control warpgroup 88 (the MMA issuer keeps its precomputed descriptors in registers), the two
-    // epilogue warpgroups 208 each (88 + 2 x 208 = 3 x 168): no spills on either side.
     if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 88;");
-    if (warp == 0) {
-        // ================================ activation producer ===============================
-        if (lane == 0) {
-            int stage = 0, phase = 0, n_issued = 0;
-            for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-                int b, t0, nt, slice;
-                decode(item, b, t0, nt, slice);
-                for (int kc = 0; kc < p.nkc; ++kc) {
-                    const bool first = kc < p.nkc_a;
-                    const CUtensorMap *mh = first ? &tm_hi : &tm2_hi, *ml = first ? &tm_lo : &tm2_lo;
-                    const int oct0 = (first ? kc : kc - p.nkc_a) * KOCT;
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (warp == 0) {
+            // ================================ activation producer ===============================
+            if (lane == 0) {
+                int stage = 0, phase = 0, n_issued = 0;
+                for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+                    int b, t0, nt, slice;
+                    decode(item, b, t0, nt, slice);
                     for (int t = 0; t < nt; ++t) {
                         const int tt = t0 + t;
                         const int y0 = (tt / p.tiles_x) * T_R, x0 = (tt % p.tiles_x) * T_C;
-                        mbar_wait(&empty[stage], phase ^ 1);
-                        uint8_t *s = sA + stage * A_STAGE;
-                        if ((p.dbg & 2) && n_issued >= NSTAGE) {
-                            mbar_arrive(&full[stage]);                 // experiment: reuse stale tiles
-                        } else {
-                            mbar_arrive_expect_tx(&full[stage], A_STAGE);
-                            tma_load_4d(s, mh, &full[stage], (x0 - 1) * 8, y0 - 1, oct0, b);
-                            tma_load_4d(s + A_HALF, ml, &full[stage], (x0 - 1) * 8, y0 - 1, oct0, b);
-                        }
-                        ++n_issued;
-                        if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
-                    }
-                }
-            }
-        }
-    } else if (warp == 3) {
-        // ================================ weight producer ===================================
-        // its own thread: a chunk is requested the moment its slot frees, not after the
-        // activation stream of the previous chunk has been issued
-        if (lane == 0) {
-            int bst = 0, bphase = 0;
-            for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-                int b, t0, nt, slice;
-                decode(item, b, t0, nt, slice);
-                if (w_resident && item != (int)blockIdx.x) break;
-                for (int kc = 0; kc < p.nkc; ++kc) {
-                    mbar_wait(&bempty[bst], bphase ^ 1);
-                    mbar_arrive_expect_tx(&bfull[bst], w_chunk);
-                    const uint8_t *src = q.wblob + W_HDR + ((size_t)slice * p.nkc + kc) * w_chunk;
-                    for (uint32_t off = 0; off < w_chunk; off += 36864) {
-                        const uint32_t n = min(36864u, w_chunk - off);
-                        asm volatile(
-                            "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                            ::"r"(smem_u32(sW + bst * w_chunk + off)), "l"(src + off), "r"(n), "r"(smem_u32(&bfull[bst]))
-                            : "memory");
-                    }
-                    if (++bst == NBST) { bst = 0; bphase ^= 1; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ================================ MMA issuer ========================================
-        // the whole warp walks the loop (uniform control flow, operands in uniform registers); one elected lane issues
-        {
-            // B = [W_hi | W_lo] stacked along N (2N rows per octet): an N = 64 MMA occupies the tensor
-            // pipe as long as an N = 128 one (A-operand fetch bound, ncu: pipe_tc 81 % vs math 40 %),
-            // so x_hi*[W_hi|W_lo] (N = 2N) + x_lo*W_hi (N) is 2 MMAs per K step instead of 3
-            const uint32_t idesc = umma_idesc_f16(128, 2 * p.N, 0);
-            const uint32_t idesc_lo = umma_idesc_f16(128, p.N, 0);
-            const uint32_t b_lbo = 2 * p.N * 16;             // next channel octet of the weights
-            int stage = 0, phase = 0, bst = 0, bphase = 0;
-            uint32_t tph = 0;                                  // per-accumulator phase bits
-            for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-                int b, t0, nt, slice;
-                decode(item, b, t0, nt, slice);
-                const bool first_item = item == (int)blockIdx.x;
-                for (int kc = 0; kc < p.nkc; ++kc) {
-                    if (!w_resident || first_item) {
-                        mbar_wait(&bfull[bst], bphase);
-                        tc_fence_after();
-                    }
-                    const uint32_t w_st = smem_u32(sW + bst * w_chunk);
-                    for (int t = 0; t < nt; ++t) {
-                        if (kc == 0) {
-                            mbar_wait(&tempty[t], ((tph >> t) & 1u) ^ 1u);
-                            tc_fence_after();
-                        }
-                        const uint32_t d = tmem_base + t * 2 * p.N;
-                        mbar_wait(&full[stage], phase);
-                        tc_fence_after();
-                        const uint32_t a_hi = smem_u32(sA + stage * A_STAGE);
-                        // descriptors of (tap 0, k-step 0); every other MMA is a constant offset away
-                        // descriptor words: low = start address (>> 4) | LBO << 16, high = SBO | version (constant)
-                        const uint32_t dah_lo = ((a_hi & 0x3FFFF) >> 4) | ((uint32_t)(A_OCT_B >> 4) << 16);
-                        const uint32_t dal_lo = (((a_hi + A_HALF) & 0x3FFFF) >> 4) | ((uint32_t)(A_OCT_B >> 4) << 16);
-                        const uint32_t da_hi = (uint32_t)(ROW_B >> 4) | (1u << 14);
-                        const uint32_t db_lo0 = ((w_st & 0x3FFFF) >> 4) | ((b_lbo >> 4) << 16);
-                        const uint32_t db_hi = (128u >> 4) | (1u << 14);
-                        // ONE elected thread issues the tile's 36 MMAs as straight-line code: inside `if (elect_one())` ptxas
-                        // emits plain UTCHMMAs with the constant operands (descriptor high words, idesc, accumulator) moved
-                        // to uniform registers once, instead of an elect + five R2UR moves in front of every MMA
-                        if (elect_one()) {
-                            const uint32_t b_row = (3 * KOCT * b_lbo) >> 4;
-#pragma unroll 1
-                            for (int dy = 0; dy < 3; ++dy) {
-                                const uint32_t ar = dy * ((A_C * 16) >> 4), br = db_lo0 + dy * b_row;
-#pragma unroll
-                                for (int dx = 0; dx < 3; ++dx) {
-#pragma unroll
-                                    for (int j = 0; j < KOCT / 2; ++j) {
-                                        const uint32_t ao = ar + ((dx * 16 + j * 2 * A_OCT_B) >> 4);
-                                        const uint32_t bo = ((dx * KOCT + j * 2) * b_lbo) >> 4;
-                                        // x_hi * [W_hi | W_lo]  (N = 2N)  +  x_lo * W_hi  (first N rows only)
-                                        umma_f16_1(d, dah_lo + ao, da_hi, br + bo, db_hi, idesc, (kc | dy | dx | j) != 0);
-                                        umma_f16_1(d, dal_lo + ao, da_hi, br + bo, db_hi, idesc_lo, 1);
-                                    }
-                                }
+                        for (int kc = 0; kc < p.nkc; ++kc) {
+                            const bool first = kc < p.nkc_a;
+                            const CUtensorMap *mh = first ? &tm_hi : &tm2_hi, *ml = first ? &tm_lo : &tm2_lo;
+                            const int oct0 = (first ? kc : kc - p.nkc_a) * KOCT;
+                            mbar_wait(&empty[stage], phase ^ 1);
+                            uint8_t *s = sA + stage * A_STAGE;
+                            if ((p.dbg & 2) && n_issued >= NST) {
+                                mbar_arrive(&full[stage]);                 // experiment: reuse stale tiles
+                            } else {
+                                mbar_arrive_expect_tx(&full[stage], A_STAGE);
+                                tma_load_4d(s, mh, &full[stage], (x0 - 1) * 8, y0 - 1, oct0, b);
+                                tma_load_4d(s + A_HALF, ml, &full[stage], (x0 - 1) * 8, y0 - 1, oct0, b);
                             }
-                            umma_commit(&empty[stage]);
-                            if (kc == p.nkc - 1) umma_commit(&tfull[t]);
+                            ++n_issued;
+                            if (++stage == NST) { stage = 0; phase ^= 1; }
                         }
-                        __syncwarp();
-                        if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
-                        if (kc == p.nkc - 1) tph ^= 1u << t;
                     }
-                    if (!w_resident) umma_commit_w(&bempty[bst]);
-                    if (++bst == NBST) { bst = 0; bphase ^= 1; }
                 }
-                if (w_resident) { bst = 0; }          // chunk kc always lives in slot kc
+            }
+        } else if (warp == 3) {
+            // ================================ weight producer ===================================
+            if (lane == 0) {
+                int bst = 0, bphase = 0;
+                for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+                    int b, t0, nt, slice;
+                    decode(item, b, t0, nt, slice);
+                    if (w_resident && item != (int)blockIdx.x) break;
+                    for (int kc = 0; kc < p.nkc; ++kc) {
+                        mbar_wait(&bempty[bst], bphase ^ 1);
+                        mbar_arrive_expect_tx(&bfull[bst], w_chunk);
+                        const uint8_t *src = q.wblob + W_HDR + ((size_t)slice * p.nkc + kc) * w_chunk;
+                        for (uint32_t off = 0; off < w_chunk; off += 36864) {
+                            const uint32_t n = min(36864u, w_chunk - off);
+                            asm volatile(
+                                "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                                ::"r"(smem_u32(sW + bst * w_chunk + off)), "l"(src + off), "r"(n), "r"(smem_u32(&bfull[bst]))
+                                : "memory");
+                        }
+                        if (++bst == NBST) { bst = 0; bphase ^= 1; }
+                    }
+                }
             }
         }
-    }
     } else {
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 208;");
-        // ================================ epilogue ==========================================
-        // 8 warps: warp w owns TMEM lane quarter (w & 3) = 32 output pixels, and the 32-column block
-        // c0 = 32 * ((w - 4) >> 2) of every accumulator.  (With 4 warps the serial per-thread chain
-        // TMEM load -> scale/act -> fp16 split -> store of 64 channels took longer than the tile's MMAs.)
-        const int e = (threadIdx.x - 128) & 127;            // pixel of the tile
-        const int quarter = warp & 3;
-        const int c0 = ((warp - 4) >> 2) * 32;
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+        // ================================ MMA + epilogue ====================================
+        const int wg = (warp >> 2) - 1;                      // consumer warpgroup: output rows [64 wg, 64 wg + 64)
+        const int wt = threadIdx.x & 127;
+        const int e = wg * 64 + (wt & 63);                   // epilogue: pixel of the tile ...
+        const int c0 = (wt >> 6) * 32;                       // ... and its 32-column block
         const float out_scale = ldexpf(1.f, -(p.sa_in + sw));
         const float res_scale = ldexpf(1.f, -p.sa_res);
         const float so = ldexpf(1.f, p.sa_out);
         const bool has1 = q.res_hi != nullptr;              // warp-uniform
         const bool fast = epilogue_fast_ok(q, p);           // specialised straight-line epilogue for full blocks
-        uint32_t tph = 0;
+        constexpr uint32_t b_lbo = 2 * N * 16;               // next channel octet of the weights
+        constexpr uint32_t a_row0 = 8 * ROW_B;               // the second warpgroup's rows start 8 pixel rows down
+        int stage = 0, phase = 0, bst = 0, bphase = 0;
         for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
             int b, t0, nt, slice;
             decode(item, b, t0, nt, slice);
-            const int o_base = slice * p.N;
+            const bool first_item = item == (int)blockIdx.x;
+            const int o_base = slice * N;
             asm volatile("bar.sync 1, 256;" ::: "memory");          // previous item's sbias readers are done
-            if (threadIdx.x - 128 < p.N) {
+            if (threadIdx.x - 128 < N) {
                 const float bv = (q.bias && o_base + (int)threadIdx.x - 128 < p.Cout) ? q.bias[o_base + threadIdx.x - 128] : 0.f;
                 sbias[threadIdx.x - 128] = bv;
                 sbias[UC_NMAX + threadIdx.x - 128] = bv * so;       // pre-scaled copy for the specialised epilogue
             }
             asm volatile("bar.sync 1, 256;" ::: "memory");
-            const bool full_blk = fast && c0 + 32 <= p.N && o_base + c0 + 32 <= p.Cout;
+            const bool full_blk = fast && c0 + 32 <= N && o_base + c0 + 32 <= p.Cout;
             for (int t = 0; t < nt; ++t) {
                 const int tt = t0 + t;
                 const int y = (tt / p.tiles_x) * T_R + e / T_C, x = (tt % p.tiles_x) * T_C + e % T_C;
                 const bool ok = y < p.H && x < p.W;
                 ResRegs ra;
-                if (has1 && c0 < p.N) {
-                    if (full_blk) {
-                        prefetch_residual_full(q.res_hi, q.res_lo, p, b, y, x, ok, o_base, c0, ra);
-                        // next tile's residual octets -> L2 now, so that its register prefetch (issued just before its
-                        // accumulator wait, which is short since the epilogue got lean) finds them on chip
-                        if (t + 1 < nt) {
-                            const int tn = tt + 1;
-                            const int yn = (tn / p.tiles_x) * T_R + e / T_C, xn = (tn % p.tiles_x) * T_C + e % T_C;
-                            if (yn < p.H && xn < p.W) {
-                                const size_t plane = (size_t)p.H * p.W * 8;
-                                const size_t off = ((size_t)b * p.C8out + (o_base + c0) / 8) * plane + ((size_t)yn * p.W + xn) * 8;
+                if (has1 && c0 < N) {
+                    if (full_blk) prefetch_residual_full(q.res_hi, q.res_lo, p, b, y, x, ok, o_base, c0, ra);
+                    else prefetch_residual(q.res_hi, q.res_lo, p, b, y, x, ok, o_base, c0, ra);
+                }
+                float acc[N];                                        // 64 x 2N: [x*W_hi | x*W_lo] partial sums
+                for (int kc = 0; kc < p.nkc; ++kc) {
+                    const int wslot = w_resident ? kc : bst;         // resident: chunk kc always lives in slot kc
+                    if (!w_resident || (first_item && t == 0)) mbar_wait(&bfull[wslot], w_resident ? 0 : bphase);
+                    mbar_wait(&full[stage], phase);
+                    const uint32_t a_hi = smem_u32(sA + stage * A_STAGE) + wg * a_row0;
+                    const uint64_t dah = wg_smem_desc(a_hi, A_OCT_B, ROW_B);
+                    const uint64_t dal = wg_smem_desc(a_hi + A_HALF, A_OCT_B, ROW_B);
+                    const uint64_t db = wg_smem_desc(smem_u32(sW + wslot * w_chunk), b_lbo, 128);
+                    wgmma_fence();
 #pragma unroll
-                                for (int o8 = 0; o8 < 4; ++o8) {
-                                    asm volatile("prefetch.global.L2 [%0];" ::"l"(q.res_hi + off + o8 * plane));
-                                    asm volatile("prefetch.global.L2 [%0];" ::"l"(q.res_lo + off + o8 * plane));
-                                }
-                            }
+                    for (int tap = 0; tap < 9; ++tap) {
+#pragma unroll
+                        for (int j = 0; j < KOCT / 2; ++j) {
+                            const uint32_t ao = (tap / 3) * ROW_B + (tap % 3) * 16 + j * 2 * A_OCT_B;
+                            const uint32_t bo = (tap * KOCT + j * 2) * b_lbo;
+                            Wgmma<2 * N>::mma(acc, wg_desc_advance(dah, ao), wg_desc_advance(db, bo), (kc | tap | j) != 0);
+                            Wgmma<N>::mma(acc, wg_desc_advance(dal, ao), wg_desc_advance(db, bo), 1);
                         }
-                    } else {
-                        prefetch_residual(q.res_hi, q.res_lo, p, b, y, x, ok, o_base, c0, ra);
+                    }
+                    wgmma_commit();
+                    wgmma_wait_all();
+                    mbar_arrive(&empty[stage]);
+                    if (++stage == NST) { stage = 0; phase ^= 1; }
+                    if (!w_resident) {
+                        mbar_arrive(&bempty[bst]);
+                        if (++bst == NBST) { bst = 0; bphase ^= 1; }
                     }
                 }
-                mbar_wait(&tfull[t], (tph >> t) & 1u);
-                tph ^= 1u << t;
-                tc_fence_after();
-                const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + t * 2 * p.N;
-                if (c0 < p.N) {
+                float v[N / 2];
+#pragma unroll
+                for (int i = 0; i < N / 2; ++i) v[i] = acc[i] + acc[i + N / 2];      // columns c and N + c
+                asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");          // previous tile's epilogue is done
+                acc_store(acc_s, wg * 64, v);
+                asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+                if (c0 < N) {
                     if (full_blk)
-                        epilogue_fast_dispatch<true>(q, p, taddr, c0, b, y, x, ok, o_base, sbias + UC_NMAX, out_scale * so,
-                                                     res_scale * so, has1 ? &ra : nullptr);
+                        epilogue_fast_dispatch(q, p, acc_s + e, c0, b, y, x, ok, o_base, sbias + UC_NMAX, out_scale * so,
+                                               res_scale * so, has1 ? &ra : nullptr);
                     else
-                        epilogue_store_block(q, p, taddr, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, so,
+                        epilogue_store_block(q, p, acc_s + e, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, so,
                                              has1 ? &ra : nullptr);
                 }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tempty[t]);
             }
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, tmem_cols);
-    }
-}
-
-
-// ------------------------------------------------------------------------------------------
-// CTA-pair version (cta_group::2, cluster of 2): the 1-CTA kernel above is bound by the tensor core's shared-memory
-// OPERAND FETCH, not by its math (14 KB per K step for 96 cycles of MMA; ncu: tensor pipe 56 % active).  A pair of
-// CTAs issues ONE M = 256 MMA: each CTA feeds its own 128-pixel A tile and only HALF of the B (weight) rows from
-// its own shared memory, so the fetch per CTA and K step drops to 4 + 2 (x_hi * [W_hi|W_lo]) + 4 + 1 (x_lo * W_hi)
-// = 11 KB.  Per-CTA weight rows of one (tap, octet): [0, N) = W_hi (rank 0) / W_lo (rank 1)   -> MMA 1, N_mma = 2N
-//                                                    [N, 1.5N) = W_hi rows [rank*N/2, +N/2)   -> MMA 2, N_mma = N
-// (same offsets in both CTAs, as the instruction requires).  Accumulator layout per CTA is unchanged (128 lanes x
-// 2N stacked columns), so the epilogue is shared with the 1-CTA kernel.
-// Synchronisation: everything the leader's MMA thread waits for lives in the LEADER: full[] / bfull[] have count 2
-// (local TMA + a forwarded arrive from the peer, whose idle MMA warp waits on its local barrier and arrives remotely),
-// tempty[] has count 16 (8 local + 8 remote epilogue warps).  What the MMA thread signals (empty[], bempty[],
-// tfull[]) is committed with .multicast::cluster to the barrier at the same offset in both CTAs.
-// ------------------------------------------------------------------------------------------
-constexpr int NSTAGE2 = 4;
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(384, 1)
-conv3x3_umma2_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo,
-                     const __grid_constant__ CUtensorMap tm2_hi, const __grid_constant__ CUtensorMap tm2_lo,
-                     const ConvPtrs q, const ConvParams p) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    const uint32_t w_rows = p.N + p.N / 2;
-    const uint32_t w_chunk = 9u * KOCT * w_rows * 16;                     // bytes of one chunk in THIS CTA
-    uint8_t *sW = smem;                                                  // [NBST][w_chunk]
-    uint8_t *sA = smem + NBST * w_chunk;                                 // w_chunk is a multiple of 128
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sA + NSTAGE2 * A_STAGE);
-    uint64_t *full = bars, *empty = full + NSTAGE2, *bfull = empty + NSTAGE2, *bempty = bfull + NBST,
-             *tfull = bempty + NBST, *tempty = tfull + MAXT;
-    uint32_t *tmem_base_p = reinterpret_cast<uint32_t *>(tempty + MAXT);
-    float *sbias = reinterpret_cast<float *>(tmem_base_p + 4);           // [N], 16 B aligned (float4 reads)
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const bool leader = rank == 0;
-    const int tiles_img = p.tiles_x * p.tiles_y;
-    const int n_items = p.B * p.n_st * p.nslice;          // pair items; n_st = ceil(tiles_img / (2 T))
-    const int pair = blockIdx.x >> 1, n_pairs = gridDim.x >> 1;
-    const uint32_t need_cols = 2u * p.N * p.T;
-    const uint32_t tmem_cols = need_cols <= 32 ? 32 : need_cols <= 64 ? 64 : need_cols <= 128 ? 128
-                               : need_cols <= 256 ? 256 : 512;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&tm_hi);
-        tma_prefetch_desc(&tm_lo);
-        tma_prefetch_desc(&tm2_hi);
-        tma_prefetch_desc(&tm2_lo);
-    }
-    if (warp == 1 && lane == 0) {
-        for (int i = 0; i < NSTAGE2; ++i) { mbar_init(&full[i], leader ? 2 : 1); mbar_init(&empty[i], 1); }
-        for (int i = 0; i < NBST; ++i) { mbar_init(&bfull[i], leader ? 2 : 1); mbar_init(&bempty[i], 1); }
-        for (int i = 0; i < MAXT; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], 16); }
-        fence_mbar_init();
-    }
-    if (warp == 2) {
-        tmem_alloc2(tmem_base_p, tmem_cols);
-        tmem_relinquish2();
-    }
-    tc_fence_before();
-    cluster_sync_all();                                    // both CTAs' barriers exist before anyone signals remotely
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_base_p;
-    const int sw = *reinterpret_cast<const int *>(q.wblob);              // weight scale exponent
-    const bool w_resident = p.nslice == 1 && p.nkc <= NBST;
-
-    // pair item -> (b, first tile, tiles per CTA, slice); CTA `rank` takes tiles t0 + 2 t + rank (a tile index
-    // beyond the image is a dummy: its TMA box is entirely out of bounds = zeros, its epilogue stores nothing)
-    auto decode = [&](int item, int &b, int &t0, int &nt, int &slice) {
-        slice = item % p.nslice;
-        const int r = item / p.nslice;
-        const int st = r % p.n_st;
-        b = r / p.n_st;
-        t0 = st * 2 * p.T;
-        nt = min(p.T, (tiles_img - t0 + 1) / 2);
-    };
-
-    if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 88;");
-    if (warp == 0) {
-        // ================================ activation producer ===============================
-        if (lane == 0) {
-            int stage = 0, phase = 0;
-            for (int item = pair; item < n_items; item += n_pairs) {
-                int b, t0, nt, slice;
-                decode(item, b, t0, nt, slice);
-                for (int kc = 0; kc < p.nkc; ++kc) {
-                    const bool first = kc < p.nkc_a;
-                    const CUtensorMap *mh = first ? &tm_hi : &tm2_hi, *ml = first ? &tm_lo : &tm2_lo;
-                    const int oct0 = (first ? kc : kc - p.nkc_a) * KOCT;
-                    for (int t = 0; t < nt; ++t) {
-                        const int tt = t0 + 2 * t + (int)rank;
-                        const int y0 = tt < tiles_img ? (tt / p.tiles_x) * T_R : p.H + T_R, x0 = (tt % p.tiles_x) * T_C;
-                        mbar_wait(&empty[stage], phase ^ 1);
-                        uint8_t *s = sA + stage * A_STAGE;
-                        mbar_arrive_expect_tx(&full[stage], A_STAGE);
-                        tma_load_4d(s, mh, &full[stage], (x0 - 1) * 8, y0 - 1, oct0, b);
-                        tma_load_4d(s + A_HALF, ml, &full[stage], (x0 - 1) * 8, y0 - 1, oct0, b);
-                        if (++stage == NSTAGE2) { stage = 0; phase ^= 1; }
-                    }
-                }
-            }
-        }
-    } else if (warp == 3) {
-        // ================================ weight producer ===================================
-        if (lane == 0) {
-            int bst = 0, bphase = 0;
-            for (int item = pair; item < n_items; item += n_pairs) {
-                int b, t0, nt, slice;
-                decode(item, b, t0, nt, slice);
-                if (w_resident && item != pair) break;
-                for (int kc = 0; kc < p.nkc; ++kc) {
-                    mbar_wait(&bempty[bst], bphase ^ 1);
-                    mbar_arrive_expect_tx(&bfull[bst], w_chunk);
-                    const uint8_t *src = q.wblob + p.w2_off + (((size_t)slice * p.nkc + kc) * 2 + rank) * w_chunk;
-                    for (uint32_t off = 0; off < w_chunk; off += 27648) {
-                        const uint32_t n = min(27648u, w_chunk - off);
-                        asm volatile(
-                            "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                            ::"r"(smem_u32(sW + bst * w_chunk + off)), "l"(src + off), "r"(n), "r"(smem_u32(&bfull[bst]))
-                            : "memory");
-                    }
-                    if (++bst == NBST) { bst = 0; bphase ^= 1; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (leader) {
-            // ================================ MMA issuer (leader CTA) ==========================
-            // whole warp, uniform control flow; one elected lane issues (see umma_f16_w).
-            // Two tiles are in flight at once and their MMAs alternate: consecutive MMAs into the SAME accumulator
-            // serialise on the accumulate dependency (ncu: tensor pipe 57 % active with 64-cycle MMAs, shared-memory
-            // banks 34 %, issue slots idle), so the instruction stream interleaves two independent accumulators.
-            const uint32_t idesc = umma_idesc_f16(256, 2 * p.N, 0);
-            const uint32_t idesc_lo = umma_idesc_f16(256, p.N, 0);
-            const uint32_t b_lbo = w_rows * 16;              // next channel octet of the weights
-            const uint32_t da_hi = (uint32_t)(ROW_B >> 4) | (1u << 14);
-            const uint32_t db_hi = (128u >> 4) | (1u << 14);
-            int stage = 0, phase = 0, bst = 0, bphase = 0;
-            uint32_t tph = 0;
-            for (int item = pair; item < n_items; item += n_pairs) {
-                int b, t0, nt, slice;
-                decode(item, b, t0, nt, slice);
-                const bool first_item = item == pair;
-                for (int kc = 0; kc < p.nkc; ++kc) {
-                    if (!w_resident || first_item) {
-                        mbar_wait(&bfull[bst], bphase);
-                        tc_fence_after();
-                    }
-                    const uint32_t w_st = smem_u32(sW + bst * w_chunk);
-                    const uint32_t db_lo0 = ((w_st & 0x3FFFF) >> 4) | ((b_lbo >> 4) << 16);              // rows [0, N): MMA 1
-                    const uint32_t db_lo1 = (((w_st + p.N * 16) & 0x3FFFF) >> 4) | ((b_lbo >> 4) << 16);   // rows [N, 1.5 N): MMA 2
-                    for (int t = 0; t < nt; t += 2) {
-                        const bool two = t + 1 < nt;
-                        int stage1 = stage + 1, phase1 = phase;
-                        if (stage1 == NSTAGE2) { stage1 = 0; phase1 ^= 1; }
-                        if (kc == 0) {
-                            mbar_wait(&tempty[t], ((tph >> t) & 1u) ^ 1u);
-                            if (two) mbar_wait(&tempty[t + 1], ((tph >> (t + 1)) & 1u) ^ 1u);
-                            tc_fence_after();
-                        }
-                        const uint32_t d0 = tmem_base + t * 2 * p.N, d1 = d0 + 2 * p.N;
-                        mbar_wait(&full[stage], phase);
-                        if (two) mbar_wait(&full[stage1], phase1);
-                        tc_fence_after();
-                        const uint32_t a0 = smem_u32(sA + stage * A_STAGE), a1 = smem_u32(sA + stage1 * A_STAGE);
-                        const uint32_t ah0 = ((a0 & 0x3FFFF) >> 4) | ((uint32_t)(A_OCT_B >> 4) << 16);
-                        const uint32_t al0 = (((a0 + A_HALF) & 0x3FFFF) >> 4) | ((uint32_t)(A_OCT_B >> 4) << 16);
-                        const uint32_t ah1 = ((a1 & 0x3FFFF) >> 4) | ((uint32_t)(A_OCT_B >> 4) << 16);
-                        const uint32_t al1 = (((a1 + A_HALF) & 0x3FFFF) >> 4) | ((uint32_t)(A_OCT_B >> 4) << 16);
-                        if (two) {
-#pragma unroll
-                            for (int tap = 0; tap < 9; ++tap) {
-#pragma unroll
-                                for (int j = 0; j < KOCT / 2; ++j) {
-                                    const uint32_t ao = (((tap / 3) * A_C + tap % 3) * 16 + j * 2 * A_OCT_B) >> 4;
-                                    const uint32_t bo = ((tap * KOCT + j * 2) * b_lbo) >> 4;
-                                    const uint32_t acc = (kc | tap | j) != 0;
-                                    umma2_f16_w(d0, ah0 + ao, da_hi, db_lo0 + bo, db_hi, idesc, acc);
-                                    umma2_f16_w(d1, ah1 + ao, da_hi, db_lo0 + bo, db_hi, idesc, acc);
-                                    umma2_f16_w(d0, al0 + ao, da_hi, db_lo1 + bo, db_hi, idesc_lo, 1);
-                                    umma2_f16_w(d1, al1 + ao, da_hi, db_lo1 + bo, db_hi, idesc_lo, 1);
-                                }
-                            }
-                        } else {
-#pragma unroll
-                            for (int tap = 0; tap < 9; ++tap) {
-#pragma unroll
-                                for (int j = 0; j < KOCT / 2; ++j) {
-                                    const uint32_t ao = (((tap / 3) * A_C + tap % 3) * 16 + j * 2 * A_OCT_B) >> 4;
-                                    const uint32_t bo = ((tap * KOCT + j * 2) * b_lbo) >> 4;
-                                    umma2_f16_w(d0, ah0 + ao, da_hi, db_lo0 + bo, db_hi, idesc, (kc | tap | j) != 0);
-                                    umma2_f16_w(d0, al0 + ao, da_hi, db_lo1 + bo, db_hi, idesc_lo, 1);
-                                }
-                            }
-                        }
-                        umma_commit2_w(&empty[stage]);
-                        if (two) umma_commit2_w(&empty[stage1]);
-                        if (kc == p.nkc - 1) {
-                            umma_commit2_w(&tfull[t]);
-                            tph ^= 1u << t;
-                            if (two) { umma_commit2_w(&tfull[t + 1]); tph ^= 1u << (t + 1); }
-                        }
-                        if (two) { stage = stage1; phase = phase1; }
-                        if (++stage == NSTAGE2) { stage = 0; phase ^= 1; }
-                    }
-                    if (!w_resident) umma_commit2_w(&bempty[bst]);
-                    if (++bst == NBST) { bst = 0; bphase ^= 1; }
-                }
-                if (w_resident) { bst = 0; }
-            }
-        } else if (lane == 0) {
-            // ================================ forwarder (peer CTA) =============================
-            // same walk as the issuer: when this CTA's weights / activation stage have landed, tell the leader
-            int stage = 0, phase = 0, bst = 0, bphase = 0;
-            for (int item = pair; item < n_items; item += n_pairs) {
-                int b, t0, nt, slice;
-                decode(item, b, t0, nt, slice);
-                const bool first_item = item == pair;
-                for (int kc = 0; kc < p.nkc; ++kc) {
-                    if (!w_resident || first_item) {
-                        mbar_wait(&bfull[bst], bphase);
-                        mbar_arrive_remote(mapa_u32(smem_u32(&bfull[bst]), 0));
-                    }
-                    for (int t = 0; t < nt; ++t) {
-                        mbar_wait(&full[stage], phase);
-                        mbar_arrive_remote(mapa_u32(smem_u32(&full[stage]), 0));
-                        if (++stage == NSTAGE2) { stage = 0; phase ^= 1; }
-                    }
-                    if (++bst == NBST) { bst = 0; bphase ^= 1; }
-                }
-                if (w_resident) { bst = 0; }
-            }
-        }
-    }
-    } else {
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 208;");
-        // ================================ epilogue ==========================================
-        const int e = (threadIdx.x - 128) & 127;            // pixel of the tile
-        const int quarter = warp & 3;
-        const int c0 = ((warp - 4) >> 2) * 32;
-        const float out_scale = ldexpf(1.f, -(p.sa_in + sw));
-        const float res_scale = ldexpf(1.f, -p.sa_res);
-        const float so = ldexpf(1.f, p.sa_out);
-        const bool has1 = q.res_hi != nullptr;              // warp-uniform
-        const bool fast = epilogue_fast_ok(q, p);           // specialised straight-line epilogue for full blocks
-        uint32_t tph = 0;
-        for (int item = pair; item < n_items; item += n_pairs) {
-            int b, t0, nt, slice;
-            decode(item, b, t0, nt, slice);
-            const int o_base = slice * p.N;
-            asm volatile("bar.sync 1, 256;" ::: "memory");          // previous item's sbias readers are done
-            if (threadIdx.x - 128 < p.N) {
-                const float bv = (q.bias && o_base + (int)threadIdx.x - 128 < p.Cout) ? q.bias[o_base + threadIdx.x - 128] : 0.f;
-                sbias[threadIdx.x - 128] = bv;
-                sbias[UC_NMAX + threadIdx.x - 128] = bv * so;       // pre-scaled copy for the specialised epilogue
-            }
-            asm volatile("bar.sync 1, 256;" ::: "memory");
-            for (int t = 0; t < nt; ++t) {
-                const int tt = t0 + 2 * t + (int)rank;
-                const int y = (tt / p.tiles_x) * T_R + e / T_C, x = (tt % p.tiles_x) * T_C + e % T_C;
-                const bool ok = tt < tiles_img && y < p.H && x < p.W;
-                ResRegs ra;
-                if (has1 && c0 < p.N) {
-                    if (fast && c0 + 32 <= p.N && o_base + c0 + 32 <= p.Cout)
-                        prefetch_residual_full(q.res_hi, q.res_lo, p, b, y, x, ok, o_base, c0, ra);
-                    else
-                        prefetch_residual(q.res_hi, q.res_lo, p, b, y, x, ok, o_base, c0, ra);
-                }
-                mbar_wait(&tfull[t], (tph >> t) & 1u);
-                tph ^= 1u << t;
-                tc_fence_after();
-                const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + t * 2 * p.N;
-                if (c0 < p.N) {
-                    if (fast && c0 + 32 <= p.N && o_base + c0 + 32 <= p.Cout)
-                        epilogue_fast_dispatch<true>(q, p, taddr, c0, b, y, x, ok, o_base, sbias + UC_NMAX, out_scale * so,
-                                                     res_scale * so, has1 ? &ra : nullptr);
-                    else
-                        epilogue_store_block(q, p, taddr, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, so,
-                                             has1 ? &ra : nullptr);
-                }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) {
-                    if (leader) mbar_arrive(&tempty[t]);
-                    else mbar_arrive_remote(mapa_u32(smem_u32(&tempty[t]), 0));
-                }
-            }
-        }
-    }
-
-    tc_fence_before();
-    cluster_sync_all();                                    // nobody leaves while the pair's barriers / TMEM are in use
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc2(tmem_base, tmem_cols);
     }
 }
 
@@ -688,7 +312,7 @@ __global__ void psa_interleave_kernel(const uint4 *__restrict__ hi, const uint4 
     }
 }
 
-// 2x2 / stride 2 max-pool on a PSA tensor (VGG pool1/pool2 between tcgen05 convolutions): the
+// 2x2 / stride 2 max-pool on a PSA tensor (VGG pool1/pool2 between tensor-core convolutions): the
 // pooled map stays in the operand layout, no fp32 round trip through HBM.  max(hi+lo) is taken on
 // the reconstructed fp32 values and re-split (the re-split of an already-split value is exact).
 __global__ void psa_maxpool2_kernel(const __half *__restrict__ hi, const __half *__restrict__ lo, int C8, int H, int W,
@@ -768,33 +392,6 @@ __global__ void wpack_kernel(const float *__restrict__ w, int Cin, int Cout, int
     }
 }
 
-// CTA-pair layout (after the 1-CTA layout in the same blob): [slice][kc][rank][tap][octet][1.5 N rows][8] fp16,
-// rows [0, N) = W_hi (rank 0) / W_lo (rank 1) of the slice's couts, rows [N, 1.5 N) = W_hi of couts [rank * N/2, +N/2)
-__global__ void wpack2_kernel(const float *__restrict__ w, int Cin, int Cout, int N, int nkc, int nslice,
-                              const uint8_t *__restrict__ blob_hdr, __half *__restrict__ dst) {
-    const float S = ldexpf(1.f, *reinterpret_cast<const int *>(blob_hdr));      // written by wpack_kernel (same stream)
-    const int R = N + N / 2;
-    const long long total = (long long)nslice * nkc * 2 * 9 * KOCT * R * 8;
-    for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
-        const int j = (int)(e & 7);
-        long long rest = e >> 3;
-        const int row = (int)(rest % R); rest /= R;
-        const int oct = (int)(rest % KOCT); rest /= KOCT;
-        const int tap = (int)(rest % 9); rest /= 9;
-        const int rank = (int)(rest % 2); rest /= 2;
-        const int kc = (int)(rest % nkc);
-        const int slice = (int)(rest / nkc);
-        const int c = (kc * KOCT + oct) * 8 + j;
-        const int ol = row < N ? row : rank * (N / 2) + (row - N);
-        const int lo = row < N ? rank : 0;
-        const int o = slice * NMAX + ol;
-        float v = 0.f;
-        if (c < Cin && o < Cout) v = w[((size_t)o * Cin + c) * 9 + tap] * S;
-        const __half hh = __float2half_rn(v);
-        dst[e] = lo ? __float2half_rn(v - __half2float(hh)) : hh;
-    }
-}
-
 // ------------------------------------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
                                   const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
@@ -833,14 +430,10 @@ static inline int n_slice(int cout) { return cout <= NMAX ? 1 : (cout + NMAX - 1
 using namespace c2m;
 
 static inline size_t layout1_bytes(int Cin, int Cout) { return (size_t)n_slice(Cout) * n_kc(Cin) * 2 * 9 * KOCT * slice_n(Cout) * 16; }
-static inline size_t layout2_bytes(int Cin, int Cout) {
-    const int N = slice_n(Cout);
-    return (size_t)n_slice(Cout) * n_kc(Cin) * 2 * 9 * KOCT * (N + N / 2) * 16;
-}
 
 extern "C" size_t c2m_conv3x3_packed_weight_bytes(int Cin, int Cout) {
     if (Cin <= 0 || Cout <= 0) return 0;
-    return (size_t)W_HDR + layout1_bytes(Cin, Cout) + layout2_bytes(Cin, Cout);       // 1-CTA layout + CTA-pair layout
+    return (size_t)W_HDR + layout1_bytes(Cin, Cout);
 }
 
 extern "C" int c2m_conv3x3_pack_weights_f32(const float *w, int Cin, int Cout, void *packed, c2m_stream_t stream) {
@@ -856,9 +449,6 @@ extern "C" int c2m_conv3x3_pack_weights_f32(const float *w, int Cin, int Cout, v
     const int blocks = (int)((total + 255) / 256 > 592 ? 592 : (total + 255) / 256);
     wpack_kernel<<<blocks, 256, 0, st>>>(w, Cin, Cout, N, nkc, ns, reinterpret_cast<uint8_t *>(packed));
     C2M_LAUNCH_CHECK("wpack_kernel");
-    wpack2_kernel<<<blocks, 256, 0, st>>>(w, Cin, Cout, N, nkc, ns, reinterpret_cast<const uint8_t *>(packed),
-                                          reinterpret_cast<__half *>(reinterpret_cast<uint8_t *>(packed) + W_HDR + layout1_bytes(Cin, Cout)));
-    C2M_LAUNCH_CHECK("wpack2_kernel");
     return C2M_OK;
 }
 
@@ -896,7 +486,7 @@ extern "C" int c2m_psa_interleave(const void *hi, const void *lo, int B, int C, 
                   (reinterpret_cast<uintptr_t>(out) & 31) == 0, "psa_interleave: planes must be 16 B, the output 32 B aligned");
     const long long n = (long long)B * ((C + 7) / 8) * H * W;
     int bx = (int)((n + 255) / 256);
-    if (bx > 148 * 16) bx = 148 * 16;
+    if (bx > 4096) bx = 4096;
     psa_interleave_kernel<<<bx, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
         reinterpret_cast<const uint4 *>(hi), reinterpret_cast<const uint4 *>(lo), n, reinterpret_cast<uint4 *>(out));
     C2M_LAUNCH_CHECK("psa_interleave_kernel");
@@ -941,14 +531,18 @@ extern "C" int c2m_conv3x3(const c2m_conv3x3_args *a, c2m_stream_t stream) {
     if (a->Cin2) p.nkc_a = a->Cin / (KOCT * 8);
     p.Cout = a->Cout; p.N = slice_n(a->Cout); p.nslice = n_slice(a->Cout);
     p.tiles_x = ceil_div(a->W, T_C); p.tiles_y = ceil_div(a->H, T_R);
-    p.T = 512 / (2 * p.N) < MAXT ? 512 / (2 * p.N) : MAXT;
-    // small problems (e.g. 64->64 on 160x160 maps = 200 items of 4 tiles for 148 SMs): halve the item size
-    if (p.T > 2 && (long long)a->B * p.tiles_x * p.tiles_y * p.nslice / p.T < 3 * 148) p.T = 2;
+    int dev = 0, sms = 0;
+    C2M_CUDA(cudaGetDevice(&dev));
+    C2M_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    p.T = MAXT;
+    // small problems (e.g. 64->64 on 160x160 maps): fewer tiles per item so that every SM gets several items
+    if ((long long)a->B * p.tiles_x * p.tiles_y * p.nslice / p.T < 3 * sms) p.T = 2;
+    // weights that do not stay resident are streamed per (item, K chunk): one tile per item
+    if (!(p.nslice == 1 && p.nkc <= NBST)) p.T = 1;
     if (const char *ev = getenv("C2M_CONV_T")) {          // tuning knob: tiles per work item
         const int t = atoi(ev);
         if (t >= 1 && t < p.T) p.T = t;
     }
-    p.stacked = 1;
     p.dbg = 0;
     p.cs = 0;
     if (const char *ev = getenv("C2M_CONV_DBG")) p.dbg = atoi(ev);
@@ -980,50 +574,25 @@ extern "C" int c2m_conv3x3(const c2m_conv3x3_args *a, c2m_stream_t stream) {
     } else {
         m2h = mh; m2l = ml;
     }
-    int dev = 0, sms = 0;
-    C2M_CUDA(cudaGetDevice(&dev));
-    C2M_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    p.w2_off = (unsigned)(W_HDR + layout1_bytes((int)(a->Cin + a->Cin2), a->Cout));
-    // CTA pairs (cta_group::2): implemented and parity-tested, but measured SLOWER than the 1-CTA kernel on every
-    // shape of the network (profiles/r02_conv_epilogue_bound.md: the kernel was epilogue-bound, not operand-fetch
-    // bound) — off by default, C2M_CONV_2CTA=1 selects it for experiments.
-    bool use2 = false;
-    if (const char *ev = getenv("C2M_CONV_2CTA")) use2 = atoi(ev) != 0;
-    if (use2) {
-        const int tiles_img = p.tiles_x * p.tiles_y;
-        p.T = 512 / (2 * p.N) < MAXT ? 512 / (2 * p.N) : MAXT;
-        // small problems: fewer tiles per pair item so that every pair of SMs gets several items
-        while (p.T > 1 && (long long)a->B * ceil_div(tiles_img, 2 * p.T) * p.nslice < 3 * (sms / 2)) p.T /= 2;
-        if (const char *ev = getenv("C2M_CONV_T")) {
-            const int t = atoi(ev);
-            if (t >= 1 && t < p.T) p.T = t;
-        }
-        p.n_st = ceil_div(tiles_img, 2 * p.T);
-        const int n_pair_items = a->B * p.n_st * p.nslice;
-        const int pairs = n_pair_items < sms / 2 ? n_pair_items : sms / 2;
-        const size_t smem2 = (size_t)NBST * 9 * KOCT * (p.N + p.N / 2) * 16 + NSTAGE2 * A_STAGE + 4096;
-        C2M_CUDA(cudaFuncSetAttribute(conv3x3_umma2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
-        const double cin_t2 = (double)a->Cin + a->Cin2, px2 = (double)a->B * a->H * a->W;
-        const double flops2 = 2.0 * cin_t2 * a->Cout * 9.0 * px2;
-        const double bytes2 = 4.0 * px2 * (cin_t2 + a->Cout * ((a->out_hi ? 1 : 0) + (a->out_f32 ? 1 : 0)) +
-                                           a->Cout * ((a->res_hi ? 1 : 0) + (a->res2_hi ? 1 : 0) + (a->add_f32 ? 1 : 0)));
-        void *ph2 = prof_begin(PROF_CONV3X3, flops2, bytes2, st);
-        conv3x3_umma2_kernel<<<2 * pairs, 384, smem2, st>>>(mh, ml, m2h, m2l, q, p);
-        C2M_LAUNCH_CHECK("conv3x3_umma2_kernel");
-        prof_end(ph2, st);
-        return C2M_OK;
-    }
-    const size_t smem = (size_t)NBST * 2 * 9 * KOCT * p.N * 16 + NSTAGE * A_STAGE + 4096;
-    C2M_CUDA(cudaFuncSetAttribute(conv3x3_umma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    C2M_CUDA(cudaFuncSetAttribute(conv3x3_wgmma_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)conv_smem_bytes(16)));
+    C2M_CUDA(cudaFuncSetAttribute(conv3x3_wgmma_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)conv_smem_bytes(32)));
+    C2M_CUDA(cudaFuncSetAttribute(conv3x3_wgmma_kernel<48>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)conv_smem_bytes(48)));
+    C2M_CUDA(cudaFuncSetAttribute(conv3x3_wgmma_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)conv_smem_bytes(64)));
     const int n_items = a->B * p.n_st * p.nslice;
     // algorithmic work: 2*Cin*Cout*9 flops per output pixel; bytes = PSA in (4 B/elem) + out
     const double cin_t = (double)a->Cin + a->Cin2, px = (double)a->B * a->H * a->W;
     const double flops = 2.0 * cin_t * a->Cout * 9.0 * px;
     const double bytes = 4.0 * px * (cin_t + a->Cout * ((a->out_hi ? 1 : 0) + (a->out_f32 ? 1 : 0)) +
                                      a->Cout * ((a->res_hi ? 1 : 0) + (a->res2_hi ? 1 : 0) + (a->add_f32 ? 1 : 0)));
+    const int grid = n_items < sms ? n_items : sms;
     void *ph = prof_begin(PROF_CONV3X3, flops, bytes, st);
-    conv3x3_umma_kernel<<<n_items < sms ? n_items : sms, 384, smem, st>>>(mh, ml, m2h, m2l, q, p);
-    C2M_LAUNCH_CHECK("conv3x3_umma_kernel");
+    switch (p.N) {
+    case 16: conv3x3_wgmma_kernel<16><<<grid, 384, conv_smem_bytes(16), st>>>(mh, ml, m2h, m2l, q, p); break;
+    case 32: conv3x3_wgmma_kernel<32><<<grid, 384, conv_smem_bytes(32), st>>>(mh, ml, m2h, m2l, q, p); break;
+    case 48: conv3x3_wgmma_kernel<48><<<grid, 384, conv_smem_bytes(48), st>>>(mh, ml, m2h, m2l, q, p); break;
+    default: conv3x3_wgmma_kernel<64><<<grid, 384, conv_smem_bytes(64), st>>>(mh, ml, m2h, m2l, q, p); break;
+    }
+    C2M_LAUNCH_CHECK("conv3x3_wgmma_kernel");
     prof_end(ph, st);
     return C2M_OK;
 }

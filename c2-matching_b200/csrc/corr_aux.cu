@@ -172,7 +172,7 @@ int corr_rinv_launch(const CorrGeom &g, const CorrWorkspace &ws, int is_norm, cu
 // Generic candidate search on CUDA cores (fp32 FFMA): any patch size, strides, channel count.
 // Block = 64 queries x (all Ref patches of one chunk), 64x64 score tiles, 4x4 per thread,
 // K streamed 8 channels of one tap at a time.  Emits the same Candidate partials as the
-// tcgen05 search; the final answer always comes from the rescoring pass.
+// tensor-core search; the final answer always comes from the rescoring pass.
 // ------------------------------------------------------------------------------------------
 constexpr int GS_T = 64;
 

@@ -6,11 +6,11 @@
 //   hi,lo [B][Cp/8][HW][8]   fp16 split operands of x * 2^sexp:  hi = rn(x*S), lo = rn(x*S - hi).
 //                            One 16-byte element per (channel-octet, pixel): a (W*8)-wide row of
 //                            one image row is contiguous, so a TMA box of (cols*8, rows, octets)
-//                            lands in shared memory as [octet][pixel][8 halfs] = the tcgen05
+//                            lands in shared memory as [octet][pixel][8 halfs] = the wgmma
 //                            K-major no-swizzle core-matrix layout with rows 16 B apart.
 //   ss    [B][HW]            fp32 per-pixel sum of squares of p32 (for the patch norms).
 //   rinv  [B][NR]            fp32 1 / (sqrt(sum_{patch} ss) + 1e-5)   (1 when !is_norm)
-//   part  [B][nchunk][NQ]    Candidate: approximate top-8 (tcgen05) / top-4 (FFMA) of each query over one Ref chunk (nchunk <= 32).
+//   part  [B][nchunk][NQ]    Candidate: approximate top-8 (tensor cores) / top-4 (FFMA) of each query over one Ref chunk (nchunk <= 32).
 //   ovf   [B*NQ]             (query, chunk bit mask) of the (query, chunk) pairs whose top-2 list may be incomplete:
 //                            the exhaustive pass re-scans those chunks exactly (see corr_aux.cu).
 #pragma once
@@ -18,7 +18,7 @@
 
 namespace c2m {
 
-constexpr int CORR_TOPK = 8;      // candidate slots per (query, Ref chunk): the tcgen05 search fills all of them (its window is
+constexpr int CORR_TOPK = 8;      // candidate slots per (query, Ref chunk): the tensor-core search fills all of them (its window is
                                   // 2^-10-wide because the Ref operand is a plain fp16 rounding), the FFMA search GEN_TOPK
 constexpr int GEN_TOPK = 4;
 struct __align__(16) Candidate {

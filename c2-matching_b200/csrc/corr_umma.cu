@@ -1,4 +1,4 @@
-// Fused all-pairs patch correlation + running top-2 on the sm_100a tensor cores.
+// Fused all-pairs patch correlation + running top-k on the sm_90a tensor cores (wgmma).
 //
 // Replaces the reference's chunked `F.conv2d(feat_in, ref_patches)` + `max`
 // (mmsr/models/archs/ref_map_util.py:54-76), which materialises a [n_ref, h', w'] score tensor
@@ -10,23 +10,23 @@
 //     score(q, r) = V(q, r) + V(q+(0,1), r+(0,1)) + V(q+(0,2), r+(0,2))        3-term diagonal sum
 // Pixel blocks are 16 columns wide on both sides (14 patch origins + 2 halo columns), stored by ONE TMA box per
 // operand half as [octet][row][16 px][8 halfs]: 16 px x 16 B = 256 B rows are contiguous, so M index m = 16*row + x
-// (query block: 8 rows -> M = 128) and N index n = 16*row + x (Ref block: 16 rows -> N = 256) are CONTIGUOUS pixel
-// runs in the tcgen05 K-major no-swizzle layout (8-pixel core-matrix groups 128 B apart = SBO, channel octets
+// (query block: 8 rows -> M = 128) and N index n = 16*row + x (Ref block: 8 rows -> N = 128) are CONTIGUOUS pixel
+// runs in the wgmma K-major no-swizzle layout (8-pixel core-matrix groups 128 B apart = SBO, channel octets
 // one block apart = LBO), and the row tap dy is a +256 B start-address offset on both descriptors.
-// In the accumulator, lane m+dx / column n+dx hold V(q+(0,dx), r+(0,dx)): a warp's 32 lanes are exactly two
-// 16-px block rows, so the diagonal sum is two __shfl_down per score — no shared memory, no extra TMEM traffic.
+// In the staged accumulator, row m+dx / column n+dx hold V(q+(0,dx), r+(0,dx)); the epilogue runs one thread per
+// row, so a warp's 32 threads are exactly two 16-px block rows and the diagonal sum is two __shfl_down per score.
 // Tile efficiency (14/16)^2 = 0.77, i.e. 2.3x fewer MMA cycles per score than issuing all nine taps.
 //
 // Precision.  Operands are split fp16 pairs of x*2^sexp (hi + lo, 22 mantissa bits); each K step
-// issues hi*hi + hi*lo + lo*hi into the same fp32 TMEM accumulator (M=128, N=256).  The scores
-// only RANK candidates: the epilogue keeps a top-4 per (query, Ref chunk) and the exact rescoring kernel
+// issues q_hi*r_hi + q_lo*r_hi into the same fp32 accumulator (M=128, N=128).  The scores
+// only RANK candidates: the epilogue keeps a top-8 per (query, Ref chunk) and the exact rescoring kernel
 // (corr_aux.cu) decides, so tensor-core rounding cannot leak into the index map; corr_aux.cu states the error
-// bound that sizes the rescoring window and the exhaustive fallback that makes the top-4 lists sufficient.
+// bound that sizes the rescoring window and the exhaustive fallback that makes the top-8 lists sufficient.
 //
-// CTA = 256 threads: warp 0 TMA producer, warp 1 MMA issuer, warp 2 TMEM allocator, warps 4-7
-// epilogue (TMEM lane quarter = warp % 4 = two query-block rows).  3-stage smem ring (56 KB per
-// stage), 2 x 256-column TMEM accumulators so the epilogue of Ref tile n overlaps the MMAs of
-// tile n+1.  Persistent: grid = #SMs, work item = (image, query tile, Ref chunk).
+// CTA = 512 threads: warp 0 TMA producer, warps 4-7 epilogue (one accumulator row per thread), warps 8-15 two
+// MMA warpgroups (accumulator rows 0-63 / 64-127, 64 fp32 registers per thread).  4-stage smem ring (30 KB per
+// stage); a finished accumulator is staged in shared memory, so the epilogue of Ref tile n overlaps the MMAs of
+// tile n+1 (which accumulate in registers).  Persistent: grid = #SMs, work item = (image, query tile, Ref chunk).
 #include "corr_internal.cuh"
 
 namespace c2m {
@@ -35,24 +35,24 @@ namespace {
 constexpr int PATCH = 3;
 constexpr int BW = 16;                             // block width in pixels (both sides)
 constexpr int TV = BW - (PATCH - 1);               // 14 valid patch origins per block row
-constexpr int TQ_R = 8;                            // query block rows  -> UMMA M = 8 * 16 = 128
-constexpr int TR_R = 16;                           // Ref block rows    -> UMMA N = 16 * 16 = 256
+constexpr int TQ_R = 8;                            // query block rows  -> M = 8 * 16 = 128 (two m64 warpgroups)
+constexpr int TR_R = 8;                            // Ref block rows    -> wgmma N = 8 * 16 = 128
 constexpr int A_R = TQ_R + PATCH - 1;              // 10 staged rows
-constexpr int B_R = TR_R + PATCH - 1;              // 18
+constexpr int B_R = TR_R + PATCH - 1;              // 10
 constexpr int KOCT = 4;                            // channel octets per stage (32 channels)
 constexpr int ROW_B = BW * 16;                     // 256 B block row pitch (= row-tap offset)
 constexpr int A_OCT_B = A_R * ROW_B;               // 2560 B octet pitch of A (= LBO)
-constexpr int B_OCT_B = B_R * ROW_B;               // 4608 B octet pitch of B (= LBO)
+constexpr int B_OCT_B = B_R * ROW_B;               // 2560 B octet pitch of B (= LBO)
 constexpr int A_BYTES = KOCT * A_OCT_B;            // 10240
-constexpr int B_BYTES = KOCT * B_OCT_B;            // 18432
-constexpr int STAGE_BYTES = 2 * A_BYTES + B_BYTES;     // query hi + lo, Ref hi = 38912
-constexpr int NSTAGE = 5;
-constexpr int UM = TQ_R * BW, UN = TR_R * BW;      // 128, 256
-constexpr int TMEM_COLS = 512;
+constexpr int B_BYTES = KOCT * B_OCT_B;            // 10240
+constexpr int STAGE_BYTES = 2 * A_BYTES + B_BYTES;     // query hi + lo, Ref hi = 30720
+constexpr int NSTAGE = 4;
+constexpr int UM = TQ_R * BW, UN = TR_R * BW;      // 128, 128
 constexpr int SMEM_AUX = 2 * UN * 8 + 128;         // (scale, bias) per column, double buffered, + barriers
-constexpr int SMEM_BYTES = NSTAGE * STAGE_BYTES + SMEM_AUX + 1024;
+constexpr int SMEM_BYTES = NSTAGE * STAGE_BYTES + acc_stage_bytes(UN) + SMEM_AUX + 1024;
 static_assert(A_BYTES % 128 == 0 && B_BYTES % 128 == 0, "TMA destinations must stay 128B aligned");
-static_assert(UM == 128 && UN == 256, "tile shape is tied to the UMMA instruction shape");
+static_assert(UM == 128 && UN == 128, "tile shape: two m64 warpgroups x an n128 wgmma");
+static_assert(SMEM_BYTES <= 227 * 1024, "shared memory per block");
 
 struct UmmaParams {
     int B, C8;
@@ -63,18 +63,18 @@ struct UmmaParams {
 };
 }  // namespace
 
-__global__ void __launch_bounds__(256, 1)
+__global__ void __launch_bounds__(512, 1)
 corr_umma_kernel(const __grid_constant__ CUtensorMap tm_in_hi, const __grid_constant__ CUtensorMap tm_in_lo,
-                 const __grid_constant__ CUtensorMap tm_ref_hi, const __grid_constant__ CUtensorMap tm_ref_lo,
+                 const __grid_constant__ CUtensorMap tm_ref_hi,
                  const float *__restrict__ rinv, const int *__restrict__ sexp, Candidate *__restrict__ part,
                  const UmmaParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t *aux = smem + NSTAGE * STAGE_BYTES;
+    float *acc_s = reinterpret_cast<float *>(smem + NSTAGE * STAGE_BYTES);          // [UN][ACC_PITCH]
+    uint8_t *aux = smem + NSTAGE * STAGE_BYTES + acc_stage_bytes(UN);
     float2 *rcol = reinterpret_cast<float2 *>(aux);                 // [2][UN] (score scale, bias)
     uint64_t *bars = reinterpret_cast<uint64_t *>(aux + 2 * UN * 8);
-    uint64_t *full = bars, *empty = bars + NSTAGE, *tfull = bars + 2 * NSTAGE, *tempty = bars + 2 * NSTAGE + 2;
-    uint32_t *tmem_base_p = reinterpret_cast<uint32_t *>(bars + 2 * NSTAGE + 4);
+    uint64_t *full = bars, *empty = bars + NSTAGE, *tfull = bars + 2 * NSTAGE, *tempty = bars + 2 * NSTAGE + 1;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -84,26 +84,20 @@ corr_umma_kernel(const __grid_constant__ CUtensorMap tm_in_hi, const __grid_cons
         tma_prefetch_desc(&tm_ref_hi);
     }
     if (warp == 1 && lane == 0) {
-        for (int i = 0; i < NSTAGE; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], 4); }
+        for (int i = 0; i < NSTAGE; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 256); }
+        mbar_init(tfull, 256);
+        mbar_init(tempty, 4);
         fence_mbar_init();
     }
-    if (warp == 2) {
-        tmem_alloc(tmem_base_p, TMEM_COLS);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_base_p;
 
     const int n_qt = p.qt_x * p.qt_y, n_rt = p.rt_x * p.rt_y;
     const int n_items = p.B * n_qt * p.nchunk;
     const int n_kc = (p.C8 + KOCT - 1) / KOCT;
 
-    if (warp == 0) {
+    if (warp < 4) {
         // ================================ TMA producer =====================================
-        if (lane == 0) {
+        if (warp == 0 && lane == 0) {
             int stage = 0, phase = 0;
             for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
                 const int chunk = item % p.nchunk, qt = (item / p.nchunk) % n_qt, b = item / (p.nchunk * n_qt);
@@ -123,60 +117,62 @@ corr_umma_kernel(const __grid_constant__ CUtensorMap tm_in_hi, const __grid_cons
                 }
             }
         }
-    } else if (warp == 1) {
-        // ================================ MMA issuer =======================================
-        if (lane == 0) {
-            constexpr uint32_t idesc = umma_idesc_f16(UM, UN, 0);
-            int stage = 0, phase = 0, acc = 0, acc_phase = 0;
-            for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-                const int chunk = item % p.nchunk;
-                const int rt_b = chunk * p.rt_per_chunk, rt_e = min(n_rt, rt_b + p.rt_per_chunk);
-                for (int rt = rt_b; rt < rt_e; ++rt) {
-                    mbar_wait(&tempty[acc], acc_phase ^ 1);
-                    tc_fence_after();
-                    const uint32_t d = tmem_base + acc * UN;
-                    for (int kc = 0; kc < n_kc; ++kc) {
-                        mbar_wait(&full[stage], phase);
-                        tc_fence_after();
-                        const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
-                        // descriptors of (row tap 0, k-step 0); every other MMA is a constant offset away
-                        const uint64_t dah0 = umma_smem_desc(sa, A_OCT_B, 128);
-                        const uint64_t dal0 = umma_smem_desc(sa + A_BYTES, A_OCT_B, 128);
-                        const uint64_t dbh0 = umma_smem_desc(sa + 2 * A_BYTES, B_OCT_B, 128);
+    } else if (warp >= 8) {
+        // ================================ MMA ==============================================
+        // warpgroup wg computes accumulator rows [64 wg, 64 wg + 64) (query block rows 4 wg .. 4 wg + 3): its A
+        // operand starts 8 core-matrix groups (1024 B) further in
+        const int wg = (warp >> 2) - 2;
+        int stage = 0, phase = 0;
+        uint32_t tphase = 0;
+        for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+            const int chunk = item % p.nchunk;
+            const int rt_b = chunk * p.rt_per_chunk, rt_e = min(n_rt, rt_b + p.rt_per_chunk);
+            for (int rt = rt_b; rt < rt_e; ++rt) {
+                float acc[UN / 2];
+                for (int kc = 0; kc < n_kc; ++kc) {
+                    mbar_wait(&full[stage], phase);
+                    const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
+                    // descriptors of (row tap 0, k-step 0); every other MMA is a constant offset away
+                    const uint64_t dah0 = wg_smem_desc(sa + wg * 1024, A_OCT_B, 128);
+                    const uint64_t dal0 = wg_smem_desc(sa + A_BYTES + wg * 1024, A_OCT_B, 128);
+                    const uint64_t dbh0 = wg_smem_desc(sa + 2 * A_BYTES, B_OCT_B, 128);
+                    wgmma_fence();
 #pragma unroll
-                        for (int dy = 0; dy < PATCH; ++dy) {
+                    for (int dy = 0; dy < PATCH; ++dy) {
 #pragma unroll
-                            for (int j = 0; j < KOCT / 2; ++j) {
-                                const uint32_t ao = dy * ROW_B + j * 2 * A_OCT_B, bo = dy * ROW_B + j * 2 * B_OCT_B;
-                                const uint64_t dah = umma_desc_advance(dah0, ao), dal = umma_desc_advance(dal0, ao);
-                                const uint64_t dbh = umma_desc_advance(dbh0, bo);
-                                // (q_hi + q_lo) * r_hi: the query keeps its 22-bit split, the Ref operand is its fp16
-                                // rounding.  The search only RANKS; the 2^-11 this costs is part of the rescoring
-                                // window (DESIGN.md K2), and a third of the MMAs of the three-product scheme is gone.
-                                umma_f16(d, dah, dbh, idesc, (kc | dy | j) != 0);
-                                umma_f16(d, dal, dbh, idesc, 1);
-                            }
+                        for (int j = 0; j < KOCT / 2; ++j) {
+                            const uint32_t ao = dy * ROW_B + j * 2 * A_OCT_B, bo = dy * ROW_B + j * 2 * B_OCT_B;
+                            const uint64_t dbh = wg_desc_advance(dbh0, bo);
+                            // (q_hi + q_lo) * r_hi: the query keeps its 22-bit split, the Ref operand is its fp16
+                            // rounding.  The search only RANKS; the 2^-11 this costs is part of the rescoring
+                            // window (DESIGN.md K2).
+                            Wgmma<UN>::mma(acc, wg_desc_advance(dah0, ao), dbh, (kc | dy | j) != 0);
+                            Wgmma<UN>::mma(acc, wg_desc_advance(dal0, ao), dbh, 1);
                         }
-                        umma_commit(&empty[stage]);        // smem slot free once these MMAs retire
-                        if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
                     }
-                    umma_commit(&tfull[acc]);               // accumulator complete
-                    if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+                    wgmma_commit();
+                    wgmma_wait_all();
+                    mbar_arrive(&empty[stage]);                 // smem slot free
+                    if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
                 }
+                mbar_wait(tempty, tphase ^ 1);                  // the epilogue has read the previous tile
+                acc_store(acc_s, wg * 64, acc);
+                mbar_arrive(tfull);                             // accumulator complete
+                tphase ^= 1;
             }
         }
-    } else if (warp >= 4) {
+    } else {
         // ================================ epilogue =========================================
-        // Branch-free inner loop (the per-score compare-and-insert of the first version kept the tensor pipe at
-        // 38 %): per 32-column block (two Ref block rows, 28 valid scores) only min / max run per score —
-        // m1 >= m2 >= m3 = the block's three best — and only m1, m2 are offered to the top-4 list.
+        // Branch-free inner loop: per 32-column block (two Ref block rows, 28 valid scores) only min / max run per
+        // score — m1 >= m2 >= m3 = the block's three best — and only m1, m2 are offered to the top-k list.
         // Everything that is not in the list (block thirds, evicted entries) feeds `dropped`, the largest score
         // left behind; the rescoring pass re-scans the chunk exhaustively when `dropped` reaches its window.
         const int e = threadIdx.x - 128;                    // 0..127 = accumulator row m = 16 * block row + block column
-        const int quarter = warp & 3;
         const int yy = e >> 4, xx = e & 15;
         const float sinv = ldexpf(1.f, -(sexp[0] + sexp[1]));
-        int acc = 0, acc_phase = 0;
+        const float *acc_row = acc_s + e;
+        int acc = 0;
+        uint32_t tphase = 0;
         for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
             const int chunk = item % p.nchunk, qt = (item / p.nchunk) % n_qt, b = item / (p.nchunk * n_qt);
             const int qy = (qt / p.qt_x) * TQ_R + yy, qx = (qt % p.qt_x) * TV + xx;
@@ -198,15 +194,13 @@ corr_umma_kernel(const __grid_constant__ CUtensorMap tm_in_hi, const __grid_cons
                     rc[n] = ok ? make_float2(rinvb[ry * p.rw + rx] * sinv, 0.f) : make_float2(0.f, -INFINITY);
                 }
                 asm volatile("bar.sync 1, 128;" ::: "memory");
-                mbar_wait(&tfull[acc], acc_phase);
-                tc_fence_after();
-                const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + acc * UN;
+                mbar_wait(tfull, tphase);
+                tphase ^= 1;
                 const uint32_t rc_s = smem_u32(rc);
 #pragma unroll 1
                 for (int cc = 0; cc < UN / 32; ++cc) {      // 32 columns = two Ref block rows
                     uint32_t reg[32];
-                    tmem_ld_32x32(taddr + cc * 32, reg);
-                    tmem_ld_wait();
+                    acc_ld32(acc_row, cc * 32, UN, reg);
                     float sv[2 * TV];
                     float m1 = -INFINITY, m2 = -INFINITY, m3 = -INFINITY;      // block best, second, third
 #pragma unroll
@@ -244,22 +238,15 @@ corr_umma_kernel(const __grid_constant__ CUtensorMap tm_in_hi, const __grid_cons
                         dropped = fmaxf(dropped, m2);
                     }
                 }
-                tc_fence_before();
                 __syncwarp();
-                if (lane == 0) mbar_arrive(&tempty[acc]);
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+                if (lane == 0) mbar_arrive(tempty);
+                acc ^= 1;
             }
             if (xx < TV && qy < p.gh && qx < p.gw)
                 part[((size_t)b * p.nchunk + chunk) * p.NQ + qy * p.gw + qx] = cand_pack(cv, ci, dropped);
         }
     }
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, TMEM_COLS);
-    }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -311,7 +298,7 @@ void corr_umma_tiles(const CorrGeom &g, int &n_qt, int &n_rt) {
 int corr_umma_pick_nchunk(const CorrGeom &g, int sms) {
     int n_qt, n_rt;
     corr_umma_tiles(g, n_qt, n_rt);
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
     int best_n = 1;
     double best_cost = 1e300;
     for (int n = 1; n <= CORR_MAX_CHUNKS && n <= n_rt; ++n) {
@@ -321,7 +308,7 @@ int corr_umma_pick_nchunk(const CorrGeom &g, int sms) {
         const long long items = (long long)g.B * n_qt * n;
         const double waves = (double)((items + sms - 1) / sms);
         // + what the exhaustive re-scan of overflowing (query, chunk) pairs costs per query tile: it grows with the chunk
-        // length (fitted on the bench step, `profiles/r02_search_chunks.md`); shorter chunks also mean more list slots
+        // length (fitted on the bench step); shorter chunks also mean more list slots
         const double q_tiles = (double)g.B * n_qt;
         const double cost = waves * (per + 0.35) + q_tiles * 2e-3 * per;
         if (cost < best_cost - 1e-9) { best_cost = cost; best_n = n; }
@@ -340,13 +327,12 @@ void corr_umma_chunk_geom(const CorrGeom &g, int nchunk, CorrChunkGeom &cg) {
 }
 
 int corr_search_umma_launch(const CorrGeom &g, const CorrWorkspace &ws, cudaStream_t st) {
-    CUtensorMap tih, til, trh, trl;
+    CUtensorMap tih, til, trh;
     const int C8 = g.Cp / 8;
     int rc;
     if ((rc = make_map(&tih, ws.hi_in, g.B, C8, g.h, g.w, A_R))) return rc;
     if ((rc = make_map(&til, ws.lo_in, g.B, C8, g.h, g.w, A_R))) return rc;
     if ((rc = make_map(&trh, ws.hi_ref, g.B, C8, g.hr, g.wr, B_R))) return rc;
-    if ((rc = make_map(&trl, ws.lo_ref, g.B, C8, g.hr, g.wr, B_R))) return rc;
 
     UmmaParams p;
     p.B = g.B; p.C8 = C8;
@@ -364,7 +350,7 @@ int corr_search_umma_launch(const CorrGeom &g, const CorrWorkspace &ws, cudaStre
     C2M_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     const int n_items = g.B * p.qt_x * p.qt_y * p.nchunk;
     const int grid = n_items < sms ? n_items : sms;
-    corr_umma_kernel<<<grid, 256, SMEM_BYTES, st>>>(tih, til, trh, trl, ws.rinv, ws.sexp, ws.part, p);
+    corr_umma_kernel<<<grid, 512, SMEM_BYTES, st>>>(tih, til, trh, ws.rinv, ws.sexp, ws.part, p);
     C2M_LAUNCH_CHECK("corr_umma_kernel");
     return C2M_OK;
 }

@@ -125,7 +125,7 @@ static int make_geo(Geo &g, const c2m_dcn_shape *s) {
     C2M_CHECK_ARG(g.Ho > 0 && g.Wo > 0, "dcn backward: empty output");
     return C2M_OK;
 }
-static inline int blocks_for(long long n) { long long b = (n + 255) / 256; return (int)(b > 148 * 16 ? 148 * 16 : b); }
+static inline int blocks_for(long long n) { long long b = (n + 255) / 256; return (int)(b > 132 * 16 ? 132 * 16 : b); }
 
 }  // namespace c2m
 

@@ -1,15 +1,15 @@
-// Modulated deformable convolution v2 forward on the sm_100a tensor cores (3x3, stride 1, pad 1,
+// Modulated deformable convolution v2 forward on the sm_90a tensor cores (3x3, stride 1, pad 1,
 // dilation 1 — every DCN of C2-Matching), fused with DCN_sep_pre_multi_offset's prologue.
 //
 // Replaces `_ext.dcn_v2_forward` (mmsr/models/archs/DCNv2/src/cuda/dcn_v2_cuda.cu:42-172: im2col
 // into a 236-944 MB `columns` buffer + batched fp32 SGEMM) and the Python prologue
 // (DCNv2/dcn_v2.py:233-250).  Sampling arithmetic follows dcn_v2_im2col_cuda.cu:25-54,125-195
-// operation for operation; the contraction is a split-fp16 (hi*hi + hi*lo + lo*hi) tcgen05 GEMM
-// with fp32 TMEM accumulation, i.e. fp32-grade.
+// operation for operation; the contraction is a split-fp16 (hi*hi + hi*lo + lo*hi) wgmma GEMM
+// with fp32 accumulation, i.e. fp32-grade.
 //
 // Structure = conv3x3_umma.cu with the TMA activation producer replaced by GATHER warps:
 //   K is ordered (deformable group g, tap, channel-in-group); a stage = (128-pixel tile, 4 K octets).
-//   16 gather warps build the column tile [4 octets][128 px][8] directly in the tcgen05 K-major
+//   16 gather warps build the column tile [4 octets][128 px][8] directly in the wgmma K-major
 //   no-swizzle layout (hi and lo halves).  A gather thread owns (pixel, run of L K-octets that share one
 //   (g, tap) pair), L = min(C/dg/8, 4): the sampling point — raw conv_offset_mask output + pre-offset, sigmoid
 //   mask, the 4 corner offsets and mask-folded bilinear weights — is computed ONCE per (pixel, g, tap) and reused
@@ -17,15 +17,14 @@
 //   16 B (hi) + 16 B (lo) per corner from the octet-planar PSA input (L2 evict-last: the input map is re-read by all
 //   nine taps and must stay resident, while offsets / outputs stream through with evict-first), blended (hi halves
 //   in fp32, lo halves in packed fp16), split and stored with one 16 B st.shared per half;
-//   fence.proxy.async + mbarrier hand the stage to the MMA-issuing thread.
-//   Pre-offsets: per tile group the index-map cells a tile can touch ((16/s + 2) x (8/s + 2) per tile) are
-//   decoded once into a shared-memory flow table, so the per-(pixel, tap) pre-offset is one ld.shared instead
-//   of an 8-byte global load, two integer divisions and a modulo per (pixel, g, tap).
-//   Weights stream as 8 KB chunks (bulk copy ring), shared by a group of up to 8 pixel
-//   tiles (512/N TMEM accumulators, rotated across groups); every CTA owns an evenly sized contiguous
-//   range of the flat (slice, image, tile) list, so small problems (BASELINE config 4: 200 tiles)
-//   spread over all SMs.  The epilogue (bias, LeakyReLU, PSA and / or fp32 store) is shared with
-//   the plain convolution.
+//   fence.proxy.async + mbarrier hand the stage to the MMA warpgroup.
+//   Pre-offsets: per tile the index-map cells it can touch ((16/s + 2) x (8/s + 2)) are decoded once into a
+//   shared-memory flow table, so the per-(pixel, tap) pre-offset is one ld.shared instead of an 8-byte global
+//   load, two integer divisions and a modulo per (pixel, g, tap).
+//   Weights stream as 8 KB chunks (bulk copy ring).  One launch computes one 64-wide slice of the output channels
+//   (the fp32 accumulator of a 128 x 64 tile is what one warpgroup holds in registers next to the gather warps);
+//   wider layers take one launch per slice.  The epilogue (bias, LeakyReLU, PSA and / or fp32 store) is shared
+//   with the plain convolution.
 // The im2col matrix never exists outside shared memory.
 #include <cstdlib>
 
@@ -63,7 +62,8 @@ struct DcnTc {
     int opp_shift;             // log2(opp) when opp is a power of two, else -1 (then L == 1)
     int nstage, nbst;          // ring depths (activation stages, weight chunks); powers of two
     int nstage_shift;          // log2(nstage)
-    int tg;                    // pixel tiles per work item (<= T)
+    int tg;                    // pixel tiles per work item (1: the accumulator lives in registers)
+    int slice;                 // 64-wide output-channel slice this launch computes
     int policy;                // L2 policies: 1 = input map evict-last, 2 = offsets / mask evict-first, 4 = streaming output stores
     int sc_shift;              // log2(pre_scale) when the flow table is used (idx given, scale in {1,2,4,8}), else -1
     int tab_h, tab_w;          // flow-table cells per tile: 16/s + 2, 8/s + 2
@@ -104,11 +104,10 @@ __device__ __forceinline__ uint4 ldg_keep_v4(const void *ptr, uint64_t pol) {
                  : "l"(ptr), "l"(pol));
     return v;
 }
-// one (pixel, octet) of the interleaved operand: 32 B = one sector, one 256-bit load
+// one (pixel, octet) of the interleaved operand: 32 B = one sector, two 128-bit loads
 __device__ __forceinline__ void ldg_keep_v8(const void *ptr, uint64_t pol, uint4 &h, uint4 &l) {
-    asm volatile("ld.global.nc.L2::cache_hint.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8], %9;"
-                 : "=r"(h.x), "=r"(h.y), "=r"(h.z), "=r"(h.w), "=r"(l.x), "=r"(l.y), "=r"(l.z), "=r"(l.w)
-                 : "l"(ptr), "l"(pol));
+    h = ldg_keep_v4(ptr, pol);
+    l = ldg_keep_v4(static_cast<const uint8_t *>(ptr) + 16, pol);
 }
 __device__ __forceinline__ float2 ldg_stream_f2(const float *ptr, uint64_t pol) {
     float2 v;
@@ -121,53 +120,39 @@ __device__ __forceinline__ float ldg_stream_f1(const float *ptr, uint64_t pol) {
     return v;
 }
 
+template <int N>
 __global__ void __launch_bounds__(NTHREADS, 1)
-dcn_umma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
+dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    const uint32_t w_half = (uint32_t)KOCT * p.N * 16;
-    const uint32_t w_chunk = 2 * w_half;
+    constexpr uint32_t w_half = (uint32_t)KOCT * N * 16;
+    constexpr uint32_t w_chunk = 2 * w_half;
     uint8_t *sW = smem;                                   // [nbst][hi | lo]
     uint8_t *sA = smem + d.nbst * w_chunk;                // N multiple of 16 -> multiple of 128
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sA + d.nstage * A_STAGE);
-    uint64_t *full = bars, *empty = full + MAX_NSTAGE, *bfull = empty + MAX_NSTAGE, *bempty = bfull + MAX_NBST,
-             *tfull = bempty + MAX_NBST, *tempty = tfull + MAXT;
-    uint32_t *tmem_base_p = reinterpret_cast<uint32_t *>(tempty + MAXT);
-    float *sbias = reinterpret_cast<float *>(tmem_base_p + 4);                    // [N <= 256], 16 B aligned
-    int4 *tile_info = reinterpret_cast<int4 *>(sbias + 256);                      // [2][MAXT] (b, y0, x0, image pixel base)
+    float *acc_s = reinterpret_cast<float *>(sA + d.nstage * A_STAGE);             // [N][ACC_PITCH]
+    uint64_t *bars = reinterpret_cast<uint64_t *>(reinterpret_cast<uint8_t *>(acc_s) + acc_stage_bytes(N));
+    uint64_t *full = bars, *empty = full + MAX_NSTAGE, *bfull = empty + MAX_NSTAGE, *bempty = bfull + MAX_NBST;
+    float *sbias = reinterpret_cast<float *>(bempty + MAX_NBST);                  // [N <= 64], 16 B aligned
+    int4 *tile_info = reinterpret_cast<int4 *>(sbias + 64);                       // [2][MAXT] (b, y0, x0, image pixel base)
     float2 *flow_tab = reinterpret_cast<float2 *>(tile_info + 2 * MAXT);          // [2][T][tab_h * tab_w]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tiles_img = p.tiles_x * p.tiles_y;
-    // Work = flat list of (image, pixel tile), cut into items of Tg consecutive tiles (they share the streamed weight
-    // chunks); item i runs on CTA i % grid.  At any moment the CTAs therefore work on ~grid * Tg CONSECUTIVE tiles —
-    // a third of one image at the largest layer — so the gathered input map of ONE image (105 MB) is what has to
-    // stay in L2, not the whole batch (contiguous per-CTA ranges spread the CTAs over all images at once: ncu showed
-    // 7.3 GB of DRAM reads for 2.3 GB of algorithmic traffic).  Tg shrinks for small problems so all SMs get work.
+    // Work = flat list of (image, pixel tile), one tile per item (its accumulator lives in the MMA warpgroup's
+    // registers); item i runs on CTA i % grid, so at any moment the CTAs work on ~grid CONSECUTIVE tiles and the
+    // gathered input map of ONE image is what has to stay in L2, not the whole batch.
     const int TT = p.B * tiles_img;
     const int n_work = TT;
     const int Tg = d.tg;
     const int n_items = (n_work + Tg - 1) / Tg;
-    const int nacc = p.T;                                // TMEM accumulators, rotated across groups
-    const uint32_t need_cols = (uint32_t)p.N * p.T;
-    const uint32_t tmem_cols = need_cols <= 32 ? 32 : need_cols <= 64 ? 64 : need_cols <= 128 ? 128
-                               : need_cols <= 256 ? 256 : 512;
     const int nstage_mask = d.nstage - 1;                // ring depths are powers of two
 
     if (warp == 1 && lane == 0) {
-        for (int i = 0; i < d.nstage; ++i) { mbar_init(&full[i], NGATHER_WARPS >> d.lshift); mbar_init(&empty[i], 1); }
-        for (int i = 0; i < d.nbst; ++i) { mbar_init(&bfull[i], 1); mbar_init(&bempty[i], 1); }
-        for (int i = 0; i < MAXT; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], 4); }
+        for (int i = 0; i < d.nstage; ++i) { mbar_init(&full[i], NGATHER_WARPS >> d.lshift); mbar_init(&empty[i], 128); }
+        for (int i = 0; i < d.nbst; ++i) { mbar_init(&bfull[i], 1); mbar_init(&bempty[i], 128); }
         fence_mbar_init();
     }
-    if (warp == 2) {
-        tmem_alloc(tmem_base_p, tmem_cols);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_base_p;
     const int sw = *reinterpret_cast<const int *>(q.wblob);
 
     auto group = [&](int item, int &pos, int &nt) {
@@ -176,19 +161,21 @@ dcn_umma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
     };
 
     // Register budget per warpgroup.  The CTA's pool is what it was launched with (80 x 768 = 61440):
-    // the control warpgroup gives 40 x 128 back and the epilogue (32 TMEM columns in flight) takes
-    // them, 40 + 120 + 4 x 80 = 480 = 6 x 80.  Requests beyond the pool would block forever.
+    // the control warpgroup gives 56 x 128 back and the MMA / epilogue warpgroup takes them,
+    // 24 + 136 + 4 x 80 = 480 = 6 x 80.  Requests beyond the pool would block forever.
     if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");
     if (warp == 0) {
         // ================================ weight producer ===================================
         if (lane == 0) {
             int bst = 0, bphase = 0;
             for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+                int pos, nt;
+                group(item, pos, nt);
                 for (int kc = 0; kc < p.nkc; ++kc) {
                     mbar_wait(&bempty[bst], bphase ^ 1);
                     mbar_arrive_expect_tx(&bfull[bst], w_chunk);
-                    const uint8_t *src = q.wblob + W_HDR + (size_t)kc * w_chunk;
+                    const uint8_t *src = q.wblob + W_HDR + ((size_t)d.slice * p.nkc + kc) * w_chunk;
                     asm volatile(
                         "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                         ::"r"(smem_u32(sW + bst * w_chunk)), "l"(src), "r"(w_chunk), "r"(smem_u32(&bfull[bst]))
@@ -197,95 +184,66 @@ dcn_umma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
                 }
             }
         }
-    } else if (warp == 1) {
-        // ================================ MMA issuer ========================================
-        {   // whole warp, uniform control flow; one elected lane issues (see umma_f16_w)
-            const uint32_t idesc = umma_idesc_f16(128, p.N, 0);
-            const uint32_t b_lbo = p.N * 16;
-            int stage = 0, phase = 0, bst = 0, bphase = 0;
-            uint32_t tph = 0;
-            int abase = 0;
-            for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-                int pos, nt;
-                group(item, pos, nt);
-                for (int kc = 0; kc < p.nkc; ++kc) {
-                    mbar_wait(&bfull[bst], bphase);
-                    tc_fence_after();
-                    const uint32_t w_hi = smem_u32(sW + bst * w_chunk), w_lo = w_hi + w_half;
-                    for (int t = 0; t < nt; ++t) {
-                        int a = abase + t;
-                        if (a >= nacc) a -= nacc;
-                        if (kc == 0) {
-                            mbar_wait(&tempty[a], ((tph >> a) & 1u) ^ 1u);
-                            tc_fence_after();
-                        }
-                        const uint32_t dacc = tmem_base + a * p.N;
-                        mbar_wait(&full[stage], phase);
-                        tc_fence_after();
-                        const uint32_t a_hi = smem_u32(sA + stage * A_STAGE), a_lo = a_hi + A_HALF;
-#pragma unroll
-                        for (int j = 0; j < KOCT / 2; ++j) {
-                            const uint32_t ao = j * 2 * A_OCT_B, bo = j * 2 * b_lbo;
-                            const uint64_t dah = umma_smem_desc(a_hi + ao, A_OCT_B, 128);
-                            const uint64_t dal = umma_smem_desc(a_lo + ao, A_OCT_B, 128);
-                            const uint64_t dbh = umma_smem_desc(w_hi + bo, b_lbo, 128);
-                            const uint64_t dbl = umma_smem_desc(w_lo + bo, b_lbo, 128);
-                            umma_f16_w(dacc, dah, dbh, idesc, (kc | j) != 0);
-                            umma_f16_w(dacc, dah, dbl, idesc, 1);
-                            umma_f16_w(dacc, dal, dbh, idesc, 1);
-                        }
-                        umma_commit_w(&empty[stage]);
-                        if (++stage == d.nstage) { stage = 0; phase ^= 1; }
-                        if (kc == p.nkc - 1) { umma_commit_w(&tfull[a]); tph ^= 1u << a; }
-                    }
-                    umma_commit_w(&bempty[bst]);
-                    if (++bst == d.nbst) { bst = 0; bphase ^= 1; }
-                }
-                abase += nt;
-                if (abase >= nacc) abase -= nacc;
-            }
-        }
     }
     } else if (warp < 8) {
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 120;");
-        // ================================ epilogue ==========================================
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 136;");
+        // ================================ MMA + epilogue ====================================
+        // one warpgroup: the wgmmas of both 64-row halves of the tile (A rows 64.. start 8 core-matrix groups in),
+        // then the accumulator goes through shared memory to the epilogue, one pixel per thread
         const int e = threadIdx.x - 128;
-        const int quarter = warp & 3;
         const float out_scale = ldexpf(1.f, -(p.sa_in + sw));
         const float res_scale = 1.f;
         const float so = ldexpf(1.f, p.sa_out);
         const bool fast = epilogue_fast_ok(q, p) && p.sa_out == 0;     // (this kernel does not pre-scale bias / factors)
-        uint32_t tph = 0;
-        int abase = 0;
-        for (int i = e; i < p.N; i += 128) sbias[i] = (q.bias && i < p.Cout) ? q.bias[i] : 0.f;
+        const int o_base = d.slice * N;
+        for (int i = e; i < N; i += 128) sbias[i] = (q.bias && o_base + i < p.Cout) ? q.bias[o_base + i] : 0.f;
         asm volatile("bar.sync 1, 128;" ::: "memory");
-        const int o_base = 0;
+        constexpr uint32_t b_lbo = N * 16;
+        int stage = 0, phase = 0, bst = 0, bphase = 0;
         for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
             int pos, nt;
             group(item, pos, nt);
-            for (int t = 0; t < nt; ++t) {
-                const int r = pos + t;
-                const int b = r / tiles_img, tt = r - b * tiles_img;
-                const int y = (tt / p.tiles_x) * T_R + e / T_C, x = (tt % p.tiles_x) * T_C + e % T_C;
-                const bool ok = y < p.H && x < p.W;
-                int a = abase + t;
-                if (a >= nacc) a -= nacc;
-                mbar_wait(&tfull[a], (tph >> a) & 1u);
-                tph ^= 1u << a;
-                tc_fence_after();
-                const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + a * p.N;
-                for (int c0 = 0; c0 < p.N; c0 += 32) {
-                    if (fast && c0 + 32 <= p.N && c0 + 32 <= p.Cout)
-                        epilogue_fast_dispatch<false>(q, p, taddr, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, nullptr);
-                    else
-                        epilogue_store_block(q, p, taddr, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, so);
+            const int b = pos / tiles_img, tt = pos - b * tiles_img;
+            const int y = (tt / p.tiles_x) * T_R + e / T_C, x = (tt % p.tiles_x) * T_C + e % T_C;
+            const bool ok = y < p.H && x < p.W;
+            float acc0[N / 2], acc1[N / 2];                 // rows [0, 64) and [64, 128)
+            for (int kc = 0; kc < p.nkc; ++kc) {
+                mbar_wait(&bfull[bst], bphase);
+                mbar_wait(&full[stage], phase);
+                const uint32_t w_hi = smem_u32(sW + bst * w_chunk), w_lo = w_hi + w_half;
+                const uint32_t a_hi = smem_u32(sA + stage * A_STAGE), a_lo = a_hi + A_HALF;
+                wgmma_fence();
+#pragma unroll
+                for (int j = 0; j < KOCT / 2; ++j) {
+                    const uint32_t ao = j * 2 * A_OCT_B, bo = j * 2 * b_lbo;
+                    const uint64_t dbh = wg_smem_desc(w_hi + bo, b_lbo, 128);
+                    const uint64_t dbl = wg_smem_desc(w_lo + bo, b_lbo, 128);
+                    const uint64_t dah = wg_smem_desc(a_hi + ao, A_OCT_B, 128);
+                    const uint64_t dal = wg_smem_desc(a_lo + ao, A_OCT_B, 128);
+                    Wgmma<N>::mma(acc0, dah, dbh, (kc | j) != 0);
+                    Wgmma<N>::mma(acc0, dah, dbl, 1);
+                    Wgmma<N>::mma(acc0, dal, dbh, 1);
+                    Wgmma<N>::mma(acc1, wg_desc_advance(dah, 1024), dbh, (kc | j) != 0);
+                    Wgmma<N>::mma(acc1, wg_desc_advance(dah, 1024), dbl, 1);
+                    Wgmma<N>::mma(acc1, wg_desc_advance(dal, 1024), dbh, 1);
                 }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tempty[a]);
+                wgmma_commit();
+                wgmma_wait_all();
+                mbar_arrive(&empty[stage]);
+                mbar_arrive(&bempty[bst]);
+                if (++stage == d.nstage) { stage = 0; phase ^= 1; }
+                if (++bst == d.nbst) { bst = 0; bphase ^= 1; }
             }
-            abase += nt;
-            if (abase >= nacc) abase -= nacc;
+            asm volatile("bar.sync 1, 128;" ::: "memory");          // previous tile's epilogue is done
+            acc_store(acc_s, 0, acc0);
+            acc_store(acc_s, 64, acc1);
+            asm volatile("bar.sync 1, 128;" ::: "memory");
+            for (int c0 = 0; c0 < N; c0 += 32) {
+                if (fast && c0 + 32 <= N && o_base + c0 + 32 <= p.Cout)
+                    epilogue_fast_dispatch(q, p, acc_s + e, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, nullptr);
+                else
+                    epilogue_store_block(q, p, acc_s + e, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, so);
+            }
         }
     } else {
         // ================================ gather producers ==================================
@@ -522,12 +480,6 @@ dcn_umma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
         }
     }
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, tmem_cols);
-    }
 }
 
 // blob: header | [slice][kc][hi|lo][octet 4][N][8], K ordered (g, tap, channel-in-group)
@@ -575,10 +527,10 @@ __global__ void dcn_wamax_kernel(const float *__restrict__ w, int n, unsigned *_
 }
 
 static inline int d_pad16(int c) { return (c + 15) / 16 * 16; }
-// the gather is the expensive side, so one CTA owns ALL output channels (N up to 256) instead of
-// re-gathering per 64-wide slice; tiles per item shrink so that T*N <= 512 TMEM columns
-static inline int d_slice_n(int cout) { return d_pad16(cout); }
-static inline int d_n_slice(int cout) { (void)cout; return 1; }
+// output channels per launch: a 128 x 64 fp32 accumulator is what the MMA warpgroup keeps in registers
+constexpr int D_NMAX = 64;
+static inline int d_slice_n(int cout) { return cout <= D_NMAX ? d_pad16(cout) : D_NMAX; }
+static inline int d_n_slice(int cout) { return (cout + D_NMAX - 1) / D_NMAX; }
 static inline int d_nkc(int C) { return ((C / 8) * 9 + KOCT - 1) / KOCT; }
 
 }  // namespace c2m
@@ -624,12 +576,11 @@ extern "C" int c2m_dcn_v2_fused_tc(const c2m_dcn_tc_args *a, c2m_stream_t stream
     p.nkc = d_nkc(a->C); p.nkc_a = p.nkc;
     p.Cout = a->Cout; p.N = d_slice_n(a->Cout); p.nslice = d_n_slice(a->Cout);
     p.tiles_x = ceil_div(a->W, T_C); p.tiles_y = ceil_div(a->H, T_R);
-    p.T = 512 / p.N < MAXT ? 512 / p.N : MAXT;
+    p.T = 1;
     p.n_st = ceil_div(p.tiles_x * p.tiles_y, p.T);
     p.act = a->lrelu ? 2 : 0;
     p.sa_in = 0; p.sa_res = 0; p.sa_out = a->sa_out;
     p.ps = 0;
-    p.stacked = 0;
     p.dbg = 0;
     p.cs = 1;
     p.C8out = (a->Cout + 7) / 8; p.Hout = a->H; p.Wout = a->W;
@@ -641,7 +592,7 @@ extern "C" int c2m_dcn_v2_fused_tc(const c2m_dcn_tc_args *a, c2m_stream_t stream
     q.out_hi = reinterpret_cast<__half *>(a->out_hi); q.out_lo = reinterpret_cast<__half *>(a->out_lo);
     q.out_f32 = a->out_f32;
     DcnTc d;
-    d.policy = 5;      // measured (profiles/r02_dcn_experiments.md): hints change nothing beyond noise; 2 (offsets evict-first) costs 3 %
+    d.policy = 5;      // L2 policies: 1 input map evict-last, 4 streaming output stores
     if (const char *ev = getenv("C2M_DCN_POLICY")) d.policy = atoi(ev);     // tuning experiments
     p.cs = (d.policy & 4) ? 1 : 0;
     if (const char *ev = getenv("C2M_L2_PERSIST_MB")) {                      // experiment: L2 set-aside for evict-last lines
@@ -686,29 +637,37 @@ extern "C" int c2m_dcn_v2_fused_tc(const c2m_dcn_tc_args *a, c2m_stream_t stream
     const size_t w_chunk = (size_t)2 * KOCT * p.N * 16;
     d.nstage = d.L == 1 ? 4 : 8;
     d.nstage_shift = d.L == 1 ? 2 : 3;
-    const size_t fixed = (size_t)d.nstage * A_STAGE + (2 * MAX_NSTAGE + 2 * MAX_NBST + 2 * MAXT) * 8 + 16 + 256 * 4 +
+    const size_t fixed = (size_t)d.nstage * A_STAGE + acc_stage_bytes(p.N) + (2 * MAX_NSTAGE + 2 * MAX_NBST) * 8 + 64 * 4 +
                          2 * MAXT * 16 + (size_t)2 * p.T * d.tab_h * d.tab_w * 8 + 1024 + 128;
     d.nbst = fixed + 4 * w_chunk <= 227 * 1024 ? 4 : 2;
     const size_t smem = fixed + d.nbst * w_chunk;
     C2M_CHECK_ARG(smem <= 227 * 1024, "dcn_v2_fused_tc: %zu bytes of shared memory needed", smem);
-    C2M_CUDA(cudaFuncSetAttribute(dcn_umma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    C2M_CUDA(cudaFuncSetAttribute(dcn_wgmma_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    C2M_CUDA(cudaFuncSetAttribute(dcn_wgmma_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    C2M_CUDA(cudaFuncSetAttribute(dcn_wgmma_kernel<48>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    C2M_CUDA(cudaFuncSetAttribute(dcn_wgmma_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int dev = 0, sms = 0;
     C2M_CUDA(cudaGetDevice(&dev));
     C2M_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     const long long n_work = (long long)a->B * p.tiles_x * p.tiles_y;
     C2M_CHECK_ARG(n_work < (1 << 23), "dcn_v2_fused_tc: too many pixel tiles");
-    // tiles per work item: all T accumulators when there is plenty of work, fewer so that every SM gets an item otherwise
-    d.tg = (int)((n_work + sms - 1) / sms);
-    if (d.tg > p.T) d.tg = p.T;
-    if (d.tg < 1) d.tg = 1;
+    d.tg = 1;
     const int n_items = (int)((n_work + d.tg - 1) / d.tg);
     // SURVEY.md §8(d): flops = 2*B*Cout*C*9*Ho*Wo; bytes = 4*B*(C*H*W + 3*dg*9*H*W + Cout*H*W) + weights
     const double px = (double)a->B * a->H * a->W;
     const double flops = 2.0 * a->Cout * a->C * 9.0 * px;
     const double bytes = 4.0 * px * (a->C + 27.0 * a->dg + a->Cout) + 4.0 * a->Cout * (a->C * 9.0 + 1.0);
     void *ph = prof_begin(PROF_DCN, flops, bytes, st);
-    dcn_umma_kernel<<<n_items < sms ? n_items : sms, NTHREADS, smem, st>>>(q, p, d);
-    C2M_LAUNCH_CHECK("dcn_umma_kernel");
+    const int grid = n_items < sms ? n_items : sms;
+    for (d.slice = 0; d.slice < p.nslice; ++d.slice) {
+        switch (p.N) {
+        case 16: dcn_wgmma_kernel<16><<<grid, NTHREADS, smem, st>>>(q, p, d); break;
+        case 32: dcn_wgmma_kernel<32><<<grid, NTHREADS, smem, st>>>(q, p, d); break;
+        case 48: dcn_wgmma_kernel<48><<<grid, NTHREADS, smem, st>>>(q, p, d); break;
+        default: dcn_wgmma_kernel<64><<<grid, NTHREADS, smem, st>>>(q, p, d); break;
+        }
+        C2M_LAUNCH_CHECK("dcn_wgmma_kernel");
+    }
     prof_end(ph, st);
     return C2M_OK;
 }

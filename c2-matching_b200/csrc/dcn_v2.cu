@@ -1,4 +1,4 @@
-// Fused modulated deformable convolution v2 forward (fp32) for sm_100a.
+// Fused modulated deformable convolution v2 forward (fp32) for sm_90a.
 //
 // Replaces `_ext.dcn_v2_forward` (mmsr/models/archs/DCNv2/src/cuda/dcn_v2_cuda.cu:42-172): the
 // reference writes the whole im2col matrix `columns[B, C*kh*kw, Ho*Wo]` to HBM (0.94 GB per image

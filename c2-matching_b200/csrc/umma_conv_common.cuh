@@ -1,7 +1,7 @@
-// Shared pieces of the tcgen05 implicit-GEMM kernels (plain 3x3 conv, deformable conv):
-// parameter blocks and the epilogue that turns one 128-pixel x N-column TMEM accumulator into
-// packed-split (PSA) and / or strided fp32 output with bias, activation, residuals and an optional
-// fused PixelShuffle(2).
+// Shared pieces of the wgmma implicit-GEMM kernels (plain 3x3 conv, deformable conv):
+// parameter blocks and the epilogue that turns one 128-pixel x N-column accumulator (staged in shared
+// memory, see acc_store) into packed-split (PSA) and / or strided fp32 output with bias, activation, residuals
+// and an optional fused PixelShuffle(2).
 #pragma once
 #include "c2m_common.cuh"
 
@@ -17,9 +17,7 @@ struct ConvParams {
     int act;                  // 0 none, 1 relu, 2 leaky relu 0.1
     int sa_in, sa_res, sa_out;
     int ps;                   // 0 or 2: PixelShuffle(2) applied to the PSA output
-    int stacked;              // 1: accumulator has 2N columns, value = col[c] + col[N + c]
     int dbg;                  // tuning experiments only (C2M_CONV_DBG): 1 = no global stores, 2 = no TMA reloads
-    unsigned w2_off;          // byte offset of the CTA-pair weight layout inside the packed blob
     int cs;                   // 1: PSA output stored with st.global.cs (streaming: the DCN output must not evict the
                               // gathered input map from L2)
     int C8out, Hout, Wout;    // geometry of the PSA output tensor
@@ -42,10 +40,9 @@ struct ConvPtrs {
     const float *add_f32;
 };
 
-// One thread = one output pixel (TMEM lane); `taddr` already carries the lane quarter and the
-// accumulator's first column.
+// One thread = one output pixel; `acc` points at that pixel's row of the staged accumulator.
 // Residual registers of one 32-column block (4 channel octets); fetched by `prefetch_residual`
-// BEFORE the thread blocks on the accumulator / tcgen05.ld, so the HBM/L2 latency of the residual
+// BEFORE the thread waits for the accumulator, so the HBM/L2 latency of the residual
 // overlaps the MMAs instead of being paid once per octet inside the loop.
 struct ResRegs {
     uint4 h[4], l[4];
@@ -69,47 +66,13 @@ __device__ __forceinline__ void prefetch_residual(const __half *rh, const __half
 
 // One 32-column block [c0, c0+32) of the accumulator.  r1: prefetched first residual (or null);
 // a second residual (q.res2_*, rare) is read in place.
-__device__ __forceinline__ void epilogue_store_block(const ConvPtrs &q, const ConvParams &p, uint32_t taddr, int c0, int b,
+__device__ __forceinline__ void epilogue_store_block(const ConvPtrs &q, const ConvParams &p, const float *acc, int c0, int b,
                                                      int y, int x, bool ok, int o_base, const float *sbias,
                                                      float out_scale, float res_scale, float so,
                                                      const ResRegs *r1 = nullptr) {
                     {
                         uint32_t reg[32];
-                        if (p.N - c0 >= 32) {
-                            tmem_ld_32x32(taddr + c0, reg);
-                        } else {   // 16-column tail
-                            asm volatile(
-                                "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-                                "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                                : "=r"(reg[0]), "=r"(reg[1]), "=r"(reg[2]), "=r"(reg[3]), "=r"(reg[4]), "=r"(reg[5]),
-                                  "=r"(reg[6]), "=r"(reg[7]), "=r"(reg[8]), "=r"(reg[9]), "=r"(reg[10]), "=r"(reg[11]),
-                                  "=r"(reg[12]), "=r"(reg[13]), "=r"(reg[14]), "=r"(reg[15])
-                                : "r"(taddr + c0)
-                                : "memory");
-                        }
-                        if (p.stacked) {
-                            // B operand was [W_hi | W_lo] stacked along N: columns c and N + c hold the
-                            // (x * w_hi) and (x * w_lo) partial sums of output channel c
-                            uint32_t reg2[32];
-                            if (p.N - c0 >= 32) {
-                                tmem_ld_32x32(taddr + p.N + c0, reg2);
-                            } else {
-                                asm volatile(
-                                    "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-                                    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                                    : "=r"(reg2[0]), "=r"(reg2[1]), "=r"(reg2[2]), "=r"(reg2[3]), "=r"(reg2[4]), "=r"(reg2[5]),
-                                      "=r"(reg2[6]), "=r"(reg2[7]), "=r"(reg2[8]), "=r"(reg2[9]), "=r"(reg2[10]), "=r"(reg2[11]),
-                                      "=r"(reg2[12]), "=r"(reg2[13]), "=r"(reg2[14]), "=r"(reg2[15])
-                                    : "r"(taddr + p.N + c0)
-                                    : "memory");
-                            }
-                            tmem_ld_wait();
-#pragma unroll
-                            for (int j = 0; j < 32; ++j)
-                                reg[j] = __float_as_uint(__uint_as_float(reg[j]) + __uint_as_float(reg2[j]));
-                        } else {
-                            tmem_ld_wait();
-                        }
+                        acc_ld32(acc, c0, p.N, reg);
                         if (!ok || (p.dbg & 1)) return;
                         const int ncol = min(32, p.N - c0);
                         float v[32];
@@ -220,12 +183,10 @@ __device__ __forceinline__ void epilogue_store_block(const ConvPtrs &q, const Co
 
 // ---------------------------------------------------------------------------------------------------------------
 // Specialised epilogue of one full 32-column block (4 complete channel octets): the generic function above spends
-// ~930 SASS instructions per (warp, tile) on per-element bounds predicates, activation selects and address
-// arithmetic — with it the 8 epilogue warps were busy 87 % of the time while the tensor pipe sat at 57 % (ncu,
-// profiles/r02_conv_epilogue_bound.md).  Here everything that is uniform per launch is a template parameter and the
-// block is straight-line code: ~10 instructions per output element.
+// most of its instructions on per-element bounds predicates, activation selects and address arithmetic.  Here
+// everything that is uniform per launch is a template parameter and the block is straight-line code.
 //   ACT 0 none / 1 ReLU / 2 LeakyReLU(0.1);  RES: one PSA residual (prefetched);  F32OCT: octet-planar fp32 output
-//   instead of PSA;  STACKED: accumulator columns [c, N + c) hold the x*W_hi and x*W_lo partial sums.
+//   instead of PSA.
 // Preconditions (checked by the caller, warp-uniform): c0 + 32 <= N, o_base + c0 + 32 <= Cout, ps == 0, no res2,
 // exactly one output kind.  A PSA output scale 2^sa_out is folded in by the caller: `sbias`, `out_scale` and `res_scale`
 // arrive pre-multiplied by it (ReLU / LeakyReLU commute with a positive scale), so it costs nothing per element.
@@ -244,10 +205,10 @@ __device__ __forceinline__ void prefetch_residual_full(const __half *rh, const _
     }
 }
 
-// The residual octets are fetched BEFORE the thread blocks on the accumulator so their HBM / L2 latency overlaps the
-// MMAs.  Their fp16 -> fp32 conversion does not depend on the accumulator, so the compiler hoists it above the wait —
-// which puts four serialised load round trips in front of every tile (measured: +160 us on a 64->64 @640x640 launch).
-// This no-op "modifies" the registers after the wait, so nothing can consume them earlier.
+// The residual octets are fetched BEFORE the thread waits for the accumulator so their HBM / L2 latency overlaps the
+// MMAs.  Their fp16 -> fp32 conversion does not depend on the accumulator, so the compiler would hoist it above the
+// wait — which puts four serialised load round trips in front of every tile.  This no-op "modifies" the registers
+// after the wait, so nothing can consume them earlier.
 __device__ __forceinline__ void pin_residual(ResRegs &r) {
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -261,21 +222,12 @@ __device__ __forceinline__ float4 lds_f4(const float *p) {
     return v;
 }
 
-template <int ACT, bool RES, bool F32OCT, bool STACKED>
-__device__ __forceinline__ void epilogue_fast_block(const ConvPtrs &q, const ConvParams &p, uint32_t taddr, int c0, int b,
+template <int ACT, bool RES, bool F32OCT>
+__device__ __forceinline__ void epilogue_fast_block(const ConvPtrs &q, const ConvParams &p, const float *acc, int c0, int b,
                                                     int y, int x, bool ok, int o_base, const float *sbias,
                                                     float out_scale, float res_scale, ResRegs *r1) {
     uint32_t reg[32];
-    tmem_ld_32x32(taddr + c0, reg);
-    if (STACKED) {
-        uint32_t reg2[32];
-        tmem_ld_32x32(taddr + p.N + c0, reg2);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 32; ++j) reg[j] = __float_as_uint(__uint_as_float(reg[j]) + __uint_as_float(reg2[j]));
-    } else {
-        tmem_ld_wait();
-    }
+    acc_ld32(acc, c0, c0 + 32, reg);
     if (RES) pin_residual(*r1);
     if (!ok) return;
     const size_t plane = (size_t)p.H * p.W * 8;                       // elements per channel octet
@@ -335,23 +287,22 @@ __device__ __forceinline__ bool epilogue_fast_ok(const ConvPtrs &q, const ConvPa
     return p.ps == 0 && !q.res2_hi && !(p.dbg & 1) && (psa_only || (oct_only && !q.res_hi && p.sa_out == 0));
 }
 
-template <bool STACKED>
-__device__ __forceinline__ void epilogue_fast_dispatch(const ConvPtrs &q, const ConvParams &p, uint32_t taddr, int c0, int b,
+__device__ __forceinline__ void epilogue_fast_dispatch(const ConvPtrs &q, const ConvParams &p, const float *acc, int c0, int b,
                                                        int y, int x, bool ok, int o_base, const float *sbias,
                                                        float out_scale, float res_scale, ResRegs *r1) {
     const bool oct = q.out_f32 != nullptr;
     if (oct) {
-        if (p.act == 0) epilogue_fast_block<0, false, true, STACKED>(q, p, taddr, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, r1);
-        else if (p.act == 1) epilogue_fast_block<1, false, true, STACKED>(q, p, taddr, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, r1);
-        else epilogue_fast_block<2, false, true, STACKED>(q, p, taddr, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, r1);
+        if (p.act == 0) epilogue_fast_block<0, false, true>(q, p, acc, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, r1);
+        else if (p.act == 1) epilogue_fast_block<1, false, true>(q, p, acc, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, r1);
+        else epilogue_fast_block<2, false, true>(q, p, acc, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, r1);
     } else if (r1) {
-        if (p.act == 0) epilogue_fast_block<0, true, false, STACKED>(q, p, taddr, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, r1);
-        else if (p.act == 1) epilogue_fast_block<1, true, false, STACKED>(q, p, taddr, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, r1);
-        else epilogue_fast_block<2, true, false, STACKED>(q, p, taddr, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, r1);
+        if (p.act == 0) epilogue_fast_block<0, true, false>(q, p, acc, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, r1);
+        else if (p.act == 1) epilogue_fast_block<1, true, false>(q, p, acc, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, r1);
+        else epilogue_fast_block<2, true, false>(q, p, acc, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, r1);
     } else {
-        if (p.act == 0) epilogue_fast_block<0, false, false, STACKED>(q, p, taddr, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, r1);
-        else if (p.act == 1) epilogue_fast_block<1, false, false, STACKED>(q, p, taddr, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, r1);
-        else epilogue_fast_block<2, false, false, STACKED>(q, p, taddr, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, r1);
+        if (p.act == 0) epilogue_fast_block<0, false, false>(q, p, acc, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, r1);
+        else if (p.act == 1) epilogue_fast_block<1, false, false>(q, p, acc, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, r1);
+        else epilogue_fast_block<2, false, false>(q, p, acc, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, r1);
     }
 }
 

@@ -241,7 +241,7 @@ def create_dataloader(dataset, dataset_opt, num_gpu=1, dist=False, sampler=None)
     shape are batched (`batch_size`, default 1 = the reference's behaviour), several workers decode ahead — one PAIR
     per worker task (`PairBatcher`; `per_sample_workers: false` restores one batch per worker task)."""
     if dataset_opt.get('phase', 'test') == 'train':
-        raise NotImplementedError('training loaders are outside the B200 hot-path scope')
+        raise NotImplementedError('training loaders are outside the H100 hot-path scope')
     from .data_sampler import ShapeBucketBatchSampler, ShardedEvalSampler
     if sampler is None:
         sampler = ShardedEvalSampler(dataset) if dist else ShardedEvalSampler(dataset, 1, 0)

@@ -60,9 +60,9 @@ class RefCUFEDDataset(data.Dataset):
         super().__init__()
         self.opt = opt
         if (opt.get('io_backend') or {'type': 'disk'}).get('type', 'disk') != 'disk':
-            raise NotImplementedError('only the disk io_backend is supported in the B200 build')
+            raise NotImplementedError('only the disk io_backend is supported in the H100 build')
         if opt.get('phase', 'test') == 'train':
-            raise NotImplementedError('training datasets are outside the B200 hot-path scope')
+            raise NotImplementedError('training datasets are outside the H100 hot-path scope')
         self.paths = []
         with open(opt['ann_file']) as f:       # "<input> <ref>" per line (data/util.py:153-191)
             for line in f:

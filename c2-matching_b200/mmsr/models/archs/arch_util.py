@@ -56,19 +56,19 @@ def fast_conv_enabled():
 
 
 def psa_path_ok(x, *convs, cat_first=32):
-    """True if the tcgen05 3x3 kernel can take over for tensor `x` [B,C,H,W] and these convs.  `cat_first`: channel count of
+    """True if the tensor-core 3x3 kernel can take over for tensor `x` [B,C,H,W] and these convs.  `cat_first`: channel count of
     the FIRST input of the two-input (concatenating) convolutions on the path — the kernel needs a multiple of 32 there."""
     if not (fast_conv_enabled() and x.is_cuda and x.dtype == torch.float32 and not torch.is_grad_enabled()):
         return False
     if x.shape[2] < 18 or x.shape[3] < 10:
-        # not silent: the tcgen05 kernel needs one 18x10 halo tile; smaller maps run the plain modules (cuDNN, exact fp32)
+        # not silent: the tensor-core kernel needs one 18x10 halo tile; smaller maps run the plain modules (cuDNN, exact fp32)
         global _warned_small
         if not _warned_small:
             _warned_small = True
             import logging
             logging.getLogger('base').warning(
                 f'c2m: feature map {x.shape[2]}x{x.shape[3]} is smaller than one halo tile (18x10): the plain 3x3 convolutions '
-                'of this call run on nn.Conv2d (cuDNN, TF32 off), not on the tcgen05 kernel')
+                'of this call run on nn.Conv2d (cuDNN, TF32 off), not on the tensor-core kernel')
         return False
     return all(isinstance(c, nn.Conv2d) and c.kernel_size == (3, 3) and c.stride == (1, 1) and c.padding == (1, 1) and
                c.dilation == (1, 1) and c.groups == 1 and c.weight.is_cuda for c in convs) and cat_first % 32 == 0
@@ -81,7 +81,7 @@ def conv_psa(conv, xp, act=None, **kw):
 
 
 def resblocks_psa(body, hp, final_residual2=None):
-    """Run a Sequential of ResidualBlockNoBN on a packed-split activation (PSA) with the tcgen05
+    """Run a Sequential of ResidualBlockNoBN on a packed-split activation (PSA) with the tensor-core
     3x3 kernel: x + conv2(relu(conv1(x))) per block, two launches per block, no fp32 round trip.
     `final_residual2` is added in the last block's epilogue (the `body(h) + x` skip of
     ref_restoration_arch.py:158,171,184).  Three PSA buffers are cycled."""
@@ -101,7 +101,7 @@ def resblocks_psa(body, hp, final_residual2=None):
 
 
 def body_forward(body, h, skip=None):
-    """body(h) (+ skip) on fp32 tensors: tcgen05 path when supported, else the plain modules."""
+    """body(h) (+ skip) on fp32 tensors: tensor-core path when supported, else the plain modules."""
     from c2m_b200 import ops
     if all(isinstance(b, ResidualBlockNoBN) for b in body) and psa_path_ok(h, body[0].conv1, body[0].conv2):
         out = resblocks_psa(body, ops.psa_from_f32(h))
@@ -134,7 +134,7 @@ def make_layer(block, n_blocks, **kwargs):
 
 def tensor_shift(x, shift=(2, 2), fill_val=0):
     """Shift [b,h,w,c] down/right with constant fill — arch_util.py:291-315.  Kept for API
-    parity; the B200 path builds all shifted offsets in one kernel (csrc/offsets.cu)."""
+    parity; the H100 path builds all shifted offsets in one kernel (csrc/offsets.cu)."""
     sh, sw = shift
     if sh < 0 or sw < 0:
         raise NotImplementedError

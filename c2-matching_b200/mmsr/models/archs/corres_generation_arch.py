@@ -1,10 +1,10 @@
 """Correspondence generation: dense LR<->Ref patch matching -> pre-offsets for the three DCN
 scales, plus VGG19 Ref features (mmsr/models/archs/corres_generation_arch.py:14-117).
 
-B200 path: ONE batched call normalises both feature maps per pixel, runs the fused
-tcgen05 correlation + argmax and the exact rescoring (csrc/corr_*.cu); the reference's Python
+H100 path: ONE batched call normalises both feature maps per pixel, runs the fused
+tensor-core (wgmma) correlation + argmax and the exact rescoring (csrc/corr_*.cu); the reference's Python
 loop over the batch, the 230 MB patch copy and the 2 x 2.09 GB score tensors per image are gone.
-The 9-shift x 3-scale offset pyramid is one small kernel per scale, produced lazily: the B200
+The 9-shift x 3-scale offset pyramid is one small kernel per scale, produced lazily: the H100
 RestorationNet consumes the index map directly and never needs it in HBM."""
 import torch
 from torch import nn

@@ -71,7 +71,7 @@ class DynamicAggregationRestoration(nn.Module):
         return x
 
     def forward_psa(self, xp, pre_offset, img_ref_feat, base):
-        """tcgen05 path: every plain convolution runs in the packed-split layout; `cat` is a
+        """tensor-core path: every plain convolution runs in the packed-split layout; `cat` is a
         two-input convolution, PixelShuffle and the final `+ base` are conv epilogues; only the
         DCN boundary (fp32 offsets/mask in, fp32 features out) leaves the layout."""
         from c2m_b200 import ops
@@ -115,7 +115,7 @@ class RestorationNet(nn.Module):
         base = F.interpolate(x, None, 4, 'bilinear', False)
         ce, dr = self.content_extractor, self.dyn_agg_restore
         # the offset / head convolutions consume cat[content (ngf channels), ref]: ngf must be a multiple of 32 for the
-        # two-input tcgen05 convolution, otherwise the module path below runs
+        # two-input tensor-core convolution, otherwise the module path below runs
         if arch_util.psa_path_ok(x, ce.conv_first, dr.small_offset_conv1, dr.head_small[0], dr.tail_large[2],
                                  cat_first=ce.conv_first.out_channels):
             return dr.forward_psa(ce.forward_psa(x), pre_offset, img_ref_feat, base.contiguous())

@@ -105,7 +105,7 @@ def pretrained_default():
 
 class PackedFeatures(dict):
     """{layer_name: fp32 feature} as the reference's extractor returns (vgg_arch.py:136-145), but the
-    features live in the packed-split operand layout the tcgen05 kernels consume (`.psa(name)`); the
+    features live in the packed-split operand layout the tensor-core kernels consume (`.psa(name)`); the
     fp32 tensor of a layer is produced on first access only (none is, on the fused inference path)."""
 
     def __init__(self, packed):
@@ -153,9 +153,9 @@ class PackedFeatures(dict):
 
 def run_trunk(trunk, x, taps=(), want_last_f32=True, packed_taps=False):
     """Run a named VGG trunk (Sequential of conv / relu / pool).  Returns (last, {tap: fp32}), or
-    (last, PackedFeatures) with packed_taps when the tcgen05 path runs.
+    (last, PackedFeatures) with packed_taps when the tensor-core path runs.
 
-    tcgen05 path: each conv+ReLU pair is one launch in the packed-split layout; a tapped ReLU
+    tensor-core path: each conv+ReLU pair is one launch in the packed-split layout; a tapped ReLU
     output is written both as fp32 (for the DCN sampler / the caller) and packed (attached to the
     fp32 tensor for the next consumer); convs before a max-pool emit fp32 for torch's pooling."""
     from . import arch_util
@@ -266,7 +266,7 @@ class VGGFeatureExtractor(nn.Module):
             self.register_buffer('std', torch.tensor([0.229, 0.224, 0.225]).view(1, 3, 1, 1))
 
     def forward(self, x, packed=False):
-        """packed=True (inference): features stay in the tcgen05 operand layout, fp32 on demand."""
+        """packed=True (inference): features stay in the tensor-core operand layout, fp32 on demand."""
         if self.use_input_norm:
             x = (x - self.mean) / self.std
         _, got = run_trunk(self.vgg_net, x, taps=self.layer_name_list, want_last_f32=False,

@@ -26,14 +26,14 @@ class RefRestorationModel:
     def __init__(self, opt):
         self.opt = opt
         if opt.get('is_train'):
-            raise NotImplementedError('the B200 build covers inference (restoration forward) only')
+            raise NotImplementedError('the H100 build covers inference (restoration forward) only')
         self.is_train = False
         if not torch.cuda.is_available():
-            raise RuntimeError('RefRestorationModel needs a CUDA device: the B200 hot path has no CPU fallback')
+            raise RuntimeError('RefRestorationModel needs a CUDA device: the H100 hot path has no CPU fallback')
         self.device = torch.device('cuda', torch.cuda.current_device())
         path = opt.get('path') or {}
         # parity is stated against the reference's fp32 arithmetic: any convolution that falls back to cuDNN
-        # (maps below the tcgen05 tile size, C2M_FAST_CONV=0) must not run in TF32 (torch's default)
+        # (maps below the tensor-core kernel's tile size, C2M_FAST_CONV=0) must not run in TF32 (torch's default)
         torch.backends.cudnn.allow_tf32 = False
         torch.backends.cuda.matmul.allow_tf32 = False
         # net_map's VGG19 is never loaded from a checkpoint in the reference: it is built with ImageNet weights
@@ -85,7 +85,7 @@ class RefRestorationModel:
         return out
 
     def optimize_parameters(self, step):
-        raise NotImplementedError('training is outside the B200 hot-path scope')
+        raise NotImplementedError('training is outside the H100 hot-path scope')
 
     # -- validation (ref_restoration_model.py:295-370): rank-sharded, batched, host work off the GPU's critical path
     # packed-split activations are fp16 pairs: |x * 2^sa| must stay below 65504 (c2m_b200.ops.PSA)

@@ -1,5 +1,5 @@
 /*
- * libc2m_sm100 — C ABI of the B200-native C2-Matching restoration-forward hot path.
+ * libc2m_sm100 — C ABI of the H100-native C2-Matching restoration-forward hot path.
  *
  * Plain C: raw device pointers, sizes, a CUDA stream handle, int status.  No torch / ATen
  * types.  Every entry point is asynchronous on `stream`, re-entrant (no global scratch: the
@@ -40,7 +40,7 @@ enum {
     C2M_ERR_INVALID = 1,      /* bad shape / argument (reference: AT_ASSERTM -> RuntimeError) */
     C2M_ERR_WORKSPACE = 2,    /* workspace missing or too small */
     C2M_ERR_CUDA = 3,         /* CUDA runtime / launch failure (reference only printf'd these) */
-    C2M_ERR_UNSUPPORTED = 4   /* no sm_100 device / driver entry point missing */
+    C2M_ERR_UNSUPPORTED = 4   /* no sm_90 device / driver entry point missing */
 };
 
 int c2m_abi_version(void);      /* 4 since c2m_dcn_tc_args.x_il / c2m_psa_interleave (3: .mask; 2: out_f32_octets / om_octets) */
@@ -55,8 +55,8 @@ const char *c2m_last_error(void);
  * l2norm != 0 first applies x[:,p] / max(||x[:,p]||, 1e-12) to both maps (the caller's
  * F.normalize in the reference).
  *
- * flags: bit0 = force the generic CUDA-core search instead of the tcgen05 kernel.
- * The tcgen05 search proposes candidates; the returned idx/val always come from the exact
+ * flags: bit0 = force the generic CUDA-core search instead of the tensor-core kernel.
+ * The tensor-core search proposes candidates; the returned idx/val always come from the exact
  * (double-accumulated, float-rounded) rescoring pass, so they do not depend on tensor-core
  * rounding.
  */
@@ -108,7 +108,7 @@ int c2m_dcn_v2_fused_forward_f32(const float *x, const float *om, const float *p
                                  const float *bias, float lrelu_slope, float *out,
                                  const c2m_dcn_shape *shape, c2m_stream_t stream);
 
-/* --- plain 3x3 / stride 1 / pad 1 convolution on tcgen05, fp32-grade (split fp16 x 3) -------
+/* --- plain 3x3 / stride 1 / pad 1 convolution on the tensor cores (wgmma), fp32-grade (split fp16 x 3) -------
  * (SURVEY.md §8f N3: every plain convolution of RestorationNet / the VGG trunks; the reference
  * runs them through cuDNN, e.g. arch_util.py:80-136, ref_restoration_arch.py:147-187.)
  * Activations travel between these convolutions in the packed-split layout "PSA":
@@ -149,7 +149,7 @@ int c2m_psa_interleave(const void *hi, const void *lo, int B, int C, int H, int 
 int c2m_psa_maxpool2(const void *hi, const void *lo, int B, int C, int H, int W, void *out_hi, void *out_lo,
                      c2m_stream_t stream);
 
-/* --- DCNv2 forward on tcgen05 (3x3 / stride 1 / pad 1 / dilation 1, C/dg % 8 == 0, Cout <= 256) ---
+/* --- DCNv2 forward on the tensor cores (wgmma) (3x3 / stride 1 / pad 1 / dilation 1, C/dg % 8 == 0, Cout <= 256) ---
  * Same contract as c2m_dcn_v2_fused_forward_f32 (raw conv_offset_mask output `om`, pre-offsets from
  * `pre` or rebuilt from `idx`), but the contraction runs as a split-fp16 tensor-core GEMM fed by
  * gather warps; the input is a PSA tensor (x_hi / x_lo, see c2m_psa_from_f32): its octet-planar layout

@@ -2,7 +2,7 @@
 
 Everything is drawn from numpy's PCG64 (`np.random.default_rng`), whose stream is
 stable across numpy versions and machines, so the same tensors are rebuilt on the GPU
-box without shipping them.  The reference nets and the B200 nets share state-dict keys
+box without shipping them.  The reference nets and the H100 nets share state-dict keys
 (SURVEY.md §5 "checkpoint"), so filling by *sorted key* gives both the same weights.
 """
 import hashlib

@@ -139,7 +139,7 @@ def dcn_diag():
 
 
 def conv_diag():
-    section('conv3x3 tcgen05 (fp16x3) vs fp64 reference')
+    section('conv3x3 tensor-core (fp16x3) vs fp64 reference')
     import torch.nn.functional as F
     from c2m_b200 import ops
     for (B, cin, cout, H, W, act, res) in ((2, 64, 64, 40, 44, 'relu', False), (1, 64, 64, 37, 29, None, True),

@@ -81,7 +81,7 @@ def test_full_forward_config2_vs_oracle():
     """One pair of BASELINE config 2 (LR 160x160 -> 640x640, Ref 500x500 zero-padded) through the public
     pipeline vs oracle/ref_path.full_forward on the same inputs and weights.  The index map may differ from
     the oracle's only where the two candidates' fp64 scores are closer than 1e-4 (the feature maps come from
-    the tcgen05 convolutions here and from oneDNN there: ~1e-6 apart); given this run's own index map the SR
+    the tensor-core convolutions here and from oneDNN there: ~1e-6 apart); given this run's own index map the SR
     image is within 1e-3 relative of the oracle restoration, and the PSNR (reference metric, against the
     bicubic input as ground-truth proxy) within 0.01 dB of the oracle's end-to-end result."""
     from c2m_b200.pipeline import RestorationPipeline, synthetic_pair

@@ -1,4 +1,4 @@
-"""GPU parity tests proper (-m gpu): the sm_100a kernels, called through the reference-shaped
+"""GPU parity tests proper (-m gpu): the sm_90a kernels, called through the reference-shaped
 boundaries (`_ext`, `feature_match_index`, the arch classes — all of which go through the C ABI),
 against the golden fixtures minted from the unmodified reference and against the oracle.
 
@@ -91,7 +91,7 @@ def test_corr_batched_and_fused_l2norm_matches_per_image_oracle():
 def test_corr_full_size_properties():
     """BASELINE config 2 map size (256 ch, 160x160 vs 160x160) — too big for the CPU oracle in a
     test, so size-independent properties: (1) planted translation is recovered on the interior,
-    (2) the tcgen05 search and the generic CUDA-core search agree bit-for-bit, (3) val is the
+    (2) the tensor-core search and the generic CUDA-core search agree bit-for-bit, (3) val is the
     exact score of idx (recomputed in fp64 for a sample of queries)."""
     import c2m_b200 as c2m
     dy, dx = 5, 9
@@ -192,7 +192,7 @@ def _dcn_case_tensors(case):
 @pytest.mark.parametrize('case', mg.DCN_CASES, ids=[c[0] for c in mg.DCN_CASES])
 def test_ext_dcn_v2_forward_vs_literal_oracle(case, channels_last, route, monkeypatch):
     """B1 boundary.  3x3/s1/p1/d1 shapes with C/dg % 8 == 0 ('wide' here, every DCN of the model) are routed to
-    the tcgen05 kernel (split-fp16 contraction: 2e-5 of the output scale vs the fp64-accumulating oracle);
+    the tensor-core kernel (split-fp16 contraction: 2e-5 of the output scale vs the fp64-accumulating oracle);
     everything else, and everything with C2M_EXT_DCN_TC=0, runs the operation-for-operation FFMA kernel (1e-5)."""
     import _ext
     from c2m_b200 import ops
@@ -389,7 +389,7 @@ def test_validation_gpu_metrics_equal_host_metrics(tmp_path):
     assert len(list((tmp_path / 'synth').glob('*.png'))) == 5
 
 
-# ------------------------------------------------------------------------------- tcgen05 3x3 conv
+# ------------------------------------------------------------------------------- tensor-core 3x3 conv
 @pytest.mark.parametrize('cfg', [(2, 64, 64, 40, 44, 'relu', False), (1, 64, 64, 37, 29, None, True),
                                  (1, 64, 32, 32, 32, 'lrelu', False), (1, 32, 3, 48, 40, None, False),
                                  (2, 3, 64, 32, 24, 'lrelu', False), (1, 24, 40, 33, 21, 'relu', True)],
@@ -429,7 +429,7 @@ def test_resblock_chain_fast_path_equals_module_path():
 
 
 def test_conv3x3_general_modes_vs_fp64():
-    """Generalised tcgen05 conv: two concatenated inputs, >64 output channels (sliced), fused
+    """Generalised tensor-core conv: two concatenated inputs, >64 output channels (sliced), fused
     PixelShuffle(2), fp32 strided output with an added tensor, both outputs at once."""
     from c2m_b200 import ops
     for (B, c1, c2, cout, H, W, act, mode) in ((1, 64, 256, 256, 40, 40, 'lrelu', 'psa'), (2, 64, 128, 128, 24, 40, 'lrelu', 'psa'),
@@ -482,7 +482,7 @@ def _module_path_on_idx(pipe, args, idx_given):
 
 
 def test_fast_conv_path_equals_cudnn_path(monkeypatch):
-    """The whole pipeline with every plain conv on the tcgen05 kernel vs the same pipeline with
+    """The whole pipeline with every plain conv on the tensor-core kernel vs the same pipeline with
     them on exact-fp32 cuDNN (C2M_FAST_CONV=0): same index map, SR within 1e-3 relative."""
     from c2m_b200.pipeline import RestorationPipeline
     sd_e, sd_m, sd_g = _weights()
@@ -500,7 +500,7 @@ def test_fast_conv_path_equals_cudnn_path(monkeypatch):
                                  (1, 256, 256, 8, 20, 20, 1), (1, 32, 48, 4, 18, 11, 1)],
                          ids=lambda c: f'C{c[1]}to{c[2]}_dg{c[3]}')
 def test_dcn_tensor_core_vs_literal_oracle(cfg):
-    """tcgen05 DCN (gather warps + split-fp16 contraction) == the literal C restatement of the
+    """tensor-core DCN (gather warps + split-fp16 contraction) == the literal C restatement of the
     reference kernel (fp64 accumulation), pre-offsets rebuilt from the index map, LeakyReLU fused,
     PSA and fp32 outputs identical."""
     import c2m_b200 as c2m
@@ -669,7 +669,7 @@ def test_cuda_graph_replay_is_bit_identical_to_eager():
 
 
 def test_non_square_pipeline_fast_vs_module_path(monkeypatch):
-    """CUFED5-like non-square pair (LR 84x124 -> 336x496, Ref 300x420 zero-padded): tcgen05 conv/DCN
+    """CUFED5-like non-square pair (LR 84x124 -> 336x496, Ref 300x420 zero-padded): tensor-core conv/DCN
     path vs the cuDNN + FFMA module path give the same index map and SR (ragged tiles on every scale)."""
     from c2m_b200.pipeline import RestorationPipeline
     pipe = RestorationPipeline(DEV).load_state_dicts(*_weights()).place()

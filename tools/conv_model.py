@@ -1,15 +1,17 @@
 """Per-shape bounds for the conv3x3 launches of one step, next to the measured times of
 tools/conv_shapes.py (its log is the argument).  Bounds, all per launch:
-  tensor : 3 x algorithmic flops (hi*hi + hi*lo + lo*hi) at the measured sustained bf16/fp16 rate
-  smem   : the kernel's own operand-fetch model (DESIGN.md K5): per 128-pixel tile, 64-wide Cout slice and K=16
-           step the tensor pipe reads 8 KB (x_hi, [W_hi|W_lo]) + 6 KB (x_lo, W_hi) at ~96 B/clk/SM -> 149 clk
-  hbm    : 4 B per input / output / residual element at the measured copy bandwidth
+  tensor : 3 x algorithmic flops (hi*hi + hi*lo + lo*hi) at the H100 SXM data-sheet dense fp16 rate
+  smem   : operand-fetch model of the wgmma kernel (DESIGN.md K5): per 128-pixel tile, 64-wide Cout slice and K=16
+           step the tensor cores read 8 KB (x_hi, [W_hi|W_lo]) + 6 KB (x_lo, W_hi) from shared memory at
+           128 B/clk/SM -> 112 clk
+  hbm    : 4 B per input / output / residual element at the H100 SXM data-sheet HBM3 bandwidth
+Data-sheet rates are for a 700 W card; a power-limited card reaches less.
 """
 import ast
 import re
 import sys
 
-PEAK_TF, PEAK_GBS, SMS, CLK_GHZ, SMEM_CLK_PER_STEP = 1430.2, 6567.4, 148, 1.80, 149.0
+PEAK_TF, PEAK_GBS, SMS, CLK_GHZ, SMEM_CLK_PER_STEP = 989.0, 3350.0, 132, 1.98, 112.0
 
 rows = []
 for ln in open(sys.argv[1]):

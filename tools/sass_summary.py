@@ -1,10 +1,10 @@
-"""cuobjdump -sass of libc2m_sm100.so -> per-kernel counts of the Blackwell-specific SASS mnemonics
-(B200_PROFILING.md "What proves a Blackwell-native kernel").  usage: python tools/sass_summary.py > profiles/rNN_sass_summary.txt"""
+"""cuobjdump -sass of libc2m_sm100.so -> per-kernel counts of the Hopper-specific SASS mnemonics (wgmma, TMA,
+mbarrier) and of the main memory / FMA instructions.  usage: python tools/sass_summary.py > sass_summary.txt"""
 import collections, os, re, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 lib = os.path.join(ROOT, 'c2-matching_b200', 'lib', 'libc2m_sm100.so')
 out = subprocess.run(['cuobjdump', '-sass', lib], capture_output=True, text=True, check=True).stdout
-WANT = ['UTCHMMA', 'UTCQMMA', 'UTCBAR', 'UTMALDG', 'UTMASTG', 'UBLKCP', 'LDTM', 'STTM', 'UTCATOMSWS', 'SYNCS', 'HMMA', 'HGMMA', 'LDGSTS', 'ELECT',
+WANT = ['HGMMA', 'WARPGROUP', 'UTMALDG', 'UTMASTG', 'UBLKCP', 'SYNCS', 'HMMA', 'LDGSTS', 'ELECT',
         'UCGABAR', 'CCTL', 'SHFL', 'LDG', 'STG', 'LDS', 'STS', 'DFMA', 'FFMA', 'HFMA2']
 cur, counts, total = None, collections.OrderedDict(), collections.Counter()
 for ln in out.splitlines():
@@ -18,12 +18,12 @@ for ln in out.splitlines():
         op = m.group(1)
         total[cur] += 1
         for w in WANT:
-            if op == w or op.startswith(w + '.') or (w in ('UTCHMMA', 'UTMALDG', 'LDTM', 'SYNCS') and op.startswith(w)):
+            if op == w or op.startswith(w + '.') or (w in ('HGMMA', 'WARPGROUP', 'UTMALDG', 'SYNCS') and op.startswith(w)):
                 counts[cur][w] += 1
-print('# SASS instruction counts per kernel of c2-matching_b200/lib/libc2m_sm100.so (sm_100a; cuobjdump -sass, nvcc 12.9)')
-print('# UTCHMMA = tcgen05.mma kind::f16, LDTM = tcgen05.ld, UTMALDG = cp.async.bulk.tensor (TMA load), UBLKCP = cp.async.bulk,')
-print('# UTCBAR = tcgen05.commit, SYNCS = mbarrier ops, ELECT = elect.sync; no HMMA / HGMMA (legacy tensor paths) anywhere\n')
+print('# SASS instruction counts per kernel of c2-matching_b200/lib/libc2m_sm100.so (sm_90a; cuobjdump -sass)')
+print('# HGMMA = wgmma.mma_async, WARPGROUP = wgmma fence / arrive, UTMALDG = cp.async.bulk.tensor (TMA load),')
+print('# UBLKCP = cp.async.bulk, SYNCS = mbarrier ops, ELECT = elect.sync, HMMA = mma.sync\n')
 for k, c in counts.items():
-    if total[k] < 40 and not any(c[w] for w in ('UTCHMMA', 'UTMALDG', 'LDTM')):
+    if total[k] < 40 and not any(c[w] for w in ('HGMMA', 'UTMALDG')):
         continue
     print(f'{k}: {total[k]} instructions; ' + ', '.join(f'{w} {c[w]}' for w in WANT if c[w]))
