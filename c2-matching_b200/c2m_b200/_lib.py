@@ -36,7 +36,7 @@ class ConvArgs(ctypes.Structure):
 
 class DcnTcArgs(ctypes.Structure):
     """c2m_dcn_tc_args (include/c2m_sm100.h)."""
-    _fields_ = [('x_hi', ctypes.c_void_p), ('x_lo', ctypes.c_void_p),
+    _fields_ = [('x_il', ctypes.c_void_p),
                 ('om', ctypes.c_void_p), ('pre', ctypes.c_void_p), ('idx', ctypes.c_void_p),
                 ('gh', ctypes.c_int), ('gw', ctypes.c_int), ('ref_gw', ctypes.c_int), ('pre_scale', ctypes.c_int),
                 ('B', ctypes.c_int), ('C', ctypes.c_int), ('H', ctypes.c_int), ('W', ctypes.c_int),
@@ -45,7 +45,7 @@ class DcnTcArgs(ctypes.Structure):
                 ('out_hi', ctypes.c_void_p), ('out_lo', ctypes.c_void_p), ('sa_out', ctypes.c_int),
                 ('out_f32', ctypes.c_void_p), ('os_b', ctypes.c_longlong), ('os_c', ctypes.c_longlong),
                 ('os_y', ctypes.c_longlong), ('os_x', ctypes.c_longlong), ('om_octets', ctypes.c_int),
-                ('mask', ctypes.c_void_p), ('x_il', ctypes.c_void_p)]
+                ('mask', ctypes.c_void_p)]
 
 
 SYMBOLS = {
@@ -87,7 +87,7 @@ class C2MError(RuntimeError):
     pass
 
 
-EXPECTED_ABI = 4      # c2m_abi_version() the ctypes structs above mirror (include/c2m_sm100.h)
+EXPECTED_ABI = 5      # c2m_abi_version() the ctypes structs above mirror (include/c2m_sm100.h)
 
 
 def lib():

@@ -485,15 +485,11 @@ def dcn_v2_fused_tc(x, om, weight, bias, deformable_group, pre_offset=None, idx=
     elif tuple(om.shape) != (B, 27 * deformable_group, H, W):
         raise RuntimeError(f'conv_offset_mask output has shape {tuple(om.shape)}')
     a = _lib.DcnTcArgs()
-    import os
-    x_il = None
-    if os.environ.get('C2M_DCN_INTERLEAVE', '1') != '0':
-        x_il = psa_interleave(xp)           # kept alive until the launch below is enqueued (same stream)
-        a.x_il = x_il.data_ptr()
+    x_il = psa_interleave(xp)               # kept alive until the launch below is enqueued (same stream)
+    a.x_il = x_il.data_ptr()
     if final_mask is not None:
         final_mask = final_mask.contiguous()
         a.mask = final_mask.data_ptr()
-    a.x_hi, a.x_lo = xp.hi.data_ptr(), xp.lo.data_ptr()
     if om_oct:
         a.om, a.om_octets = om.data.data_ptr(), 1
     else:

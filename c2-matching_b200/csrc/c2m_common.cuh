@@ -54,8 +54,22 @@ void prof_end(void *handle, cudaStream_t st);
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 __host__ __device__ static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
+// number of SMs of the current device (the persistent kernels launch at most one CTA per SM)
+static inline cudaError_t sm_count(int &sms) {
+    int dev = 0;
+    const cudaError_t e = cudaGetDevice(&dev);
+    return e != cudaSuccess ? e : cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+}
+
+// TMA descriptor of a PSA half-plane fp16 [B][C8][H][W][8] as the 4-D tensor (W*8, H, C8, B); one box is
+// box_px pixels x box_rows rows x 4 channel octets of one image.  Out-of-bounds elements load as zero.
+int make_psa_tensor_map(CUtensorMap *map, const void *base, int B, int C8, int H, int W, int box_px, int box_rows);
+
 // ---------------------------------------------------------------------------- device side
 #ifdef __CUDACC__
+// max |x[i]| over n floats, folded into *out_bits (float bits, start at 0); corr_aux.cu
+__global__ void amax_kernel(const float *__restrict__ x, size_t n, unsigned *__restrict__ out_bits);
+
 __device__ __forceinline__ uint32_t smem_u32(const void *p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }

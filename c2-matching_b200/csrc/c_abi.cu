@@ -21,6 +21,33 @@ void set_error(const char *fmt, ...) {
 }
 void count_launch(unsigned n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 
+typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
+                                  const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+int make_psa_tensor_map(CUtensorMap *map, const void *base, int B, int C8, int H, int W, int box_px, int box_rows) {
+    static EncodeTiledFn enc = nullptr;
+    if (!enc) {
+        void *pfn = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &pfn, cudaEnableDefault, &q) != cudaSuccess ||
+            q != cudaDriverEntryPointSuccess) {
+            set_error("cuTensorMapEncodeTiled entry point not available");
+            return C2M_ERR_UNSUPPORTED;
+        }
+        enc = reinterpret_cast<EncodeTiledFn>(pfn);
+    }
+    cuuint64_t dims[4] = {(cuuint64_t)W * 8, (cuuint64_t)H, (cuuint64_t)C8, (cuuint64_t)B};
+    cuuint64_t strides[3] = {(cuuint64_t)W * 16, (cuuint64_t)H * W * 16, (cuuint64_t)C8 * H * W * 16};
+    cuuint32_t box[4] = {(cuuint32_t)box_px * 8, (cuuint32_t)box_rows, 4, 1};
+    cuuint32_t estr[4] = {1, 1, 1, 1};
+    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void *>(base), dims, strides, box, estr,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed with CUresult %d", (int)r); return C2M_ERR_CUDA; }
+    return C2M_OK;
+}
+
 static std::atomic<int> g_profile{0};
 static std::mutex g_prof_mu;
 struct ProfRec { int kernel; double flops, bytes; cudaEvent_t e0, e1; };
@@ -94,7 +121,7 @@ static void carve(CorrWorkspace &ws, const CorrGeom &g, uint8_t *base) {
 
 using namespace c2m;
 
-extern "C" int c2m_abi_version(void) { return 4; }   // 4: c2m_dcn_tc_args.x_il + c2m_psa_interleave; 3: .mask; 2: out_f32_octets / om_octets
+extern "C" int c2m_abi_version(void) { return 5; }   // 5: c2m_dcn_tc_args without x_hi / x_lo; 4: .x_il + c2m_psa_interleave; 3: .mask; 2: out_f32_octets / om_octets
 extern "C" const char *c2m_last_error(void) { return g_err; }
 extern "C" unsigned long long c2m_launch_count(void) { return g_launches.load(); }
 
@@ -127,17 +154,17 @@ extern "C" int c2m_corr_argmax_f32(const float *fin, const float *fref, int B, i
     CorrChunkGeom cg;
     float window_coef;
     const int K = g.C * g.patch * g.patch;
+    int sms = 0;
+    C2M_CUDA(sm_count(sms));
     if (use_umma) {
-        int dev = 0, major = 0, sms = 0;
+        int dev = 0, major = 0;
         C2M_CUDA(cudaGetDevice(&dev));
         C2M_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-        C2M_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
         if (major != 9) {
             set_error("corr_argmax: wgmma path needs an sm_90 device (found sm_%d*)", major);
             return C2M_ERR_UNSUPPORTED;
         }
         ws.nchunk = corr_umma_pick_nchunk(g, sms);
-        if (const char *ev = getenv("C2M_CORR_NCHUNK")) { const int n = atoi(ev); if (n >= 1 && n <= CORR_MAX_CHUNKS) ws.nchunk = n; }   // experiments
         corr_umma_chunk_geom(g, ws.nchunk, cg);
         // DESIGN.md K2: the search scores (q_hi + q_lo) . r_hi.  |approx - exact| <= E = [2^-11 + 2^-22 (K/16 + 3)] ||P_q||
         // ||P_r|| rinv_r: 2^-11 = fp16 rounding of the Ref operand (Cauchy-Schwarz over the patch), K/16 wgmma
@@ -146,9 +173,6 @@ extern "C" int c2m_corr_argmax_f32(const float *fin, const float *fref, int B, i
         // for the accumulation part (x2 of slack for the tensor core's internal alignment).
         window_coef = 1.01f * ldexpf(1.f, -10) + ldexpf(1.f, -20) * (float)((K + 15) / 16 + 3);
     } else {
-        int dev = 0, sms = 0;
-        C2M_CUDA(cudaGetDevice(&dev));
-        C2M_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
         int n = ceil_div(4 * sms, g.B * ceil_div(g.NQ, 64));
         const int ntile = ceil_div(g.NR, 64);
         if (n > CORR_MAX_CHUNKS) n = CORR_MAX_CHUNKS;

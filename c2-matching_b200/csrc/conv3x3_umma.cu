@@ -18,8 +18,6 @@
 // traffic is the activation tile.  Epilogue (one output pixel per thread): *2^-(sa+sw) + bias, ReLU /
 // LeakyReLU, optional residual add (a second PSA tensor), re-split to hi/lo and store — the
 // output is directly the next convolution's operand, no fp32 round trip through HBM.
-#include <cstdlib>
-
 #include "umma_conv_common.cuh"
 
 namespace c2m {
@@ -35,7 +33,6 @@ constexpr int A_STAGE = 2 * A_HALF;       // 23040 B
 constexpr int NBST = 2;                   // weight-chunk double buffer
 constexpr int MAXT = 8;                   // pixel tiles per work item
 constexpr int NMAX = 64;                  // output channels per CTA slice
-constexpr int W_HDR = 256;                // packed-weight blob header bytes
 // activation ring depth: what is left of the 227 KB next to two weight slots and the accumulator staging
 __host__ __device__ constexpr int conv_nstage(int N) { return N >= 64 ? 2 : 4; }
 constexpr size_t conv_smem_bytes(int N) {
@@ -106,7 +103,7 @@ conv3x3_wgmma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
         if (warp == 0) {
             // ================================ activation producer ===============================
             if (lane == 0) {
-                int stage = 0, phase = 0, n_issued = 0;
+                int stage = 0, phase = 0;
                 for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
                     int b, t0, nt, slice;
                     decode(item, b, t0, nt, slice);
@@ -119,14 +116,9 @@ conv3x3_wgmma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
                             const int oct0 = (first ? kc : kc - p.nkc_a) * KOCT;
                             mbar_wait(&empty[stage], phase ^ 1);
                             uint8_t *s = sA + stage * A_STAGE;
-                            if ((p.dbg & 2) && n_issued >= NST) {
-                                mbar_arrive(&full[stage]);                 // experiment: reuse stale tiles
-                            } else {
-                                mbar_arrive_expect_tx(&full[stage], A_STAGE);
-                                tma_load_4d(s, mh, &full[stage], (x0 - 1) * 8, y0 - 1, oct0, b);
-                                tma_load_4d(s + A_HALF, ml, &full[stage], (x0 - 1) * 8, y0 - 1, oct0, b);
-                            }
-                            ++n_issued;
+                            mbar_arrive_expect_tx(&full[stage], A_STAGE);
+                            tma_load_4d(s, mh, &full[stage], (x0 - 1) * 8, y0 - 1, oct0, b);
+                            tma_load_4d(s + A_HALF, ml, &full[stage], (x0 - 1) * 8, y0 - 1, oct0, b);
                             if (++stage == NST) { stage = 0; phase ^= 1; }
                         }
                     }
@@ -351,28 +343,11 @@ __global__ void psa_maxpool2_kernel(const __half *__restrict__ hi, const __half 
     }
 }
 
-__global__ void wamax_kernel(const float *__restrict__ w, int n, unsigned *__restrict__ bits) {
-    float m = 0.f;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) m = fmaxf(m, fabsf(w[i]));
-#pragma unroll
-    for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(bits, __float_as_uint(m));
-}
-
 // blob: [int sw][unsigned amax_bits]...pad to 256 B | [slice][kc][tap][octet][hi|lo][N][8] fp16
 // (hi and lo rows of one octet are adjacent: together they are the 2N-row stacked B operand)
 __global__ void wpack_kernel(const float *__restrict__ w, int Cin, int Cout, int N, int nkc, int nslice,
                              uint8_t *__restrict__ blob) {
-    __shared__ int s_sw;
-    if (threadIdx.x == 0) {
-        const float a = __uint_as_float(reinterpret_cast<unsigned *>(blob)[1]);
-        int e = 0;
-        if (a > 0.f && isfinite(a)) frexpf(a, &e);
-        s_sw = 14 - e;                               // |w| * 2^sw <= 2^14
-        if (blockIdx.x == 0) reinterpret_cast<int *>(blob)[0] = s_sw;
-    }
-    __syncthreads();
-    const float S = ldexpf(1.f, s_sw);
+    const float S = wpack_scale(blob);
     const long long total = (long long)nslice * nkc * 2 * 9 * KOCT * N * 8;
     __half *dst = reinterpret_cast<__half *>(blob + W_HDR);
     for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
@@ -392,34 +367,15 @@ __global__ void wpack_kernel(const float *__restrict__ w, int Cin, int Cout, int
     }
 }
 
-// ------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                  const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static int make_act_map(CUtensorMap *m, const void *base, int B, int C8, int H, int W) {
-    static EncodeTiledFn enc = nullptr;
-    if (!enc) {
-        void *pfn = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &pfn, cudaEnableDefault, &q) != cudaSuccess ||
-            q != cudaDriverEntryPointSuccess) {
-            set_error("cuTensorMapEncodeTiled entry point not available");
-            return C2M_ERR_UNSUPPORTED;
-        }
-        enc = reinterpret_cast<EncodeTiledFn>(pfn);
-    }
-    cuuint64_t dims[4] = {(cuuint64_t)W * 8, (cuuint64_t)H, (cuuint64_t)C8, (cuuint64_t)B};
-    cuuint64_t strides[3] = {(cuuint64_t)W * 16, (cuuint64_t)H * W * 16, (cuuint64_t)C8 * H * W * 16};
-    cuuint32_t box[4] = {(cuuint32_t)A_C * 8, (cuuint32_t)A_R, (cuuint32_t)KOCT, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void *>(base), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed with CUresult %d", (int)r); return C2M_ERR_CUDA; }
+int wpack_header(const float *w, int n, void *packed, cudaStream_t st) {
+    C2M_CUDA(cudaMemsetAsync(packed, 0, W_HDR, st));
+    amax_kernel<<<ceil_div(n, 1024) > 64 ? 64 : ceil_div(n, 1024), 256, 0, st>>>(
+        w, (size_t)n, reinterpret_cast<unsigned *>(packed) + 1);
+    C2M_LAUNCH_CHECK("amax_kernel");
     return C2M_OK;
 }
 
+// ------------------------------------------------------------------------------------------
 static inline int pad16(int c) { return (c + 15) / 16 * 16; }
 static inline int n_kc(int cin) { return ((cin + 7) / 8 + KOCT - 1) / KOCT; }
 static inline int slice_n(int cout) { return cout <= NMAX ? pad16(cout) : NMAX; }
@@ -439,15 +395,10 @@ extern "C" size_t c2m_conv3x3_packed_weight_bytes(int Cin, int Cout) {
 extern "C" int c2m_conv3x3_pack_weights_f32(const float *w, int Cin, int Cout, void *packed, c2m_stream_t stream) {
     C2M_CHECK_ARG(w && packed && Cin > 0 && Cout > 0, "conv3x3_pack_weights: bad argument");
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    C2M_CUDA(cudaMemsetAsync(packed, 0, W_HDR, st));
-    const int n = Cout * Cin * 9;
-    wamax_kernel<<<ceil_div(n, 1024) > 64 ? 64 : ceil_div(n, 1024), 256, 0, st>>>(
-        w, n, reinterpret_cast<unsigned *>(packed) + 1);
-    C2M_LAUNCH_CHECK("wamax_kernel");
+    if (const int rc = wpack_header(w, Cout * Cin * 9, packed, st)) return rc;
     const int N = slice_n(Cout), nkc = n_kc(Cin), ns = n_slice(Cout);
     const long long total = (long long)ns * nkc * 2 * 9 * KOCT * N * 8;
-    const int blocks = (int)((total + 255) / 256 > 592 ? 592 : (total + 255) / 256);
-    wpack_kernel<<<blocks, 256, 0, st>>>(w, Cin, Cout, N, nkc, ns, reinterpret_cast<uint8_t *>(packed));
+    wpack_kernel<<<wpack_blocks(total), 256, 0, st>>>(w, Cin, Cout, N, nkc, ns, reinterpret_cast<uint8_t *>(packed));
     C2M_LAUNCH_CHECK("wpack_kernel");
     return C2M_OK;
 }
@@ -531,21 +482,14 @@ extern "C" int c2m_conv3x3(const c2m_conv3x3_args *a, c2m_stream_t stream) {
     if (a->Cin2) p.nkc_a = a->Cin / (KOCT * 8);
     p.Cout = a->Cout; p.N = slice_n(a->Cout); p.nslice = n_slice(a->Cout);
     p.tiles_x = ceil_div(a->W, T_C); p.tiles_y = ceil_div(a->H, T_R);
-    int dev = 0, sms = 0;
-    C2M_CUDA(cudaGetDevice(&dev));
-    C2M_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    int sms = 0;
+    C2M_CUDA(sm_count(sms));
     p.T = MAXT;
     // small problems (e.g. 64->64 on 160x160 maps): fewer tiles per item so that every SM gets several items
     if ((long long)a->B * p.tiles_x * p.tiles_y * p.nslice / p.T < 3 * sms) p.T = 2;
     // weights that do not stay resident are streamed per (item, K chunk): one tile per item
     if (!(p.nslice == 1 && p.nkc <= NBST)) p.T = 1;
-    if (const char *ev = getenv("C2M_CONV_T")) {          // tuning knob: tiles per work item
-        const int t = atoi(ev);
-        if (t >= 1 && t < p.T) p.T = t;
-    }
-    p.dbg = 0;
     p.cs = 0;
-    if (const char *ev = getenv("C2M_CONV_DBG")) p.dbg = atoi(ev);
     p.n_st = ceil_div(p.tiles_x * p.tiles_y, p.T);
     p.act = a->act; p.sa_in = a->sa_in; p.sa_res = a->sa_res; p.sa_out = a->sa_out;
     p.ps = a->pixel_shuffle;
@@ -566,11 +510,11 @@ extern "C" int c2m_conv3x3(const c2m_conv3x3_args *a, c2m_stream_t stream) {
     q.out_f32 = a->out_f32; q.add_f32 = a->add_f32;
     CUtensorMap mh, ml, m2h, m2l;
     int rc;
-    if ((rc = make_act_map(&mh, a->in_hi, a->B, (a->Cin + 7) / 8, a->H, a->W))) return rc;
-    if ((rc = make_act_map(&ml, a->in_lo, a->B, (a->Cin + 7) / 8, a->H, a->W))) return rc;
+    if ((rc = make_psa_tensor_map(&mh, a->in_hi, a->B, (a->Cin + 7) / 8, a->H, a->W, A_C, A_R))) return rc;
+    if ((rc = make_psa_tensor_map(&ml, a->in_lo, a->B, (a->Cin + 7) / 8, a->H, a->W, A_C, A_R))) return rc;
     if (a->Cin2) {
-        if ((rc = make_act_map(&m2h, a->in2_hi, a->B, (a->Cin2 + 7) / 8, a->H, a->W))) return rc;
-        if ((rc = make_act_map(&m2l, a->in2_lo, a->B, (a->Cin2 + 7) / 8, a->H, a->W))) return rc;
+        if ((rc = make_psa_tensor_map(&m2h, a->in2_hi, a->B, (a->Cin2 + 7) / 8, a->H, a->W, A_C, A_R))) return rc;
+        if ((rc = make_psa_tensor_map(&m2l, a->in2_lo, a->B, (a->Cin2 + 7) / 8, a->H, a->W, A_C, A_R))) return rc;
     } else {
         m2h = mh; m2l = ml;
     }

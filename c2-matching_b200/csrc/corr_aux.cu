@@ -4,9 +4,7 @@
 //
 // Reference semantics restated: mmsr/models/archs/ref_map_util.py:26-86 (feature_match_index) and
 // mmsr/models/archs/corres_generation_arch.py:56-58 (F.normalize over channels).
-#include <cstdio>
 #include <cstdlib>
-#include <vector>
 #include "corr_internal.cuh"
 
 namespace c2m {
@@ -15,6 +13,7 @@ namespace c2m {
 // amax over a whole map (all images) -> scale exponent so that |x| * 2^sexp <= 1024 (fp16-safe
 // with 5 bits of headroom below 65504 and the lo halves far above the subnormal range).
 // ------------------------------------------------------------------------------------------
+// max |x| as float bits (atomicMax on the bits of non-negative floats orders like the values); *out_bits starts at 0
 __global__ void amax_kernel(const float *__restrict__ x, size_t n, unsigned *__restrict__ out_bits) {
     float m = 0.f;
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
@@ -606,23 +605,10 @@ int corr_rescore_launch(const CorrGeom &g, const CorrWorkspace &ws, const CorrCh
                         int is_norm, int norm_input, int64_t *idx, float *val, cudaStream_t st) {
     dim3 grid(ceil_div(g.NQ, 8), g.B);
     const int K = g.Cp * g.patch * g.patch;
-    float e32_coef = ldexpf(1.f, -24) * (float)(K + 8);
-    if (const char *ev = getenv("C2M_RESCORE_PREFILTER")) if (atoi(ev) == 0) e32_coef = 1e30f;     // experiment: prefilter never skips
+    const float e32_coef = ldexpf(1.f, -24) * (float)(K + 8);
     rescore_kernel<<<grid, 256, 0, st>>>(ws.p32_in, ws.p32_ref, ws.part, g, ws.nchunk, window_coef, e32_coef, ws.rinv,
                                          ws.max_pn_bits, is_norm, ws.best, ws.qnorm, ws.ovf, ws.ovf_count);
     C2M_LAUNCH_CHECK("rescore_kernel");
-    if (getenv("C2M_CORR_DEBUG")) {                 // diagnostics only: how many (query, chunk-mask) entries overflowed
-        unsigned n_ovf = 0;
-        cudaStreamSynchronize(st);
-        cudaMemcpy(&n_ovf, ws.ovf_count, sizeof n_ovf, cudaMemcpyDeviceToHost);
-        std::vector<CorrOverflow> h(n_ovf < 4096 ? n_ovf : 4096);
-        if (!h.empty()) cudaMemcpy(h.data(), ws.ovf, h.size() * sizeof(CorrOverflow), cudaMemcpyDeviceToHost);
-        unsigned long long bits = 0;
-        for (auto &e : h) bits += __builtin_popcount(e.chunks);
-        fprintf(stderr, "[c2m corr] queries %d, chunks %d, window_coef %.3e, overflow entries %u (re-scan budget %u), flagged chunks in the first %zu: %llu\n",
-                g.B * g.NQ, ws.nchunk, window_coef, n_ovf, (unsigned)(g.B * g.NQ) / 256u < 64u ? 64u : (unsigned)(g.B * g.NQ) / 256u, h.size(), bits);
-        for (size_t i = 0; i < h.size() && i < 6; ++i) fprintf(stderr, "   q %d mask %08x\n", h[i].query, h[i].chunks);
-    }
     // fp32 prefilter of the re-scan: query patch in shared memory when it fits (it does for every model shape)
     const int qs_floats = K * 4 <= 48 * 1024 ? K : 0;
     // Budget of the exhaustive pass.  On inputs whose scores are flooded with near-ties (flat or very smooth images: most

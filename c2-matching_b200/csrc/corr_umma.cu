@@ -252,37 +252,6 @@ corr_umma_kernel(const __grid_constant__ CUtensorMap tm_in_hi, const __grid_cons
 // ------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                  const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode_fn() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void *p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn>(p);
-    }
-    return fn;
-}
-
-// map [B][C8][H][W][8] fp16 as a 4-D tensor (W*8, H, C8, B) with a (16 px * 8, rows, KOCT, 1) box
-static int make_map(CUtensorMap *m, const __half *base, int B, int C8, int H, int W, int rows) {
-    EncodeTiledFn enc = get_encode_fn();
-    if (!enc) { set_error("cuTensorMapEncodeTiled entry point not available"); return C2M_ERR_UNSUPPORTED; }
-    cuuint64_t dims[4] = {(cuuint64_t)W * 8, (cuuint64_t)H, (cuuint64_t)C8, (cuuint64_t)B};
-    cuuint64_t strides[3] = {(cuuint64_t)W * 16, (cuuint64_t)H * W * 16, (cuuint64_t)C8 * H * W * 16};
-    cuuint32_t box[4] = {(cuuint32_t)BW * 8, (cuuint32_t)rows, (cuuint32_t)KOCT, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half *>(base), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed with CUresult %d", (int)r); return C2M_ERR_CUDA; }
-    return C2M_OK;
-}
-
 bool corr_umma_supported(const CorrGeom &g) {
     return g.patch == PATCH && g.s_in == 1 && g.s_ref == 1 && g.w >= BW && g.h >= A_R && g.wr >= BW &&
            g.hr >= B_R;
@@ -330,9 +299,9 @@ int corr_search_umma_launch(const CorrGeom &g, const CorrWorkspace &ws, cudaStre
     CUtensorMap tih, til, trh;
     const int C8 = g.Cp / 8;
     int rc;
-    if ((rc = make_map(&tih, ws.hi_in, g.B, C8, g.h, g.w, A_R))) return rc;
-    if ((rc = make_map(&til, ws.lo_in, g.B, C8, g.h, g.w, A_R))) return rc;
-    if ((rc = make_map(&trh, ws.hi_ref, g.B, C8, g.hr, g.wr, B_R))) return rc;
+    if ((rc = make_psa_tensor_map(&tih, ws.hi_in, g.B, C8, g.h, g.w, BW, A_R))) return rc;
+    if ((rc = make_psa_tensor_map(&til, ws.lo_in, g.B, C8, g.h, g.w, BW, A_R))) return rc;
+    if ((rc = make_psa_tensor_map(&trh, ws.hi_ref, g.B, C8, g.hr, g.wr, BW, B_R))) return rc;
 
     UmmaParams p;
     p.B = g.B; p.C8 = C8;
@@ -345,9 +314,8 @@ int corr_search_umma_launch(const CorrGeom &g, const CorrWorkspace &ws, cudaStre
 
     // per launch: the attribute belongs to the (device, context) pair, not to the process
     C2M_CUDA(cudaFuncSetAttribute(corr_umma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    int dev = 0, sms = 0;
-    C2M_CUDA(cudaGetDevice(&dev));
-    C2M_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    int sms = 0;
+    C2M_CUDA(sm_count(sms));
     const int n_items = g.B * p.qt_x * p.qt_y * p.nchunk;
     const int grid = n_items < sms ? n_items : sms;
     corr_umma_kernel<<<grid, 512, SMEM_BYTES, st>>>(tih, til, trh, ws.rinv, ws.sexp, ws.part, p);

@@ -14,9 +14,9 @@
 //   (g, tap) pair), L = min(C/dg/8, 4): the sampling point — raw conv_offset_mask output + pre-offset, sigmoid
 //   mask, the 4 corner offsets and mask-folded bilinear weights — is computed ONCE per (pixel, g, tap) and reused
 //   for the run's octets; for L > 1 the 4 thread groups work on L consecutive stages concurrently.  Per octet:
-//   16 B (hi) + 16 B (lo) per corner from the octet-planar PSA input (L2 evict-last: the input map is re-read by all
-//   nine taps and must stay resident, while offsets / outputs stream through with evict-first), blended (hi halves
-//   in fp32, lo halves in packed fp16), split and stored with one 16 B st.shared per half;
+//   16 B (hi) + 16 B (lo) per corner, adjacent in the hi/lo-interleaved PSA input (L2 evict-last: the input map is
+//   re-read by all nine taps and must stay resident, while offsets bypass L1 and outputs use streaming stores),
+//   blended (hi halves in fp32, lo halves in packed fp16), split and stored with one 16 B st.shared per half;
 //   fence.proxy.async + mbarrier hand the stage to the MMA warpgroup.
 //   Pre-offsets: per tile the index-map cells it can touch ((16/s + 2) x (8/s + 2)) are decoded once into a
 //   shared-memory flow table, so the per-(pixel, tap) pre-offset is one ld.shared instead of an 8-byte global
@@ -26,8 +26,6 @@
 //   wider layers take one launch per slice.  The epilogue (bias, LeakyReLU, PSA and / or fp32 store) is shared
 //   with the plain convolution.
 // The im2col matrix never exists outside shared memory.
-#include <cstdlib>
-
 #include "umma_conv_common.cuh"
 
 namespace c2m {
@@ -40,14 +38,11 @@ constexpr int A_HALF = KOCT * A_OCT_B;     // 8192 B
 constexpr int A_STAGE = 2 * A_HALF;        // 16384 B
 constexpr int MAX_NSTAGE = 8;
 constexpr int MAX_NBST = 4;
-constexpr int MAXT = 8;
 constexpr int NGATHER_WARPS = 16;
 constexpr int NTHREADS = 256 + 32 * NGATHER_WARPS;
-constexpr int W_HDR = 256;
 
 struct DcnTc {
-    const __half *x_hi, *x_lo; // input in the packed-split layout [B][C/8][H][W][8] (value = hi + lo)
-    const __half *x_il;        // or (non-null) the same values interleaved [B][C/8][H][W][hi 8 | lo 8]: one sector per corner
+    const __half *x_il;        // input, packed-split and hi/lo-interleaved [B][C/8][H][W][hi 8 | lo 8] (value = hi + lo)
     int C8;
     const float *om;           // [B, 3*dg*9, H, W], or octet-planar [B][om_c8][H][W][8] when om_c8 > 0
     int om_c8;
@@ -62,9 +57,7 @@ struct DcnTc {
     int opp_shift;             // log2(opp) when opp is a power of two, else -1 (then L == 1)
     int nstage, nbst;          // ring depths (activation stages, weight chunks); powers of two
     int nstage_shift;          // log2(nstage)
-    int tg;                    // pixel tiles per work item (1: the accumulator lives in registers)
     int slice;                 // 64-wide output-channel slice this launch computes
-    int policy;                // L2 policies: 1 = input map evict-last, 2 = offsets / mask evict-first, 4 = streaming output stores
     int sc_shift;              // log2(pre_scale) when the flow table is used (idx given, scale in {1,2,4,8}), else -1
     int tab_h, tab_w;          // flow-table cells per tile: 16/s + 2, 8/s + 2
     float inv_ref_gw, inv_scale;   // reciprocals for the exact float-assisted integer divisions
@@ -90,11 +83,6 @@ __device__ __forceinline__ uint64_t l2_policy_evict_last() {
 __device__ __forceinline__ uint64_t l2_policy_evict_normal() {
     uint64_t p;
     asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(p));
-    return p;
-}
-__device__ __forceinline__ uint64_t l2_policy_evict_first() {
-    uint64_t p;
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
     return p;
 }
 __device__ __forceinline__ uint4 ldg_keep_v4(const void *ptr, uint64_t pol) {
@@ -133,18 +121,15 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
     uint64_t *bars = reinterpret_cast<uint64_t *>(reinterpret_cast<uint8_t *>(acc_s) + acc_stage_bytes(N));
     uint64_t *full = bars, *empty = full + MAX_NSTAGE, *bfull = empty + MAX_NSTAGE, *bempty = bfull + MAX_NBST;
     float *sbias = reinterpret_cast<float *>(bempty + MAX_NBST);                  // [N <= 64], 16 B aligned
-    int4 *tile_info = reinterpret_cast<int4 *>(sbias + 64);                       // [2][MAXT] (b, y0, x0, image pixel base)
-    float2 *flow_tab = reinterpret_cast<float2 *>(tile_info + 2 * MAXT);          // [2][T][tab_h * tab_w]
+    int4 *tile_info = reinterpret_cast<int4 *>(sbias + 64);                       // [2] (b, y0, x0, image pixel base)
+    float2 *flow_tab = reinterpret_cast<float2 *>(tile_info + 2);                 // [2][tab_h * tab_w]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tiles_img = p.tiles_x * p.tiles_y;
     // Work = flat list of (image, pixel tile), one tile per item (its accumulator lives in the MMA warpgroup's
     // registers); item i runs on CTA i % grid, so at any moment the CTAs work on ~grid CONSECUTIVE tiles and the
     // gathered input map of ONE image is what has to stay in L2, not the whole batch.
-    const int TT = p.B * tiles_img;
-    const int n_work = TT;
-    const int Tg = d.tg;
-    const int n_items = (n_work + Tg - 1) / Tg;
+    const int n_items = p.B * tiles_img;
     const int nstage_mask = d.nstage - 1;                // ring depths are powers of two
 
     if (warp == 1 && lane == 0) {
@@ -154,11 +139,6 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
     }
     __syncthreads();
     const int sw = *reinterpret_cast<const int *>(q.wblob);
-
-    auto group = [&](int item, int &pos, int &nt) {
-        pos = item * Tg;
-        nt = min(Tg, n_work - pos);
-    };
 
     // Register budget per warpgroup.  The CTA's pool is what it was launched with (80 x 768 = 61440):
     // the control warpgroup gives 56 x 128 back and the MMA / epilogue warpgroup takes them,
@@ -170,8 +150,6 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
         if (lane == 0) {
             int bst = 0, bphase = 0;
             for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-                int pos, nt;
-                group(item, pos, nt);
                 for (int kc = 0; kc < p.nkc; ++kc) {
                     mbar_wait(&bempty[bst], bphase ^ 1);
                     mbar_arrive_expect_tx(&bfull[bst], w_chunk);
@@ -201,9 +179,7 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
         constexpr uint32_t b_lbo = N * 16;
         int stage = 0, phase = 0, bst = 0, bphase = 0;
         for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-            int pos, nt;
-            group(item, pos, nt);
-            const int b = pos / tiles_img, tt = pos - b * tiles_img;
+            const int b = item / tiles_img, tt = item - b * tiles_img;
             const int y = (tt / p.tiles_x) * T_R + e / T_C, x = (tt % p.tiles_x) * T_C + e % T_C;
             const bool ok = y < p.H && x < p.W;
             float acc0[N / 2], acc1[N / 2];                 // rows [0, 64) and [64, 128)
@@ -259,8 +235,8 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
         const int sg = grp / NS, slot = grp - sg * NS;
         const int P = p.H * p.W, W8 = p.W * 8;
         const int mrow = m / T_C, mcol = m % T_C;
-        const uint64_t pol_keep = (d.policy & 1) ? l2_policy_evict_last() : l2_policy_evict_normal();
-        const uint64_t pol_stream = (d.policy & 2) ? l2_policy_evict_first() : l2_policy_evict_normal();
+        const uint64_t pol_keep = l2_policy_evict_last();
+        const uint64_t pol_stream = l2_policy_evict_normal();
         const int x_img = d.C8 * P * 8;                       // elements per image of one operand half (< 2^31, host-checked)
         const int om_img = (d.om_c8 > 0 ? d.om_c8 * 8 : (d.mask ? 2 : 3) * d.dg * 9) * P;
         const int om_mask_base = 2 * d.dg * 9;
@@ -270,36 +246,26 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
         const float Hf = (float)p.H, Wf = (float)p.W;
         struct Meta { float off_h, off_w, mr; };
         int ring = 0;                                       // stages issued by this CTA so far (all groups agree)
-        int gi = 0;                                         // tile-group counter (table double buffer)
+        int gi = 0;                                         // item counter (double buffer of tile info and table)
         for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++gi) {
-            int r0g, nt;                                    // (image, tile) index of the group's first tile, tiles
-            group(item, r0g, nt);
-            const int n_steps = p.nkc * nt;
-            int4 *tinfo = tile_info + (gi & 1) * MAXT;
-            float2 *tab = flow_tab + (gi & 1) * p.T * tab_n;
+            int4 *tinfo = tile_info + (gi & 1);
+            float2 *tab = flow_tab + (gi & 1) * tab_n;
 
-            // ---- per tile group: tile origins and the decoded flow of every index-map cell a tile can touch
-            if (g_tid < nt) {
-                const int r = r0g + g_tid;
-                const int b = r / tiles_img, tt = r - b * tiles_img;
-                const int ty = tt / p.tiles_x;
-                tinfo[g_tid] = make_int4(b, ty * T_R, (tt - ty * p.tiles_x) * T_C, 0);
-            }
+            // ---- per item: the tile origin and the decoded flow of every index-map cell the tile can touch
+            const int tb = item / tiles_img, tt = item - tb * tiles_img;
+            const int ty = tt / p.tiles_x, tx = tt - ty * p.tiles_x;
+            if (g_tid == 0) *tinfo = make_int4(tb, ty * T_R, tx * T_C, 0);
             if (d.sc_shift >= 0) {
-                for (int i = g_tid; i < nt * tab_n; i += 32 * NGATHER_WARPS) {
-                    const int t = i / tab_n, c = i - t * tab_n;
-                    const int r = r0g + t;
-                    const int b = r / tiles_img, tt = r - b * tiles_img;
-                    const int ty = tt / p.tiles_x, tx = tt - ty * p.tiles_x;
+                for (int c = g_tid; c < tab_n; c += 32 * NGATHER_WARPS) {
                     const int cy = c / d.tab_w, cx = c - cy * d.tab_w;
                     const int acy = ((ty * T_R) >> d.sc_shift) - 2 + cy, acx = ((tx * T_C) >> d.sc_shift) - 2 + cx;
                     float2 fl = make_float2(0.f, 0.f);
                     if (acy >= 0 && acx >= 0 && acy < d.gh && acx < d.gw) {
-                        const int v = (int)d.idx[((long long)b * d.gh + acy) * d.gw + acx];
+                        const int v = (int)d.idx[((long long)tb * d.gh + acy) * d.gw + acx];
                         const int vy = fast_div(v, d.ref_gw, d.inv_ref_gw), vx = v - vy * d.ref_gw;
                         fl = make_float2((float)((vx - acx) << d.sc_shift), (float)((vy - acy) << d.sc_shift));   // (x, y)
                     }
-                    tab[i] = fl;
+                    tab[c] = fl;
                 }
             }
             asm volatile("bar.sync 2, 512;" ::: "memory");
@@ -332,14 +298,14 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
                 c_xoff = (g * d.opp + (ko - (d.opp_shift >= 0 ? (pair << d.opp_shift) : pair * d.opp))) * P * 8;
             };
 
-            // ---- metadata of unit (kc, t): raw offsets (+ pre-offset) and mask logit of this thread's pixel
-            auto fetch = [&](int kc, int t, bool in_range, Meta &mt, int &y_out, int &x_out, int &b_out, bool &live) {
+            // ---- metadata of K chunk kc: raw offsets (+ pre-offset) and mask logit of this thread's pixel
+            auto fetch = [&](int kc, bool in_range, Meta &mt, int &y_out, int &x_out, int &b_out, bool &live) {
                 mt.off_h = mt.off_w = mt.mr = 0.f;
                 y_out = x_out = b_out = 0;
                 live = false;
                 if (!in_range) return;
                 if (kc != c_kc) set_kc(kc);
-                const int4 ti = tinfo[t];
+                const int4 ti = *tinfo;
                 const int b = ti.x, y = ti.y + mrow, xx = ti.z + mcol;
                 live = c_valid && y < p.H && xx < p.W;
                 y_out = y; x_out = xx; b_out = b;
@@ -362,7 +328,7 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
                     mt.off_w += pq.x;
                     mt.off_h += pq.y;
                 } else if (d.sc_shift >= 0) {
-                    const float2 fl = tab[t * tab_n + cell0 - c_tapcell];
+                    const float2 fl = tab[cell0 - c_tapcell];
                     mt.off_w += fl.x;
                     mt.off_h += fl.y;
                 } else if (d.idx) {                       // scales the table does not cover: decode in place
@@ -380,16 +346,12 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
                 }
             };
 
-            // my units of this group: steps sg, sg + NG, ...; (kc, t) advanced incrementally
-            int kc = 0, t = sg;
-            while (t >= nt) { t -= nt; ++kc; }
+            // my K chunks of this item: sg, sg + NG, ...
             Meta mt, nx;
             int y, ny, xx, nxx, b, nb;
             bool lv, nlv;
-            fetch(kc, t, sg < n_steps, mt, y, xx, b, lv);
-            for (int step = sg; step < n_steps; step += NG) {
-                int nkc_ = kc, nt_ = t + NG;
-                while (nt_ >= nt) { nt_ -= nt; ++nkc_; }
+            fetch(sg, sg < p.nkc, mt, y, xx, b, lv);
+            for (int kc = sg; kc < p.nkc; kc += NG) {
                 // ---- sampling point of the unit's (pixel, g, tap): dcn_v2_im2col_cuda.cu:25-54,172-190
                 int o0 = 0, o1 = 0, o2 = 0, o3 = 0;
                 float w0 = 0.f, w1 = 0.f, w2 = 0.f, w3 = 0.f;
@@ -413,34 +375,26 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
                         if (bv && rv) { o3 = r0 + W8 + 8; w3 = ml * lw; }
                     }
                 }
-                const __half *xh = d.x_hi + (size_t)b * x_img + (lv ? xoff : 0);
-                const __half *xl = d.x_lo + (size_t)b * x_img + (lv ? xoff : 0);
                 const __half2 wh0 = __float2half2_rn(w0), wh1 = __float2half2_rn(w1), wh2 = __float2half2_rn(w2),
                               wh3 = __float2half2_rn(w3);
-                const int stage_idx = ring + step;
+                const int stage_idx = ring + kc;
                 const int rs = stage_idx & nstage_mask;
                 const uint32_t rphase = (uint32_t)(stage_idx >> d.nstage_shift) & 1u;
                 uint8_t *sdst = sA + rs * A_STAGE + (slot * L) * A_OCT_B + m * 16;
                 // next unit's metadata goes out before this unit's corner fetches come back
-                fetch(nkc_, nt_, step + NG < n_steps, nx, ny, nxx, nb, nlv);
+                fetch(kc + NG, kc + NG < p.nkc, nx, ny, nxx, nb, nlv);
 #pragma unroll 1
                 for (int u = 0; u < L; ++u) {
                     // octet-planar operand: the 32 lanes of a warp (4 rows x 8 pixels) read 16 B each from runs of
                     // adjacent pixels (8 lines per request instead of 32 with a channels-last fp32 input)
                     const int po = u * P * 8;
                     uint4 ch0, ch1, ch2, ch3, cl0, cl1, cl2, cl3;
-                    if (d.x_il) {                          // element offsets double in the interleaved operand
-                        const __half *xi = d.x_il + 2 * ((size_t)b * x_img + (lv ? xoff : 0) + po);
-                        ldg_keep_v8(xi + 2 * o0, pol_keep, ch0, cl0);
-                        ldg_keep_v8(xi + 2 * o1, pol_keep, ch1, cl1);
-                        ldg_keep_v8(xi + 2 * o2, pol_keep, ch2, cl2);
-                        ldg_keep_v8(xi + 2 * o3, pol_keep, ch3, cl3);
-                    } else {
-                        ch0 = ldg_keep_v4(xh + po + o0, pol_keep); ch1 = ldg_keep_v4(xh + po + o1, pol_keep);
-                        ch2 = ldg_keep_v4(xh + po + o2, pol_keep); ch3 = ldg_keep_v4(xh + po + o3, pol_keep);
-                        cl0 = ldg_keep_v4(xl + po + o0, pol_keep); cl1 = ldg_keep_v4(xl + po + o1, pol_keep);
-                        cl2 = ldg_keep_v4(xl + po + o2, pol_keep); cl3 = ldg_keep_v4(xl + po + o3, pol_keep);
-                    }
+                    // element offsets double in the interleaved operand
+                    const __half *xi = d.x_il + 2 * ((size_t)b * x_img + (lv ? xoff : 0) + po);
+                    ldg_keep_v8(xi + 2 * o0, pol_keep, ch0, cl0);
+                    ldg_keep_v8(xi + 2 * o1, pol_keep, ch1, cl1);
+                    ldg_keep_v8(xi + 2 * o2, pol_keep, ch2, cl2);
+                    ldg_keep_v8(xi + 2 * o3, pol_keep, ch3, cl3);
                     // ---- blend, modulate, split.  value = hi + lo: the hi halves are blended in fp32, the lo halves
                     // (|lo| <= 2^-11 |value|) in packed fp16 — their rounding lands at 2^-22 of the value
                     const __half2 *hp0 = reinterpret_cast<const __half2 *>(&ch0), *hp1 = reinterpret_cast<const __half2 *>(&ch1);
@@ -473,10 +427,8 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&full[rs]);
                 mt = nx; lv = nlv; y = ny; xx = nxx; b = nb;
-                kc = nkc_;
-                t = nt_;
             }
-            ring += n_steps;
+            ring += p.nkc;
         }
     }
 
@@ -485,16 +437,7 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
 // blob: header | [slice][kc][hi|lo][octet 4][N][8], K ordered (g, tap, channel-in-group)
 __global__ void dcn_wpack_kernel(const float *__restrict__ w, int C, int Cout, int dg, int N, int nkc, int nslice,
                                  uint8_t *__restrict__ blob) {
-    __shared__ int s_sw;
-    if (threadIdx.x == 0) {
-        const float a = __uint_as_float(reinterpret_cast<unsigned *>(blob)[1]);
-        int e = 0;
-        if (a > 0.f && isfinite(a)) frexpf(a, &e);
-        s_sw = 14 - e;
-        if (blockIdx.x == 0) reinterpret_cast<int *>(blob)[0] = s_sw;
-    }
-    __syncthreads();
-    const float S = ldexpf(1.f, s_sw);
+    const float S = wpack_scale(blob);
     const int cpg = C / dg, opp = cpg / 8, n_ko = (C / 8) * 9;
     const long long total = (long long)nslice * nkc * 2 * KOCT * N * 8;
     __half *dst = reinterpret_cast<__half *>(blob + W_HDR);
@@ -516,14 +459,6 @@ __global__ void dcn_wpack_kernel(const float *__restrict__ w, int C, int Cout, i
         const __half hh = __float2half_rn(v);
         dst[e] = half ? __float2half_rn(v - __half2float(hh)) : hh;
     }
-}
-
-__global__ void dcn_wamax_kernel(const float *__restrict__ w, int n, unsigned *__restrict__ bits) {
-    float m = 0.f;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) m = fmaxf(m, fabsf(w[i]));
-#pragma unroll
-    for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(bits, __float_as_uint(m));
 }
 
 static inline int d_pad16(int c) { return (c + 15) / 16 * 16; }
@@ -550,21 +485,17 @@ extern "C" int c2m_dcn_tc_pack_weights_f32(const float *w, int C, int Cout, int 
     C2M_CHECK_ARG(w && packed, "dcn_tc_pack_weights: null pointer");
     C2M_CHECK_ARG(c2m_dcn_tc_supported(C, Cout, dg), "dcn_tc_pack_weights: C=%d dg=%d unsupported (C/dg must be a multiple of 8)", C, dg);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    C2M_CUDA(cudaMemsetAsync(packed, 0, W_HDR, st));
-    const int n = Cout * C * 9;
-    dcn_wamax_kernel<<<ceil_div(n, 1024) > 64 ? 64 : ceil_div(n, 1024), 256, 0, st>>>(w, n, reinterpret_cast<unsigned *>(packed) + 1);
-    C2M_LAUNCH_CHECK("dcn_wamax_kernel");
+    if (const int rc = wpack_header(w, Cout * C * 9, packed, st)) return rc;
     const int N = d_slice_n(Cout), nkc = d_nkc(C), ns = d_n_slice(Cout);
     const long long total = (long long)ns * nkc * 2 * KOCT * N * 8;
-    const int blocks = (int)((total + 255) / 256 > 592 ? 592 : (total + 255) / 256);
-    dcn_wpack_kernel<<<blocks, 256, 0, st>>>(w, C, Cout, dg, N, nkc, ns, reinterpret_cast<uint8_t *>(packed));
+    dcn_wpack_kernel<<<wpack_blocks(total), 256, 0, st>>>(w, C, Cout, dg, N, nkc, ns, reinterpret_cast<uint8_t *>(packed));
     C2M_LAUNCH_CHECK("dcn_wpack_kernel");
     return C2M_OK;
 }
 
 extern "C" int c2m_dcn_v2_fused_tc(const c2m_dcn_tc_args *a, c2m_stream_t stream) {
-    C2M_CHECK_ARG(a && ((a->x_hi && a->x_lo) || a->x_il) && a->om && a->packed_w, "dcn_v2_fused_tc: null pointer");
-    C2M_CHECK_ARG(!a->x_il || (reinterpret_cast<uintptr_t>(a->x_il) & 31) == 0, "dcn_v2_fused_tc: x_il must be 32 B aligned");
+    C2M_CHECK_ARG(a && a->x_il && a->om && a->packed_w, "dcn_v2_fused_tc: null pointer");
+    C2M_CHECK_ARG((reinterpret_cast<uintptr_t>(a->x_il) & 31) == 0, "dcn_v2_fused_tc: x_il must be 32 B aligned");
     C2M_CHECK_ARG(a->B > 0 && a->H > 0 && a->W > 0, "dcn_v2_fused_tc: bad shape");
     C2M_CHECK_ARG(c2m_dcn_tc_supported(a->C, a->Cout, a->dg), "dcn_v2_fused_tc: C=%d dg=%d unsupported", a->C, a->dg);
     C2M_CHECK_ARG(!(a->pre == nullptr && a->idx != nullptr) || (a->gh > 0 && a->gw > 0 && a->ref_gw > 0 && a->pre_scale > 0),
@@ -576,13 +507,10 @@ extern "C" int c2m_dcn_v2_fused_tc(const c2m_dcn_tc_args *a, c2m_stream_t stream
     p.nkc = d_nkc(a->C); p.nkc_a = p.nkc;
     p.Cout = a->Cout; p.N = d_slice_n(a->Cout); p.nslice = d_n_slice(a->Cout);
     p.tiles_x = ceil_div(a->W, T_C); p.tiles_y = ceil_div(a->H, T_R);
-    p.T = 1;
-    p.n_st = ceil_div(p.tiles_x * p.tiles_y, p.T);
     p.act = a->lrelu ? 2 : 0;
     p.sa_in = 0; p.sa_res = 0; p.sa_out = a->sa_out;
     p.ps = 0;
-    p.dbg = 0;
-    p.cs = 1;
+    p.cs = 1;          // streaming output stores: the outputs must not evict the gathered input map from L2
     p.C8out = (a->Cout + 7) / 8; p.Hout = a->H; p.Wout = a->W;
     p.os_b = a->os_b; p.os_c = a->os_c; p.os_y = a->os_y; p.os_x = a->os_x;
     p.f32_mode = a->out_f32 ? f32_store_mode(a->out_f32, nullptr, a->os_b, a->os_c, a->os_y, a->os_x) : 0;
@@ -592,16 +520,7 @@ extern "C" int c2m_dcn_v2_fused_tc(const c2m_dcn_tc_args *a, c2m_stream_t stream
     q.out_hi = reinterpret_cast<__half *>(a->out_hi); q.out_lo = reinterpret_cast<__half *>(a->out_lo);
     q.out_f32 = a->out_f32;
     DcnTc d;
-    d.policy = 5;      // L2 policies: 1 input map evict-last, 4 streaming output stores
-    if (const char *ev = getenv("C2M_DCN_POLICY")) d.policy = atoi(ev);     // tuning experiments
-    p.cs = (d.policy & 4) ? 1 : 0;
-    if (const char *ev = getenv("C2M_L2_PERSIST_MB")) {                      // experiment: L2 set-aside for evict-last lines
-        static int done = 0;
-        if (!done) { cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, (size_t)atoi(ev) << 20); done = 1; }
-    }
-    d.x_hi = reinterpret_cast<const __half *>(a->x_hi); d.x_lo = reinterpret_cast<const __half *>(a->x_lo);
     d.x_il = reinterpret_cast<const __half *>(a->x_il);
-    if (!d.x_hi) { d.x_hi = d.x_il; d.x_lo = d.x_il; }     // never dereferenced when x_il is set; keep pointers valid
     d.C8 = a->C / 8;
     d.om_c8 = a->om_octets ? (27 * a->dg + 7) / 8 : 0;
     C2M_CHECK_ARG(!a->om_octets || (reinterpret_cast<uintptr_t>(a->om) & 7) == 0, "dcn_v2_fused_tc: om must be 8 B aligned");
@@ -638,7 +557,7 @@ extern "C" int c2m_dcn_v2_fused_tc(const c2m_dcn_tc_args *a, c2m_stream_t stream
     d.nstage = d.L == 1 ? 4 : 8;
     d.nstage_shift = d.L == 1 ? 2 : 3;
     const size_t fixed = (size_t)d.nstage * A_STAGE + acc_stage_bytes(p.N) + (2 * MAX_NSTAGE + 2 * MAX_NBST) * 8 + 64 * 4 +
-                         2 * MAXT * 16 + (size_t)2 * p.T * d.tab_h * d.tab_w * 8 + 1024 + 128;
+                         2 * 16 + (size_t)2 * d.tab_h * d.tab_w * 8 + 1024 + 128;
     d.nbst = fixed + 4 * w_chunk <= 227 * 1024 ? 4 : 2;
     const size_t smem = fixed + d.nbst * w_chunk;
     C2M_CHECK_ARG(smem <= 227 * 1024, "dcn_v2_fused_tc: %zu bytes of shared memory needed", smem);
@@ -646,19 +565,16 @@ extern "C" int c2m_dcn_v2_fused_tc(const c2m_dcn_tc_args *a, c2m_stream_t stream
     C2M_CUDA(cudaFuncSetAttribute(dcn_wgmma_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     C2M_CUDA(cudaFuncSetAttribute(dcn_wgmma_kernel<48>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     C2M_CUDA(cudaFuncSetAttribute(dcn_wgmma_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int dev = 0, sms = 0;
-    C2M_CUDA(cudaGetDevice(&dev));
-    C2M_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    const long long n_work = (long long)a->B * p.tiles_x * p.tiles_y;
-    C2M_CHECK_ARG(n_work < (1 << 23), "dcn_v2_fused_tc: too many pixel tiles");
-    d.tg = 1;
-    const int n_items = (int)((n_work + d.tg - 1) / d.tg);
+    int sms = 0;
+    C2M_CUDA(sm_count(sms));
+    const long long n_items = (long long)a->B * p.tiles_x * p.tiles_y;
+    C2M_CHECK_ARG(n_items < (1 << 23), "dcn_v2_fused_tc: too many pixel tiles");
     // SURVEY.md §8(d): flops = 2*B*Cout*C*9*Ho*Wo; bytes = 4*B*(C*H*W + 3*dg*9*H*W + Cout*H*W) + weights
     const double px = (double)a->B * a->H * a->W;
     const double flops = 2.0 * a->Cout * a->C * 9.0 * px;
     const double bytes = 4.0 * px * (a->C + 27.0 * a->dg + a->Cout) + 4.0 * a->Cout * (a->C * 9.0 + 1.0);
     void *ph = prof_begin(PROF_DCN, flops, bytes, st);
-    const int grid = n_items < sms ? n_items : sms;
+    const int grid = n_items < sms ? (int)n_items : sms;
     for (d.slice = 0; d.slice < p.nslice; ++d.slice) {
         switch (p.N) {
         case 16: dcn_wgmma_kernel<16><<<grid, NTHREADS, smem, st>>>(q, p, d); break;

@@ -8,6 +8,28 @@
 namespace c2m {
 
 constexpr int UC_NMAX = 64;      // output channels per CTA slice
+constexpr int W_HDR = 256;       // packed-weight blob header bytes: [int sw][unsigned bits of max|w|], zero padded
+
+// Weight packing (conv and DCN share the header; their element layouts differ).  Packed weights are split fp16 of
+// w * 2^sw.  wpack_header zeroes the header and writes max|w| over the n weights into it (one launch on `st`).
+int wpack_header(const float *w, int n, void *packed, cudaStream_t st);
+// Grid of a pack kernel (256 threads, grid-stride loop) over `total` packed elements.
+inline int wpack_blocks(long long total) { return (int)((total + 255) / 256 > 592 ? 592 : (total + 255) / 256); }
+
+// Prologue of a pack kernel, after wpack_header: sw = 14 - exponent(max|w|), so |w| * 2^sw <= 2^14.  Block 0 writes sw
+// to the header for the convolution kernels; returns the scale 2^sw.
+__device__ __forceinline__ float wpack_scale(uint8_t *blob) {
+    __shared__ int s_sw;
+    if (threadIdx.x == 0) {
+        const float a = __uint_as_float(reinterpret_cast<unsigned *>(blob)[1]);
+        int e = 0;
+        if (a > 0.f && isfinite(a)) frexpf(a, &e);
+        s_sw = 14 - e;
+        if (blockIdx.x == 0) reinterpret_cast<int *>(blob)[0] = s_sw;
+    }
+    __syncthreads();
+    return ldexpf(1.f, s_sw);
+}
 
 struct ConvParams {
     int B, H, W;
@@ -17,7 +39,6 @@ struct ConvParams {
     int act;                  // 0 none, 1 relu, 2 leaky relu 0.1
     int sa_in, sa_res, sa_out;
     int ps;                   // 0 or 2: PixelShuffle(2) applied to the PSA output
-    int dbg;                  // tuning experiments only (C2M_CONV_DBG): 1 = no global stores, 2 = no TMA reloads
     int cs;                   // 1: PSA output stored with st.global.cs (streaming: the DCN output must not evict the
                               // gathered input map from L2)
     int C8out, Hout, Wout;    // geometry of the PSA output tensor
@@ -70,115 +91,113 @@ __device__ __forceinline__ void epilogue_store_block(const ConvPtrs &q, const Co
                                                      int y, int x, bool ok, int o_base, const float *sbias,
                                                      float out_scale, float res_scale, float so,
                                                      const ResRegs *r1 = nullptr) {
-                    {
-                        uint32_t reg[32];
-                        acc_ld32(acc, c0, p.N, reg);
-                        if (!ok || (p.dbg & 1)) return;
-                        const int ncol = min(32, p.N - c0);
-                        float v[32];
-    #pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            float a = fmaf(__uint_as_float(reg[j]), out_scale, sbias[c0 + j]);
-                            if (p.act == 1) a = fmaxf(a, 0.f);
-                            else if (p.act == 2) a = a > 0.f ? a : a * 0.1f;
-                            v[j] = (j < ncol && o_base + c0 + j < p.Cout) ? a : 0.f;
-                        }
-                        if (q.out_f32 && p.f32_mode == 2) {
-    #pragma unroll
-                            for (int o8 = 0; o8 < 4; ++o8) {
-                                const int oct = (o_base + c0) / 8 + o8;
-                                if (o8 * 8 >= ncol || oct >= p.C8out) break;
-                                float4 *dst = reinterpret_cast<float4 *>(
-                                    q.out_f32 + ((((size_t)b * p.C8out + oct) * p.H + y) * p.W + x) * 8);
-                                dst[0] = make_float4(v[o8 * 8], v[o8 * 8 + 1], v[o8 * 8 + 2], v[o8 * 8 + 3]);
-                                dst[1] = make_float4(v[o8 * 8 + 4], v[o8 * 8 + 5], v[o8 * 8 + 6], v[o8 * 8 + 7]);
-                            }
-                        } else if (q.out_f32) {
-                            const long long base = b * p.os_b + y * p.os_y + x * p.os_x + (long long)(o_base + c0) * p.os_c;
-    #pragma unroll
-                            for (int j4 = 0; j4 < 8; ++j4) {
-                                const int j = j4 * 4, o = o_base + c0 + j;
-                                if (p.f32_mode == 1 && j + 3 < ncol && o + 3 < p.Cout) {
-                                    float4 val = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-                                    if (q.add_f32) {
-                                        const float4 ad = *reinterpret_cast<const float4 *>(q.add_f32 + base + j);
-                                        val.x += ad.x; val.y += ad.y; val.z += ad.z; val.w += ad.w;
-                                    }
-                                    *reinterpret_cast<float4 *>(q.out_f32 + base + j) = val;
-                                } else {
-    #pragma unroll
-                                    for (int k = 0; k < 4; ++k)
-                                        if (j + k < ncol && o + k < p.Cout) {
-                                            const long long oi = base + (j + k) * p.os_c;
-                                            q.out_f32[oi] = q.add_f32 ? v[j + k] + q.add_f32[oi] : v[j + k];
-                                        }
-                                }
-                            }
-                        }
-                        if (q.out_hi && p.ps == 0) {
-    #pragma unroll
-                            for (int o8 = 0; o8 < 4; ++o8) {
-                                const int oct = (o_base + c0) / 8 + o8;
-                                if (o8 * 8 >= ncol || oct >= p.C8out) break;
-                                const size_t off = ((((size_t)b * p.C8out + oct) * p.H + y) * p.W + x) * 8;
-                                float r8[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-                                if (r1) {
-                                    const __half *hh = reinterpret_cast<const __half *>(&r1->h[o8]);
-                                    const __half *ll = reinterpret_cast<const __half *>(&r1->l[o8]);
-    #pragma unroll
-                                    for (int j = 0; j < 8; ++j) r8[j] = (__half2float(hh[j]) + __half2float(ll[j])) * res_scale;
-                                }
-                                if (q.res2_hi) {
-                                    const uint4 rh = *reinterpret_cast<const uint4 *>(q.res2_hi + off);
-                                    const uint4 rl = *reinterpret_cast<const uint4 *>(q.res2_lo + off);
-                                    const __half *hh = reinterpret_cast<const __half *>(&rh);
-                                    const __half *ll = reinterpret_cast<const __half *>(&rl);
-    #pragma unroll
-                                    for (int j = 0; j < 8; ++j) r8[j] += (__half2float(hh[j]) + __half2float(ll[j])) * res_scale;
-                                }
-                                __align__(16) __half h8[8];
-                                __align__(16) __half l8[8];
-    #pragma unroll
-                                for (int j = 0; j < 8; ++j) {
-                                    const int o = o_base + c0 + o8 * 8 + j;
-                                    const float vs = (o < p.Cout ? v[o8 * 8 + j] + r8[j] : 0.f) * so;
-                                    const __half hh = __float2half_rn(vs);
-                                    h8[j] = hh;
-                                    l8[j] = __float2half_rn(vs - __half2float(hh));
-                                }
-                                if (p.cs) {
-                                    __stcs(reinterpret_cast<uint4 *>(q.out_hi + off), *reinterpret_cast<const uint4 *>(h8));
-                                    __stcs(reinterpret_cast<uint4 *>(q.out_lo + off), *reinterpret_cast<const uint4 *>(l8));
-                                } else {
-                                    *reinterpret_cast<uint4 *>(q.out_hi + off) = *reinterpret_cast<const uint4 *>(h8);
-                                    *reinterpret_cast<uint4 *>(q.out_lo + off) = *reinterpret_cast<const uint4 *>(l8);
-                                }
-                            }
-                        }
-                        if (q.out_hi && p.ps == 2) {
-                            // PixelShuffle(2): conv channel o = 4c + 2i + j  ->  out[c][2y+i][2x+j]
-                            // the 32 columns at c0 hold c = (o_base+c0)/4 .. +7  = exactly one output octet
-                            const int oct = (o_base + c0) / 32;
-                            if (oct < p.C8out && ncol == 32) {
-    #pragma unroll
-                                for (int ij = 0; ij < 4; ++ij) {
-                                    const size_t off = ((((size_t)b * p.C8out + oct) * p.Hout + 2 * y + (ij >> 1)) * p.Wout +
-                                                        2 * x + (ij & 1)) * 8;
-                                    __align__(16) __half h8[8];
-                                    __align__(16) __half l8[8];
-    #pragma unroll
-                                    for (int c = 0; c < 8; ++c) {
-                                        const float vs = v[c * 4 + ij] * so;
-                                        const __half hh = __float2half_rn(vs);
-                                        h8[c] = hh;
-                                        l8[c] = __float2half_rn(vs - __half2float(hh));
-                                    }
-                                    *reinterpret_cast<uint4 *>(q.out_hi + off) = *reinterpret_cast<const uint4 *>(h8);
-                                    *reinterpret_cast<uint4 *>(q.out_lo + off) = *reinterpret_cast<const uint4 *>(l8);
-                                }
-                            }
-                        }
+    uint32_t reg[32];
+    acc_ld32(acc, c0, p.N, reg);
+    if (!ok) return;
+    const int ncol = min(32, p.N - c0);
+    float v[32];
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+        float a = fmaf(__uint_as_float(reg[j]), out_scale, sbias[c0 + j]);
+        if (p.act == 1) a = fmaxf(a, 0.f);
+        else if (p.act == 2) a = a > 0.f ? a : a * 0.1f;
+        v[j] = (j < ncol && o_base + c0 + j < p.Cout) ? a : 0.f;
+    }
+    if (q.out_f32 && p.f32_mode == 2) {
+#pragma unroll
+        for (int o8 = 0; o8 < 4; ++o8) {
+            const int oct = (o_base + c0) / 8 + o8;
+            if (o8 * 8 >= ncol || oct >= p.C8out) break;
+            float4 *dst = reinterpret_cast<float4 *>(
+                q.out_f32 + ((((size_t)b * p.C8out + oct) * p.H + y) * p.W + x) * 8);
+            dst[0] = make_float4(v[o8 * 8], v[o8 * 8 + 1], v[o8 * 8 + 2], v[o8 * 8 + 3]);
+            dst[1] = make_float4(v[o8 * 8 + 4], v[o8 * 8 + 5], v[o8 * 8 + 6], v[o8 * 8 + 7]);
+        }
+    } else if (q.out_f32) {
+        const long long base = b * p.os_b + y * p.os_y + x * p.os_x + (long long)(o_base + c0) * p.os_c;
+#pragma unroll
+        for (int j4 = 0; j4 < 8; ++j4) {
+            const int j = j4 * 4, o = o_base + c0 + j;
+            if (p.f32_mode == 1 && j + 3 < ncol && o + 3 < p.Cout) {
+                float4 val = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+                if (q.add_f32) {
+                    const float4 ad = *reinterpret_cast<const float4 *>(q.add_f32 + base + j);
+                    val.x += ad.x; val.y += ad.y; val.z += ad.z; val.w += ad.w;
+                }
+                *reinterpret_cast<float4 *>(q.out_f32 + base + j) = val;
+            } else {
+#pragma unroll
+                for (int k = 0; k < 4; ++k)
+                    if (j + k < ncol && o + k < p.Cout) {
+                        const long long oi = base + (j + k) * p.os_c;
+                        q.out_f32[oi] = q.add_f32 ? v[j + k] + q.add_f32[oi] : v[j + k];
                     }
+            }
+        }
+    }
+    if (q.out_hi && p.ps == 0) {
+#pragma unroll
+        for (int o8 = 0; o8 < 4; ++o8) {
+            const int oct = (o_base + c0) / 8 + o8;
+            if (o8 * 8 >= ncol || oct >= p.C8out) break;
+            const size_t off = ((((size_t)b * p.C8out + oct) * p.H + y) * p.W + x) * 8;
+            float r8[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+            if (r1) {
+                const __half *hh = reinterpret_cast<const __half *>(&r1->h[o8]);
+                const __half *ll = reinterpret_cast<const __half *>(&r1->l[o8]);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) r8[j] = (__half2float(hh[j]) + __half2float(ll[j])) * res_scale;
+            }
+            if (q.res2_hi) {
+                const uint4 rh = *reinterpret_cast<const uint4 *>(q.res2_hi + off);
+                const uint4 rl = *reinterpret_cast<const uint4 *>(q.res2_lo + off);
+                const __half *hh = reinterpret_cast<const __half *>(&rh);
+                const __half *ll = reinterpret_cast<const __half *>(&rl);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) r8[j] += (__half2float(hh[j]) + __half2float(ll[j])) * res_scale;
+            }
+            __align__(16) __half h8[8];
+            __align__(16) __half l8[8];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int o = o_base + c0 + o8 * 8 + j;
+                const float vs = (o < p.Cout ? v[o8 * 8 + j] + r8[j] : 0.f) * so;
+                const __half hh = __float2half_rn(vs);
+                h8[j] = hh;
+                l8[j] = __float2half_rn(vs - __half2float(hh));
+            }
+            if (p.cs) {
+                __stcs(reinterpret_cast<uint4 *>(q.out_hi + off), *reinterpret_cast<const uint4 *>(h8));
+                __stcs(reinterpret_cast<uint4 *>(q.out_lo + off), *reinterpret_cast<const uint4 *>(l8));
+            } else {
+                *reinterpret_cast<uint4 *>(q.out_hi + off) = *reinterpret_cast<const uint4 *>(h8);
+                *reinterpret_cast<uint4 *>(q.out_lo + off) = *reinterpret_cast<const uint4 *>(l8);
+            }
+        }
+    }
+    if (q.out_hi && p.ps == 2) {
+        // PixelShuffle(2): conv channel o = 4c + 2i + j  ->  out[c][2y+i][2x+j]
+        // the 32 columns at c0 hold c = (o_base+c0)/4 .. +7  = exactly one output octet
+        const int oct = (o_base + c0) / 32;
+        if (oct < p.C8out && ncol == 32) {
+#pragma unroll
+            for (int ij = 0; ij < 4; ++ij) {
+                const size_t off = ((((size_t)b * p.C8out + oct) * p.Hout + 2 * y + (ij >> 1)) * p.Wout +
+                                    2 * x + (ij & 1)) * 8;
+                __align__(16) __half h8[8];
+                __align__(16) __half l8[8];
+#pragma unroll
+                for (int c = 0; c < 8; ++c) {
+                    const float vs = v[c * 4 + ij] * so;
+                    const __half hh = __float2half_rn(vs);
+                    h8[c] = hh;
+                    l8[c] = __float2half_rn(vs - __half2float(hh));
+                }
+                *reinterpret_cast<uint4 *>(q.out_hi + off) = *reinterpret_cast<const uint4 *>(h8);
+                *reinterpret_cast<uint4 *>(q.out_lo + off) = *reinterpret_cast<const uint4 *>(l8);
+            }
+        }
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -284,7 +303,7 @@ __device__ __forceinline__ void epilogue_fast_block(const ConvPtrs &q, const Con
 __device__ __forceinline__ bool epilogue_fast_ok(const ConvPtrs &q, const ConvParams &p) {
     const bool psa_only = q.out_hi && !q.out_f32;
     const bool oct_only = q.out_f32 && p.f32_mode == 2 && !q.out_hi;
-    return p.ps == 0 && !q.res2_hi && !(p.dbg & 1) && (psa_only || (oct_only && !q.res_hi && p.sa_out == 0));
+    return p.ps == 0 && !q.res2_hi && (psa_only || (oct_only && !q.res_hi && p.sa_out == 0));
 }
 
 __device__ __forceinline__ void epilogue_fast_dispatch(const ConvPtrs &q, const ConvParams &p, const float *acc, int c0, int b,

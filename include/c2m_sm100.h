@@ -43,7 +43,7 @@ enum {
     C2M_ERR_UNSUPPORTED = 4   /* no sm_90 device / driver entry point missing */
 };
 
-int c2m_abi_version(void);      /* 4 since c2m_dcn_tc_args.x_il / c2m_psa_interleave (3: .mask; 2: out_f32_octets / om_octets) */
+int c2m_abi_version(void);      /* 5 since c2m_dcn_tc_args takes only x_il (4: .x_il / c2m_psa_interleave; 3: .mask; 2: out_f32_octets / om_octets) */
 const char *c2m_last_error(void);
 
 /* --- correlation / index_map --------------------------------------------------------------
@@ -143,7 +143,7 @@ int c2m_psa_from_f32(const float *x, int B, int C, int H, int W, long long xs_b,
 int c2m_psa_to_f32(const void *hi, const void *lo, int B, int C, int H, int W, int sa, const float *add, float *out,
                    long long os_b, long long os_c, long long os_y, long long os_x, c2m_stream_t stream);
 int c2m_conv3x3(const c2m_conv3x3_args *args, c2m_stream_t stream);
-/* hi / lo planes -> interleaved [B][ceil(C/8)][H][W][hi 8 | lo 8] (the DCN gather's preferred operand). */
+/* hi / lo planes -> interleaved [B][ceil(C/8)][H][W][hi 8 | lo 8] (the input operand of c2m_dcn_v2_fused_tc). */
 int c2m_psa_interleave(const void *hi, const void *lo, int B, int C, int H, int W, void *out, c2m_stream_t stream);
 /* MaxPool2d(2, 2) on a PSA tensor (floor semantics: odd trailing row / column dropped), PSA result. */
 int c2m_psa_maxpool2(const void *hi, const void *lo, int B, int C, int H, int W, void *out_hi, void *out_lo,
@@ -152,13 +152,14 @@ int c2m_psa_maxpool2(const void *hi, const void *lo, int B, int C, int H, int W,
 /* --- DCNv2 forward on the tensor cores (wgmma) (3x3 / stride 1 / pad 1 / dilation 1, C/dg % 8 == 0, Cout <= 256) ---
  * Same contract as c2m_dcn_v2_fused_forward_f32 (raw conv_offset_mask output `om`, pre-offsets from
  * `pre` or rebuilt from `idx`), but the contraction runs as a split-fp16 tensor-core GEMM fed by
- * gather warps; the input is a PSA tensor (x_hi / x_lo, see c2m_psa_from_f32): its octet-planar layout
- * lets a warp's corner fetches share cache lines.  Outputs: PSA (out_hi/out_lo) and / or
+ * gather warps; the input `x_il` is a PSA tensor (see c2m_psa_from_f32) with the two halves of a (pixel, octet)
+ * adjacent, fp16 [B][C/8][H][W][hi 8 | lo 8] (c2m_psa_interleave), 32 B aligned: its octet-planar layout lets a
+ * warp's corner fetches share cache lines, and a corner fetch is one 32 B sector.  Outputs: PSA (out_hi/out_lo) and / or
  * strided fp32; `lrelu` != 0 applies LeakyReLU(0.1).  Weights are packed once with
  * c2m_dcn_tc_pack_weights_f32 into c2m_dcn_tc_packed_weight_bytes(C, Cout, dg) bytes.
  */
 typedef struct {
-    const void *x_hi, *x_lo;
+    const void *x_il;
     const float *om; const float *pre; const int64_t *idx;
     int gh, gw, ref_gw, pre_scale;
     int B, C, H, W, Cout, dg;
@@ -169,9 +170,6 @@ typedef struct {
     const float *mask;           /* != NULL: the `_ext.dcn_v2_forward` contract (DCNv2/src/dcn_v2.h:9-22) — `om` is the
                                   * FINAL offset tensor [B,2*dg*9,H,W], `mask` the FINAL modulation [B,dg*9,H,W]
                                   * (no sigmoid applied); pre, idx and om_octets must be unset */
-    const void *x_il;            /* != NULL: the input with the two halves of a (pixel, octet) adjacent,
-                                  * fp16 [B][C/8][H][W][hi 8 | lo 8] (c2m_psa_interleave), 32 B aligned; x_hi / x_lo may
-                                  * then be NULL.  A corner fetch is one 32 B sector instead of two. */
 } c2m_dcn_tc_args;
 
 int c2m_dcn_tc_supported(int C, int Cout, int dg);

@@ -36,7 +36,7 @@ def _rel_ok(got, want, tol=1e-3):
 
 
 # ------------------------------------------------------------------------------- correlation
-@pytest.mark.parametrize('force_generic', [False, True], ids=['tcgen05', 'generic'])
+@pytest.mark.parametrize('force_generic', [False, True], ids=['wgmma', 'generic'])
 @pytest.mark.parametrize('case', mg.CORR_CASES, ids=[c[0] for c in mg.CORR_CASES])
 def test_feature_match_index_golden(case, force_generic, golden):
     import c2m_b200 as c2m

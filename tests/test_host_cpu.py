@@ -37,7 +37,7 @@ def test_library_exports_every_declared_symbol(built):
     assert set(declared) <= exported, set(declared) - exported
     assert set(built.SYMBOLS) == set(declared)          # the ctypes table binds all of them
     lib = built.lib()
-    assert lib.c2m_abi_version() == 4
+    assert lib.c2m_abi_version() == 5
 
 
 def test_sass_is_hopper_native(built):

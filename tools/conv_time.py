@@ -1,4 +1,4 @@
-"""Time one conv shape (CUDA events), for tuning experiments driven by env knobs."""
+"""Time the tensor-core 3x3 convolution (PSA in and out, ReLU) on four layer shapes: CUDA events over 10 launches each."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [ROOT, os.path.join(ROOT, 'c2-matching_b200')]

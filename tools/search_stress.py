@@ -1,7 +1,6 @@
 """How the search behaves on inputs with many near-ties: smooth (low-frequency) images, flat images with faint noise,
-and the bench's uniform-noise pair.  Prints the overflow-list statistics (C2M_CORR_DEBUG=1) and the time of one forward."""
+and the bench's uniform-noise pair.  Prints the time of one forward and whether the SR images are finite."""
 import os, sys, time
-os.environ['C2M_CORR_DEBUG'] = '1'
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 for p in (ROOT, os.path.join(ROOT, 'c2-matching_b200'), os.path.join(ROOT, 'tests', 'golden')):
     sys.path.insert(0, p)
@@ -28,10 +27,6 @@ def case(name, lq, ref):
     pipe.forward(*x)
     torch.cuda.synchronize()
     print(f'== {name}', flush=True)
-    os.environ['C2M_CORR_DEBUG'] = '1'
-    pipe.forward(*x)
-    torch.cuda.synchronize()
-    os.environ.pop('C2M_CORR_DEBUG')
     t = time.perf_counter()
     for _ in range(3):
         sr = pipe.forward(*x)
