@@ -31,7 +31,6 @@ constexpr int A_OCT_B = A_R * ROW_B;      // 2880 B (LBO of A)
 constexpr int A_HALF = KOCT * A_OCT_B;    // 11520 B (hi or lo of one stage)
 constexpr int A_STAGE = 2 * A_HALF;       // 23040 B
 constexpr int NBST = 2;                   // weight-chunk double buffer
-constexpr int MAXT = 8;                   // pixel tiles per work item
 constexpr int NMAX = 64;                  // output channels per CTA slice
 // activation ring depth: what is left of the 227 KB next to two weight slots and the accumulator staging
 __host__ __device__ constexpr int conv_nstage(int N) { return N >= 64 ? 2 : 4; }
@@ -42,11 +41,14 @@ constexpr size_t conv_smem_bytes(int N) {
 }  // namespace
 
 // ------------------------------------------------------------------------------------------
-// Work item = (image, super-tile of up to MAXT consecutive 16x8 pixel tiles, 64-wide Cout slice).
+// Schedule: CTA c computes the 64-wide Cout slice c % nslice of the 16x8 pixel tiles g = r, r + C, r + 2C, ... of
+// the whole batch (tiles numbered image-major, r = c / nslice, C = CTAs per slice).  Tile counts per CTA differ by at
+// most one, so no CTA does more than ceil(tiles / C); the CTAs running at any moment sweep neighbouring tiles (their
+// halos meet in L2), and the nslice CTAs of one tile are neighbours (they read its activation boxes together).
 // Warpgroup 0 produces: warp 0 streams the activation stages (one per (tile, kc), tile-major) through the TMA ring,
-// warp 3 bulk-copies the slice's weight chunks (9 taps, hi+lo, N*1152 B per 32-channel chunk kc).  When all chunks
-// of the slice fit the two slots (nslice == 1, nkc <= 2) they are loaded once per CTA and stay resident; otherwise
-// they are streamed per (item, kc) and the host gives every item a single tile.
+// warp 3 bulk-copies the slice's weight chunks (9 taps, hi+lo, N*1152 B per 32-channel chunk kc).  When the chunks
+// of a slice fit the two slots (nkc <= 2, i.e. Cin <= 64) they are loaded once per CTA and stay resident; otherwise
+// they are streamed per (tile, kc).
 // Warpgroups 1 and 2 consume: warpgroup c issues the wgmmas of output rows [64c, 64c + 64) (pixel rows 8c..8c+7)
 // of every tile, stages its accumulator in shared memory and runs the epilogue of those 64 pixels.
 // Per K step: x_hi * [W_hi | W_lo] (B = the 2N stacked weight rows, n = 2N) + x_lo * W_hi (n = N, into the first
@@ -70,7 +72,16 @@ conv3x3_wgmma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tiles_img = p.tiles_x * p.tiles_y;
-    const int n_items = p.B * p.n_st * p.nslice;
+    const int ntiles = p.B * tiles_img;
+    // the host launches the same number of CTAs for every slice
+    const int slice = blockIdx.x % p.nslice, rank = blockIdx.x / p.nslice, ctas = gridDim.x / p.nslice;
+    // global tile index -> (image, top-left output pixel)
+    auto tile_at = [&](int g, int &b, int &y0, int &x0) {
+        b = g / tiles_img;
+        const int tt = g - b * tiles_img;
+        y0 = (tt / p.tiles_x) * T_R;
+        x0 = (tt % p.tiles_x) * T_C;
+    };
 
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tm_hi);
@@ -85,18 +96,8 @@ conv3x3_wgmma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
     }
     __syncthreads();
     const int sw = *reinterpret_cast<const int *>(q.wblob);              // weight scale exponent
-    // all weight chunks of the (single) slice fit the chunk slots: load them once per CTA, not per item
-    const bool w_resident = p.nslice == 1 && p.nkc <= NBST;
-
-    // item -> (b, st, slice): slice fastest so concurrently running CTAs share activation tiles in L2
-    auto decode = [&](int item, int &b, int &t0, int &nt, int &slice) {
-        slice = item % p.nslice;
-        const int r = item / p.nslice;
-        const int st = r % p.n_st;
-        b = r / p.n_st;
-        t0 = st * p.T;
-        nt = min(p.T, tiles_img - t0);
-    };
+    // all weight chunks of the slice fit the chunk slots: load them once per CTA, not per tile
+    const bool w_resident = p.nkc <= NBST;
 
     if (warp < 4) {
         asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
@@ -104,23 +105,19 @@ conv3x3_wgmma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
             // ================================ activation producer ===============================
             if (lane == 0) {
                 int stage = 0, phase = 0;
-                for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-                    int b, t0, nt, slice;
-                    decode(item, b, t0, nt, slice);
-                    for (int t = 0; t < nt; ++t) {
-                        const int tt = t0 + t;
-                        const int y0 = (tt / p.tiles_x) * T_R, x0 = (tt % p.tiles_x) * T_C;
-                        for (int kc = 0; kc < p.nkc; ++kc) {
-                            const bool first = kc < p.nkc_a;
-                            const CUtensorMap *mh = first ? &tm_hi : &tm2_hi, *ml = first ? &tm_lo : &tm2_lo;
-                            const int oct0 = (first ? kc : kc - p.nkc_a) * KOCT;
-                            mbar_wait(&empty[stage], phase ^ 1);
-                            uint8_t *s = sA + stage * A_STAGE;
-                            mbar_arrive_expect_tx(&full[stage], A_STAGE);
-                            tma_load_4d(s, mh, &full[stage], (x0 - 1) * 8, y0 - 1, oct0, b);
-                            tma_load_4d(s + A_HALF, ml, &full[stage], (x0 - 1) * 8, y0 - 1, oct0, b);
-                            if (++stage == NST) { stage = 0; phase ^= 1; }
-                        }
+                for (int g = rank; g < ntiles; g += ctas) {
+                    int b, y0, x0;
+                    tile_at(g, b, y0, x0);
+                    for (int kc = 0; kc < p.nkc; ++kc) {
+                        const bool first = kc < p.nkc_a;
+                        const CUtensorMap *mh = first ? &tm_hi : &tm2_hi, *ml = first ? &tm_lo : &tm2_lo;
+                        const int oct0 = (first ? kc : kc - p.nkc_a) * KOCT;
+                        mbar_wait(&empty[stage], phase ^ 1);
+                        uint8_t *s = sA + stage * A_STAGE;
+                        mbar_arrive_expect_tx(&full[stage], A_STAGE);
+                        tma_load_4d(s, mh, &full[stage], (x0 - 1) * 8, y0 - 1, oct0, b);
+                        tma_load_4d(s + A_HALF, ml, &full[stage], (x0 - 1) * 8, y0 - 1, oct0, b);
+                        if (++stage == NST) { stage = 0; phase ^= 1; }
                     }
                 }
             }
@@ -128,10 +125,8 @@ conv3x3_wgmma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
             // ================================ weight producer ===================================
             if (lane == 0) {
                 int bst = 0, bphase = 0;
-                for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-                    int b, t0, nt, slice;
-                    decode(item, b, t0, nt, slice);
-                    if (w_resident && item != (int)blockIdx.x) break;
+                for (int g = rank; g < ntiles; g += ctas) {
+                    if (w_resident && g != rank) break;
                     for (int kc = 0; kc < p.nkc; ++kc) {
                         mbar_wait(&bempty[bst], bphase ^ 1);
                         mbar_arrive_expect_tx(&bfull[bst], w_chunk);
@@ -162,72 +157,67 @@ conv3x3_wgmma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
         const bool fast = epilogue_fast_ok(q, p);           // specialised straight-line epilogue for full blocks
         constexpr uint32_t b_lbo = 2 * N * 16;               // next channel octet of the weights
         constexpr uint32_t a_row0 = 8 * ROW_B;               // the second warpgroup's rows start 8 pixel rows down
+        const int o_base = slice * N;
+        if (threadIdx.x - 128 < N) {
+            const float bv = (q.bias && o_base + (int)threadIdx.x - 128 < p.Cout) ? q.bias[o_base + threadIdx.x - 128] : 0.f;
+            sbias[threadIdx.x - 128] = bv;
+            sbias[UC_NMAX + threadIdx.x - 128] = bv * so;           // pre-scaled copy for the specialised epilogue
+        }
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        const bool full_blk = fast && c0 + 32 <= N && o_base + c0 + 32 <= p.Cout;
         int stage = 0, phase = 0, bst = 0, bphase = 0;
-        for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-            int b, t0, nt, slice;
-            decode(item, b, t0, nt, slice);
-            const bool first_item = item == (int)blockIdx.x;
-            const int o_base = slice * N;
-            asm volatile("bar.sync 1, 256;" ::: "memory");          // previous item's sbias readers are done
-            if (threadIdx.x - 128 < N) {
-                const float bv = (q.bias && o_base + (int)threadIdx.x - 128 < p.Cout) ? q.bias[o_base + threadIdx.x - 128] : 0.f;
-                sbias[threadIdx.x - 128] = bv;
-                sbias[UC_NMAX + threadIdx.x - 128] = bv * so;       // pre-scaled copy for the specialised epilogue
+        for (int g = rank; g < ntiles; g += ctas) {
+            int b, y0, x0;
+            tile_at(g, b, y0, x0);
+            const int y = y0 + e / T_C, x = x0 + e % T_C;
+            const bool ok = y < p.H && x < p.W;
+            ResRegs ra;
+            if (has1 && c0 < N) {
+                if (full_blk) prefetch_residual_full(q.res_hi, q.res_lo, p, b, y, x, ok, o_base, c0, ra);
+                else prefetch_residual(q.res_hi, q.res_lo, p, b, y, x, ok, o_base, c0, ra);
             }
-            asm volatile("bar.sync 1, 256;" ::: "memory");
-            const bool full_blk = fast && c0 + 32 <= N && o_base + c0 + 32 <= p.Cout;
-            for (int t = 0; t < nt; ++t) {
-                const int tt = t0 + t;
-                const int y = (tt / p.tiles_x) * T_R + e / T_C, x = (tt % p.tiles_x) * T_C + e % T_C;
-                const bool ok = y < p.H && x < p.W;
-                ResRegs ra;
-                if (has1 && c0 < N) {
-                    if (full_blk) prefetch_residual_full(q.res_hi, q.res_lo, p, b, y, x, ok, o_base, c0, ra);
-                    else prefetch_residual(q.res_hi, q.res_lo, p, b, y, x, ok, o_base, c0, ra);
-                }
-                float acc[N];                                        // 64 x 2N: [x*W_hi | x*W_lo] partial sums
-                for (int kc = 0; kc < p.nkc; ++kc) {
-                    const int wslot = w_resident ? kc : bst;         // resident: chunk kc always lives in slot kc
-                    if (!w_resident || (first_item && t == 0)) mbar_wait(&bfull[wslot], w_resident ? 0 : bphase);
-                    mbar_wait(&full[stage], phase);
-                    const uint32_t a_hi = smem_u32(sA + stage * A_STAGE) + wg * a_row0;
-                    const uint64_t dah = wg_smem_desc(a_hi, A_OCT_B, ROW_B);
-                    const uint64_t dal = wg_smem_desc(a_hi + A_HALF, A_OCT_B, ROW_B);
-                    const uint64_t db = wg_smem_desc(smem_u32(sW + wslot * w_chunk), b_lbo, 128);
-                    wgmma_fence();
+            float acc[N];                                        // 64 x 2N: [x*W_hi | x*W_lo] partial sums
+            for (int kc = 0; kc < p.nkc; ++kc) {
+                const int wslot = w_resident ? kc : bst;         // resident: chunk kc always lives in slot kc
+                if (!w_resident || g == rank) mbar_wait(&bfull[wslot], w_resident ? 0 : bphase);
+                mbar_wait(&full[stage], phase);
+                const uint32_t a_hi = smem_u32(sA + stage * A_STAGE) + wg * a_row0;
+                const uint64_t dah = wg_smem_desc(a_hi, A_OCT_B, ROW_B);
+                const uint64_t dal = wg_smem_desc(a_hi + A_HALF, A_OCT_B, ROW_B);
+                const uint64_t db = wg_smem_desc(smem_u32(sW + wslot * w_chunk), b_lbo, 128);
+                wgmma_fence();
 #pragma unroll
-                    for (int tap = 0; tap < 9; ++tap) {
+                for (int tap = 0; tap < 9; ++tap) {
 #pragma unroll
-                        for (int j = 0; j < KOCT / 2; ++j) {
-                            const uint32_t ao = (tap / 3) * ROW_B + (tap % 3) * 16 + j * 2 * A_OCT_B;
-                            const uint32_t bo = (tap * KOCT + j * 2) * b_lbo;
-                            Wgmma<2 * N>::mma(acc, wg_desc_advance(dah, ao), wg_desc_advance(db, bo), (kc | tap | j) != 0);
-                            Wgmma<N>::mma(acc, wg_desc_advance(dal, ao), wg_desc_advance(db, bo), 1);
-                        }
-                    }
-                    wgmma_commit();
-                    wgmma_wait_all();
-                    mbar_arrive(&empty[stage]);
-                    if (++stage == NST) { stage = 0; phase ^= 1; }
-                    if (!w_resident) {
-                        mbar_arrive(&bempty[bst]);
-                        if (++bst == NBST) { bst = 0; bphase ^= 1; }
+                    for (int j = 0; j < KOCT / 2; ++j) {
+                        const uint32_t ao = (tap / 3) * ROW_B + (tap % 3) * 16 + j * 2 * A_OCT_B;
+                        const uint32_t bo = (tap * KOCT + j * 2) * b_lbo;
+                        Wgmma<2 * N>::mma(acc, wg_desc_advance(dah, ao), wg_desc_advance(db, bo), (kc | tap | j) != 0);
+                        Wgmma<N>::mma(acc, wg_desc_advance(dal, ao), wg_desc_advance(db, bo), 1);
                     }
                 }
-                float v[N / 2];
-#pragma unroll
-                for (int i = 0; i < N / 2; ++i) v[i] = acc[i] + acc[i + N / 2];      // columns c and N + c
-                asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");          // previous tile's epilogue is done
-                acc_store(acc_s, wg * 64, v);
-                asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
-                if (c0 < N) {
-                    if (full_blk)
-                        epilogue_fast_dispatch(q, p, acc_s + e, c0, b, y, x, ok, o_base, sbias + UC_NMAX, out_scale * so,
-                                               res_scale * so, has1 ? &ra : nullptr);
-                    else
-                        epilogue_store_block(q, p, acc_s + e, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, so,
-                                             has1 ? &ra : nullptr);
+                wgmma_commit();
+                wgmma_wait_all();
+                mbar_arrive(&empty[stage]);
+                if (++stage == NST) { stage = 0; phase ^= 1; }
+                if (!w_resident) {
+                    mbar_arrive(&bempty[bst]);
+                    if (++bst == NBST) { bst = 0; bphase ^= 1; }
                 }
+            }
+            float v[N / 2];
+#pragma unroll
+            for (int i = 0; i < N / 2; ++i) v[i] = acc[i] + acc[i + N / 2];      // columns c and N + c
+            asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");          // previous tile's epilogue is done
+            acc_store(acc_s, wg * 64, v);
+            asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+            if (c0 < N) {
+                if (full_blk)
+                    epilogue_fast_dispatch(q, p, acc_s + e, c0, b, y, x, ok, o_base, sbias + UC_NMAX, out_scale * so,
+                                           res_scale * so, has1 ? &ra : nullptr);
+                else
+                    epilogue_store_block(q, p, acc_s + e, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, so,
+                                         has1 ? &ra : nullptr);
             }
         }
     }
@@ -484,13 +474,7 @@ extern "C" int c2m_conv3x3(const c2m_conv3x3_args *a, c2m_stream_t stream) {
     p.tiles_x = ceil_div(a->W, T_C); p.tiles_y = ceil_div(a->H, T_R);
     int sms = 0;
     C2M_CUDA(sm_count(sms));
-    p.T = MAXT;
-    // small problems (e.g. 64->64 on 160x160 maps): fewer tiles per item so that every SM gets several items
-    if ((long long)a->B * p.tiles_x * p.tiles_y * p.nslice / p.T < 3 * sms) p.T = 2;
-    // weights that do not stay resident are streamed per (item, K chunk): one tile per item
-    if (!(p.nslice == 1 && p.nkc <= NBST)) p.T = 1;
     p.cs = 0;
-    p.n_st = ceil_div(p.tiles_x * p.tiles_y, p.T);
     p.act = a->act; p.sa_in = a->sa_in; p.sa_res = a->sa_res; p.sa_out = a->sa_out;
     p.ps = a->pixel_shuffle;
     const int c_out_psa = p.ps == 2 ? a->Cout / 4 : a->Cout;
@@ -522,13 +506,15 @@ extern "C" int c2m_conv3x3(const c2m_conv3x3_args *a, c2m_stream_t stream) {
     C2M_CUDA(cudaFuncSetAttribute(conv3x3_wgmma_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)conv_smem_bytes(32)));
     C2M_CUDA(cudaFuncSetAttribute(conv3x3_wgmma_kernel<48>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)conv_smem_bytes(48)));
     C2M_CUDA(cudaFuncSetAttribute(conv3x3_wgmma_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)conv_smem_bytes(64)));
-    const int n_items = a->B * p.n_st * p.nslice;
+    // one persistent CTA per SM, the same number for every slice, and no more per slice than there are tiles
+    const int tiles = a->B * p.tiles_x * p.tiles_y;
+    const int fit = sms / p.nslice > 0 ? sms / p.nslice : 1;
+    const int grid = p.nslice * (tiles < fit ? tiles : fit);
     // algorithmic work: 2*Cin*Cout*9 flops per output pixel; bytes = PSA in (4 B/elem) + out
     const double cin_t = (double)a->Cin + a->Cin2, px = (double)a->B * a->H * a->W;
     const double flops = 2.0 * cin_t * a->Cout * 9.0 * px;
     const double bytes = 4.0 * px * (cin_t + a->Cout * ((a->out_hi ? 1 : 0) + (a->out_f32 ? 1 : 0)) +
                                      a->Cout * ((a->res_hi ? 1 : 0) + (a->res2_hi ? 1 : 0) + (a->add_f32 ? 1 : 0)));
-    const int grid = n_items < sms ? n_items : sms;
     void *ph = prof_begin(PROF_CONV3X3, flops, bytes, st);
     switch (p.N) {
     case 16: conv3x3_wgmma_kernel<16><<<grid, 384, conv_smem_bytes(16), st>>>(mh, ml, m2h, m2l, q, p); break;

@@ -35,7 +35,7 @@ struct ConvParams {
     int B, H, W;
     int nkc_a, nkc;           // K chunks taken from input 1 / in total (input 2 supplies the rest)
     int Cout, N, nslice;      // real couts, couts per CTA slice (multiple of 16), slices; slice s starts at s*N
-    int tiles_x, tiles_y, T, n_st;   // tile grid, tiles per item, super-tiles per image
+    int tiles_x, tiles_y;     // 16x8-pixel tiles of one image along x / y
     int act;                  // 0 none, 1 relu, 2 leaky relu 0.1
     int sa_in, sa_res, sa_out;
     int ps;                   // 0 or 2: PixelShuffle(2) applied to the PSA output
