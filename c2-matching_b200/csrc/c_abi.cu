@@ -114,6 +114,7 @@ static void carve(CorrWorkspace &ws, const CorrGeom &g, uint8_t *base) {
     ws.sexp = (int *)(ws.amax_bits ? ws.amax_bits + 8 : nullptr);
     ws.ovf_count = ws.amax_bits ? ws.amax_bits + 16 : nullptr;
     ws.max_pn_bits = ws.amax_bits ? ws.amax_bits + 17 : nullptr;
+    ws.rinv_max_bits = ws.amax_bits ? ws.amax_bits + 18 : nullptr;
     ws.total_bytes = off;
 }
 
@@ -152,7 +153,7 @@ extern "C" int c2m_corr_argmax_f32(const float *fin, const float *fref, int B, i
 
     const bool use_umma = !(flags & 1u) && corr_umma_supported(g);
     CorrChunkGeom cg;
-    float window_coef;
+    float window_coef, sub_coef = 0.f;
     const int K = g.C * g.patch * g.patch;
     int sms = 0;
     C2M_CUDA(sm_count(sms));
@@ -167,11 +168,18 @@ extern "C" int c2m_corr_argmax_f32(const float *fin, const float *fref, int B, i
         ws.nchunk = corr_umma_pick_nchunk(g, sms);
         corr_umma_chunk_geom(g, ws.nchunk, cg);
         // DESIGN.md K2: the search scores (q_hi + q_lo) . r_hi.  |approx - exact| <= E = [2^-11 + 2^-22 (K/16 + 3)] ||P_q||
-        // ||P_r|| rinv_r: 2^-11 = fp16 rounding of the Ref operand (Cauchy-Schwarz over the patch), K/16 wgmma
+        // ||P_r|| rinv_r + E_sub: 2^-11 = fp16 rounding of the Ref operand (Cauchy-Schwarz over the patch), K/16 wgmma
         // instructions feed each score with 1 fp32 ulp of (|acc| + sum|products|) each, + the query's 2^-22 split.
-        // Window = 2E for the rounding part (best and candidate both err; 1 % margin for the fp16 subnormal range) and 4E
-        // for the accumulation part (x2 of slack for the tensor core's internal alignment).
+        // Window = 2E for the rounding part (best and candidate both err; 1 % margin) and 4E for the accumulation part
+        // (x2 of slack for the tensor core's internal alignment).
+        // E_sub: one scale exponent per map and call (|x| 2^sexp <= 1024 for the largest |x| of the whole batch) puts
+        // elements far below that maximum into the fp16 subnormals, whose rounding is absolute: up to 2^-25 per element
+        // of r_hi and of q_hi + q_lo, i.e. sqrt(K) 2^-25 over a patch.  E_sub = sqrt(K) 2^-25 [2^-sexp_in ||P_r|| rinv_r
+        // + ||P_q|| 2^-sexp_ref rinv_r], with ||P_r|| rinv_r <= 1 (max ||P_r|| for raw scores) and rinv_r <= the largest
+        // rinv of a nonzero Ref patch (an all-zero patch rounds exactly).  With l2norm (sexp = 10, pixel norms 1 or 0)
+        // it is ~1e-6 of the window.
         window_coef = 1.01f * ldexpf(1.f, -10) + ldexpf(1.f, -20) * (float)((K + 15) / 16 + 3);
+        sub_coef = 1.01f * ldexpf(1.f, -24) * sqrtf((float)(g.Cp * g.patch * g.patch));
     } else {
         int n = ceil_div(4 * sms, g.B * ceil_div(g.NQ, 64));
         const int ntile = ceil_div(g.NR, 64);
@@ -193,7 +201,7 @@ extern "C" int c2m_corr_argmax_f32(const float *fin, const float *fref, int B, i
     rc = use_umma ? corr_search_umma_launch(g, ws, st) : corr_search_generic_launch(g, ws, st);
     if (rc) return rc;
     prof_end(ph, st);
-    return corr_rescore_launch(g, ws, cg, window_coef, is_norm, norm_input, idx, val, st);
+    return corr_rescore_launch(g, ws, cg, window_coef, sub_coef, is_norm, norm_input, idx, val, st);
 }
 
 extern "C" int c2m_profile_enable(int on) {

@@ -11,7 +11,8 @@ namespace c2m {
 
 // ------------------------------------------------------------------------------------------
 // amax over a whole map (all images) -> scale exponent so that |x| * 2^sexp <= 1024 (fp16-safe
-// with 5 bits of headroom below 65504 and the lo halves far above the subnormal range).
+// with 5 bits of headroom below 65504).  Elements far below amax still reach the fp16 subnormals, whose
+// absolute rounding the rescoring window covers separately (c_abi.cu, DESIGN.md K2).
 // ------------------------------------------------------------------------------------------
 // max |x| as float bits (atomicMax on the bits of non-negative floats orders like the values); *out_bits starts at 0
 __global__ void amax_kernel(const float *__restrict__ x, size_t n, unsigned *__restrict__ out_bits) {
@@ -141,10 +142,11 @@ int corr_prep_launch(const float *x, int B, int C, int Cp, int HW, int l2norm, i
 // rinv[b][r] = 1 / (sqrt(sum over the patch's pixels of ss) + 1e-5)      (ref_map_util.py:63)
 // ------------------------------------------------------------------------------------------
 __global__ void rinv_kernel(const float *__restrict__ ss, float *__restrict__ rinv, int hr, int wr, int rh, int rw,
-                            int patch, int s_ref, int is_norm, unsigned *__restrict__ max_pn_bits) {
+                            int patch, int s_ref, int is_norm, unsigned *__restrict__ max_pn_bits,
+                            unsigned *__restrict__ rinv_max_bits) {
     const int b = blockIdx.y;
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
-    float pn = 0.f;
+    float pn = 0.f, rv = 0.f;
     if (r < rh * rw) {
         const int ry = (r / rw) * s_ref, rx = (r % rw) * s_ref;
         const float *s = ss + (size_t)b * hr * wr;
@@ -152,17 +154,25 @@ __global__ void rinv_kernel(const float *__restrict__ ss, float *__restrict__ ri
         for (int dy = 0; dy < patch; ++dy)
             for (int dx = 0; dx < patch; ++dx) acc += s[(ry + dy) * wr + rx + dx];
         pn = sqrtf(acc);
-        rinv[(size_t)b * rh * rw + r] = is_norm ? 1.f / (pn + 1e-5f) : 1.f;
+        const float ri = is_norm ? 1.f / (pn + 1e-5f) : 1.f;
+        rinv[(size_t)b * rh * rw + r] = ri;
+        if (pn > 0.f) rv = ri;           // an all-zero patch rounds exactly: it must not widen the window
     }
-    // largest Ref patch norm of the call: scales the rescoring window when the scores are not normalised
+    // largest Ref patch norm of the call: scales the rescoring window when the scores are not normalised; largest
+    // rinv of a nonzero Ref patch: scales the absolute (fp16 subnormal) rounding of the Ref operand
 #pragma unroll
-    for (int o = 16; o; o >>= 1) pn = fmaxf(pn, __shfl_xor_sync(0xffffffffu, pn, o));
+    for (int o = 16; o; o >>= 1) {
+        pn = fmaxf(pn, __shfl_xor_sync(0xffffffffu, pn, o));
+        rv = fmaxf(rv, __shfl_xor_sync(0xffffffffu, rv, o));
+    }
     if ((threadIdx.x & 31) == 0 && pn > 0.f) atomicMax(max_pn_bits, __float_as_uint(pn));
+    if ((threadIdx.x & 31) == 0 && rv > 0.f) atomicMax(rinv_max_bits, __float_as_uint(rv));
 }
 
 int corr_rinv_launch(const CorrGeom &g, const CorrWorkspace &ws, int is_norm, cudaStream_t st) {
     dim3 grid(ceil_div(g.NR, 256), g.B);
-    rinv_kernel<<<grid, 256, 0, st>>>(ws.ss_ref, ws.rinv, g.hr, g.wr, g.rh, g.rw, g.patch, g.s_ref, is_norm, ws.max_pn_bits);
+    rinv_kernel<<<grid, 256, 0, st>>>(ws.ss_ref, ws.rinv, g.hr, g.wr, g.rh, g.rw, g.patch, g.s_ref, is_norm, ws.max_pn_bits,
+                                       ws.rinv_max_bits);
     C2M_LAUNCH_CHECK("rinv_kernel");
     return C2M_OK;
 }
@@ -305,7 +315,7 @@ int corr_search_generic_launch(const CorrGeom &g, const CorrWorkspace &ws, cudaS
 //     s(r) = float( sum_k double(q[k]) * double( float(ref[k] / (float(sqrt(ss_r)) + 1e-5f)) ) )
 // — the reference's arithmetic (Ref patch normalised in fp32 first, ref_map_util.py:63) with an error-free
 // accumulation.  With |s~(r) - s(r)| <= E for every r (E = window/2, DESIGN.md K2 derives it from the number of
-// accumulation steps and the operand split), the exact argmax r* satisfies s~(r*) >= max s~ - 2E, so it is enough
+// accumulation steps, the operand split and the absolute rounding of fp16-subnormal operand elements), the exact argmax r* satisfies s~(r*) >= max s~ - 2E, so it is enough
 // to rescore every candidate inside that window.  The searches keep a top-2 per (query, Ref chunk): the list of a
 // chunk is COMPLETE unless its second entry is itself inside the window (then a third one could be hiding); those
 // (query, chunk) pairs go to an overflow list and `rescore_overflow_kernel` re-scans the whole chunk exactly.
@@ -401,9 +411,11 @@ __device__ __forceinline__ double query_patch_ss(const float *__restrict__ pinb,
 
 __global__ void __launch_bounds__(256) rescore_kernel(const float *__restrict__ pin, const float *__restrict__ pref,
                                                       const Candidate *__restrict__ part, CorrGeom g, int nchunk,
-                                                      float window_coef, float e32_coef, const float *__restrict__ rinv,
+                                                      float window_coef, float sub_coef, float e32_coef,
+                                                      const float *__restrict__ rinv,
                                                       const unsigned *__restrict__ max_pn_bits,
-                                                      int is_norm, unsigned long long *__restrict__ best_out,
+                                                      const unsigned *__restrict__ rinv_max_bits,
+                                                      const int *__restrict__ sexp, int is_norm, unsigned long long *__restrict__ best_out,
                                                       float *__restrict__ qnorm, CorrOverflow *__restrict__ ovf,
                                                       unsigned *__restrict__ ovf_count) {
     const int lane = threadIdx.x & 31;
@@ -434,9 +446,14 @@ __global__ void __launch_bounds__(256) rescore_kernel(const float *__restrict__ 
 #pragma unroll
     for (int o = 16; o; o >>= 1) vmax = fmaxf(vmax, __shfl_xor_sync(0xffffffffu, vmax, o));
 
-    // window = 2E: proportional to the query patch norm (and to the largest Ref patch norm when scores are raw)
+    // window = 2E: proportional to the query patch norm (and to the largest Ref patch norm when scores are raw), plus
+    // the absolute rounding of operand elements that the map's scale exponent leaves in the fp16 subnormals:
+    // sub_coef * [2^-sexp_in (query split) + ||P_q|| 2^-sexp_ref rinv_max (Ref operand)]   (see c_abi.cu)
     const float qn = (float)sqrt(query_patch_ss(pinb, g, qp, lane));
-    const float window = window_coef * qn * (is_norm ? 1.f : __uint_as_float(*max_pn_bits)) + 1e-30f;
+    const float pscale = is_norm ? 1.f : __uint_as_float(*max_pn_bits);
+    float window = window_coef * qn * pscale + 1e-30f;
+    if (sub_coef > 0.f)
+        window += sub_coef * (ldexpf(1.f, -sexp[0]) * pscale + qn * ldexpf(1.f, -sexp[1]) * __uint_as_float(*rinv_max_bits));
     const float thr = vmax - window;
 
     // a chunk's list is complete unless something it left behind (`dropped`) reaches the window -> exhaustive re-scan
@@ -602,12 +619,13 @@ __global__ void __launch_bounds__(256) rescore_finish_kernel(const unsigned long
 }
 
 int corr_rescore_launch(const CorrGeom &g, const CorrWorkspace &ws, const CorrChunkGeom &cg, float window_coef,
-                        int is_norm, int norm_input, int64_t *idx, float *val, cudaStream_t st) {
+                        float sub_coef, int is_norm, int norm_input, int64_t *idx, float *val, cudaStream_t st) {
     dim3 grid(ceil_div(g.NQ, 8), g.B);
     const int K = g.Cp * g.patch * g.patch;
     const float e32_coef = ldexpf(1.f, -24) * (float)(K + 8);
-    rescore_kernel<<<grid, 256, 0, st>>>(ws.p32_in, ws.p32_ref, ws.part, g, ws.nchunk, window_coef, e32_coef, ws.rinv,
-                                         ws.max_pn_bits, is_norm, ws.best, ws.qnorm, ws.ovf, ws.ovf_count);
+    rescore_kernel<<<grid, 256, 0, st>>>(ws.p32_in, ws.p32_ref, ws.part, g, ws.nchunk, window_coef, sub_coef, e32_coef,
+                                         ws.rinv, ws.max_pn_bits, ws.rinv_max_bits, ws.sexp, is_norm, ws.best, ws.qnorm,
+                                         ws.ovf, ws.ovf_count);
     C2M_LAUNCH_CHECK("rescore_kernel");
     // fp32 prefilter of the re-scan: query patch in shared memory when it fits (it does for every model shape)
     const int qs_floats = K * 4 <= 48 * 1024 ? K : 0;

@@ -63,6 +63,7 @@ struct CorrWorkspace {
     int *sexp;               // [2] scale exponents for (in, ref)
     unsigned *ovf_count;     // [1] entries in ovf
     unsigned *max_pn_bits;   // [1] max over Ref patches of ||P_ref|| (float bits) — window scale when !is_norm
+    unsigned *rinv_max_bits; // [1] max of rinv over Ref patches with nonzero norm (float bits)
     int nchunk;
     size_t total_bytes;
 };
@@ -134,8 +135,9 @@ bool corr_umma_supported(const CorrGeom &g);
 int corr_umma_pick_nchunk(const CorrGeom &g, int sms);
 void corr_umma_chunk_geom(const CorrGeom &g, int nchunk, CorrChunkGeom &cg);
 void corr_generic_chunk_geom(const CorrGeom &g, int nchunk, CorrChunkGeom &cg);
-// window_coef: rigorous bound on 2 x |approximate - exact score| per unit of ||P_query|| (see corr_aux.cu)
+// window_coef: rigorous bound on 2 x |approximate - exact score| per unit of ||P_query|| (see corr_aux.cu);
+// sub_coef: the same for the absolute rounding of fp16-subnormal operand elements (0 for the fp32 search, see c_abi.cu)
 int corr_rescore_launch(const CorrGeom &g, const CorrWorkspace &ws, const CorrChunkGeom &cg, float window_coef,
-                        int is_norm, int norm_input, int64_t *idx, float *val, cudaStream_t st);
+                        float sub_coef, int is_norm, int norm_input, int64_t *idx, float *val, cudaStream_t st);
 
 }  // namespace c2m
