@@ -127,6 +127,20 @@ def _out_hw(H, W, kh, kw, sh, sw, ph, pw, dh, dw):
     return ((H + 2 * ph - (dh * (kh - 1) + 1)) // sh + 1, (W + 2 * pw - (dw * (kw - 1) + 1)) // sw + 1)
 
 
+def _pre_offset_source(pre_offset, idx, B, taps, Ho, Wo):
+    """Checks the optional pre-offset source of the fused DCN forwards and returns (pre_offset, idx), each
+    contiguous or None: pre_offset [B,taps,Ho,Wo,2] (x,y) fp32 wins over idx int64 [B,gh,gw]."""
+    if pre_offset is not None:
+        _require_cuda('pre_offset', pre_offset)
+        if tuple(pre_offset.shape) != (B, taps, Ho, Wo, 2):
+            raise RuntimeError(f'pre_offset has shape {tuple(pre_offset.shape)}')
+        return pre_offset.contiguous(), None
+    if idx is not None:
+        _require_cuda('idx', idx, torch.int64)
+        return None, idx.contiguous()
+    return None, None
+
+
 def dcn_v2_forward(input, weight, bias, offset, mask, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w,
                    dilation_h, dilation_w, deformable_group):
     """`_ext.dcn_v2_forward` (DCNv2/src/dcn_v2.h:9-39; call site dcn_v2.py:26-30)."""
@@ -177,22 +191,12 @@ def dcn_v2_fused_forward(x, om, weight, bias, deformable_group, pre_offset=None,
     mf = torch.channels_last if channels_last_out else torch.contiguous_format
     out = torch.empty(B, weight.shape[0], Ho, Wo, dtype=torch.float32, device=x.device, memory_format=mf)
     s = _shape(x, weight.shape[0], kh, kw, 1, 1, kh // 2, kw // 2, 1, 1, deformable_group, out)
-    pre_p = idx_p = None
-    gh = gw = 0
-    if pre_offset is not None:
-        _require_cuda('pre_offset', pre_offset)
-        if tuple(pre_offset.shape) != (B, kh * kw, Ho, Wo, 2):
-            raise RuntimeError(f'pre_offset has shape {tuple(pre_offset.shape)}')
-        pre_offset = pre_offset.contiguous()
-        pre_p = pre_offset.data_ptr()
-    elif idx is not None:
-        _require_cuda('idx', idx, torch.int64)
-        idx = idx.contiguous()
-        gh, gw = idx.shape[1:]
-        idx_p = idx.data_ptr()
+    pre_offset, idx = _pre_offset_source(pre_offset, idx, B, kh * kw, Ho, Wo)
+    gh, gw = idx.shape[1:] if idx is not None else (0, 0)
     with torch.cuda.device(x.device):
         rc = _lib.lib().c2m_dcn_v2_fused_forward_f32(
-            x.data_ptr(), om.data_ptr(), pre_p, idx_p, gh, gw, ref_gw or gw, pre_scale,
+            x.data_ptr(), om.data_ptr(), pre_offset.data_ptr() if pre_offset is not None else None,
+            idx.data_ptr() if idx is not None else None, gh, gw, ref_gw or gw, pre_scale,
             weight.contiguous().data_ptr(), bias.contiguous().data_ptr() if bias is not None else None,
             float(lrelu_slope), out.data_ptr(), s, _stream())
         _lib.check(rc, 'c2m_dcn_v2_fused_forward_f32')
@@ -495,15 +499,10 @@ def dcn_v2_fused_tc(x, om, weight, bias, deformable_group, pre_offset=None, idx=
     else:
         om = om.contiguous()
         a.om = om.data_ptr()
+    pre_offset, idx = _pre_offset_source(pre_offset, idx, B, 9, H, W)
     if pre_offset is not None:
-        _require_cuda('pre_offset', pre_offset)
-        if tuple(pre_offset.shape) != (B, 9, H, W, 2):
-            raise RuntimeError(f'pre_offset has shape {tuple(pre_offset.shape)}')
-        pre_offset = pre_offset.contiguous()
         a.pre = pre_offset.data_ptr()
     elif idx is not None:
-        _require_cuda('idx', idx, torch.int64)
-        idx = idx.contiguous()
         a.idx = idx.data_ptr()
         a.gh, a.gw = idx.shape[1:]
         a.ref_gw, a.pre_scale = (ref_gw or idx.shape[2]), pre_scale

@@ -10,14 +10,15 @@
 // pre-offset add with the (x,y)->(y,x) reorder, sigmoid of the mask, no host sync) and can rebuild
 // the pre-offsets from the index map on the fly (corres_generation_arch.py:29-46,70-104).
 //
-// Sampling arithmetic follows modulated_deformable_im2col_gpu_kernel / dmcn_im2col_bilinear
-// (dcn_v2_im2col_cuda.cu:25-54,125-195) operation for operation.
+// The sampling rule, shape check and index-map decode are the ones in dcn_sampling.cuh, shared with
+// the backward kernels (dcn_bwd.cu) and offsets.cu.
 //
 // CTA = 256 threads = 64 output pixels x (16*NO) output channels; thread (tx,ty) owns pixels
 // 4tx..4tx+3 and channels ty+16i.  K is walked one deformable group / channel block at a time:
 // the sampling table (4 corner offsets + 4 weights + mask per (tap, pixel)) is computed once
-// and shared by all channels of the group.
-#include "c2m_common.cuh"
+// and shared by all channels of the group.  A corner outside the image is stored as element 0
+// with weight 0, so the gather loads unconditionally.
+#include "dcn_sampling.cuh"
 
 namespace c2m {
 
@@ -32,7 +33,7 @@ struct DcnArgs {
     const long long *idx;
     float *out;
     c2m_dcn_shape s;
-    int Ho, Wo, T;
+    DcnGeom g;
     int gh, gw, ref_gw, pre_scale;
     float slope;
     int CB;                   // channels per pass (<= cpg, <= MAXCB)
@@ -49,8 +50,8 @@ template <int NO>
 __global__ void __launch_bounds__(256) dcn_fwd_kernel(const DcnArgs a) {
     extern __shared__ __align__(16) uint8_t dsm[];
     const c2m_dcn_shape &s = a.s;
-    const int T = a.T, cpg = s.C / s.dg, CB = a.CB;
-    const int P = a.Ho * a.Wo;
+    const int T = a.g.T, cpg = a.g.cpg, CB = a.CB;
+    const int P = a.g.Ho * a.g.Wo;
     const int NOUT = 16 * NO;
 
     Samp *samp = reinterpret_cast<Samp *>(dsm);                               // [MAXT][TP]
@@ -74,13 +75,8 @@ __global__ void __launch_bounds__(256) dcn_fwd_kernel(const DcnArgs a) {
             // ---- sampling table for (tap, pixel), shared by the group's channels
             for (int e = t; e < TB * TP; e += 256) {
                 const int tl = e / TP, pl = e % TP, tap = t0 + tl, p = p0 + pl;
-                Samp sp;
-                sp.o[0] = sp.o[1] = sp.o[2] = sp.o[3] = 0;
-                sp.w[0] = sp.w[1] = sp.w[2] = sp.w[3] = 0.f;
-                sp.m = 0.f;
+                Samp sp = {};
                 if (p < P) {
-                    const int ho = p / a.Wo, wo = p % a.Wo;
-                    const int ki = tap / s.kw, kj = tap % s.kw;
                     const int j = g * T + tap;
                     float off_h, off_w, m;
                     if (a.om) {
@@ -89,43 +85,27 @@ __global__ void __launch_bounds__(256) dcn_fwd_kernel(const DcnArgs a) {
                         off_w = omb[(long long)(2 * j + 1) * P + p];
                         const float mr = omb[(long long)(2 * s.dg * T + j) * P + p];
                         m = 1.f / (1.f + expf(-mr));
-                        float px = 0.f, py = 0.f;
+                        float2 f = make_float2(0.f, 0.f);   // pre-offset (x, y)
                         if (a.pre) {
                             const float *pp = a.pre + (((long long)b * T + tap) * P + p) * 2;
-                            px = pp[0];
-                            py = pp[1];
+                            f = make_float2(pp[0], pp[1]);
                         } else if (a.idx) {
-                            // flow pyramid rebuilt from the index map (same rule as offsets.cu)
-                            const int sc = a.pre_scale;
-                            const int ys = ho - sc * ki, xs = wo - sc * kj;
-                            if (ys >= 0 && xs >= 0) {
-                                const int y = ys / sc, xg = xs / sc;
-                                if (y < a.gh && xg < a.gw) {
-                                    const long long v = a.idx[((long long)b * a.gh + y) * a.gw + xg];
-                                    px = (float)(sc * ((int)(v % a.ref_gw) - xg));
-                                    py = (float)(sc * ((int)(v / a.ref_gw) - y));
-                                }
-                            }
+                            f = pyramid_flow(a.idx, b, a.gh, a.gw, a.ref_gw, a.pre_scale, p / a.g.Wo, p % a.g.Wo,
+                                             tap / s.kw, tap % s.kw);
                         }
-                        off_h += py;
-                        off_w += px;
+                        off_h += f.y;
+                        off_w += f.x;
                     } else {
                         off_h = a.offset[((long long)b * 2 * s.dg * T + 2 * j) * P + p];
                         off_w = a.offset[((long long)b * 2 * s.dg * T + 2 * j + 1) * P + p];
                         m = a.mask[((long long)b * s.dg * T + j) * P + p];
                     }
-                    const float h_im = (float)(ho * s.sh - s.ph + ki * s.dh) + off_h;
-                    const float w_im = (float)(wo * s.sw - s.pw + kj * s.dw) + off_w;
-                    if (h_im > -1.f && w_im > -1.f && h_im < (float)s.H && w_im < (float)s.W) {
-                        const int h_low = (int)floorf(h_im), w_low = (int)floorf(w_im);
-                        const int h_high = h_low + 1, w_high = w_low + 1;
-                        const float lh = h_im - h_low, lw = w_im - w_low;
-                        const float hh = 1.f - lh, hw = 1.f - lw;
-                        const bool t0v = h_low >= 0, t1v = h_high <= s.H - 1, l0v = w_low >= 0, l1v = w_high <= s.W - 1;
-                        if (t0v && l0v) { sp.o[0] = (int)(h_low * s.xs_y + w_low * s.xs_x); sp.w[0] = hh * hw; }
-                        if (t0v && l1v) { sp.o[1] = (int)(h_low * s.xs_y + w_high * s.xs_x); sp.w[1] = hh * lw; }
-                        if (t1v && l0v) { sp.o[2] = (int)(h_high * s.xs_y + w_low * s.xs_x); sp.w[2] = lh * hw; }
-                        if (t1v && l1v) { sp.o[3] = (int)(h_high * s.xs_y + w_high * s.xs_x); sp.w[3] = lh * lw; }
+                    float h_im, w_im;
+                    if (dcn_sample_point(s, a.g.Wo, tap, p, off_h, off_w, h_im, w_im)) {
+                        const DcnCorners c(h_im, w_im, s.H, s.W, s.xs_y, s.xs_x);
+#pragma unroll
+                        for (int q = 0; q < 4; ++q)
+                            if (c.ok[q]) { sp.o[q] = c.o[q]; sp.w[q] = c.w[q]; }
                         sp.m = m;
                     }
                 }
@@ -142,8 +122,7 @@ __global__ void __launch_bounds__(256) dcn_fwd_kernel(const DcnArgs a) {
                         const int cl = e % CBn, rest = e / CBn, pl = rest % TP, tl = rest / TP;
                         const Samp &sp = samp[tl * TP + pl];
                         const float *xc = xb + (g * cpg + cb0 + cl);
-                        const float v = sp.w[0] * xc[sp.o[0]] + sp.w[1] * xc[sp.o[1]] + sp.w[2] * xc[sp.o[2]] +
-                                        sp.w[3] * xc[sp.o[3]];
+                        const float v = dcn_blend(sp.w, xc[sp.o[0]], xc[sp.o[1]], xc[sp.o[2]], xc[sp.o[3]]);
                         col[(cl * TB + tl) * TP + pl] = v * sp.m;
                     }
                 } else {
@@ -151,8 +130,7 @@ __global__ void __launch_bounds__(256) dcn_fwd_kernel(const DcnArgs a) {
                         const int pl = e % TP, row = e / TP, cl = row / TB, tl = row % TB;
                         const Samp &sp = samp[tl * TP + pl];
                         const float *xc = xb + (long long)(g * cpg + cb0 + cl) * s.xs_c;
-                        const float v = sp.w[0] * xc[sp.o[0]] + sp.w[1] * xc[sp.o[1]] + sp.w[2] * xc[sp.o[2]] +
-                                        sp.w[3] * xc[sp.o[3]];
+                        const float v = dcn_blend(sp.w, xc[sp.o[0]], xc[sp.o[1]], xc[sp.o[2]], xc[sp.o[3]]);
                         col[row * TP + pl] = v * sp.m;
                     }
                 }
@@ -199,7 +177,7 @@ __global__ void __launch_bounds__(256) dcn_fwd_kernel(const DcnArgs a) {
             if (p >= P) continue;
             float v = acc[i][j] + bv;
             if (a.slope != 1.f) v = v > 0.f ? v : v * a.slope;
-            ob[(long long)o * s.os_c + (long long)(p / a.Wo) * s.os_y + (long long)(p % a.Wo) * s.os_x] = v;
+            ob[(long long)o * s.os_c + (long long)(p / a.g.Wo) * s.os_y + (long long)(p % a.g.Wo) * s.os_x] = v;
         }
     }
 }
@@ -209,7 +187,7 @@ static int launch_no(const DcnArgs &a, cudaStream_t st) {
     const int NOUT = 16 * NO;
     const size_t smem = sizeof(Samp) * MAXT * TP + (size_t)a.CB * MAXT * TP * 4 + (size_t)KSUB * NOUT * 4;
     C2M_CUDA(cudaFuncSetAttribute(dcn_fwd_kernel<NO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    dim3 grid(ceil_div(a.Ho * a.Wo, TP), a.s.B, ceil_div(a.s.Cout, NOUT));
+    dim3 grid(ceil_div(a.g.Ho * a.g.Wo, TP), a.s.B, ceil_div(a.s.Cout, NOUT));
     dcn_fwd_kernel<NO><<<grid, 256, smem, st>>>(a);
     C2M_LAUNCH_CHECK("dcn_fwd_kernel");
     return C2M_OK;
@@ -217,15 +195,9 @@ static int launch_no(const DcnArgs &a, cudaStream_t st) {
 
 static int dcn_launch(DcnArgs a, cudaStream_t st) {
     const c2m_dcn_shape &s = a.s;
-    C2M_CHECK_ARG(s.B > 0 && s.C > 0 && s.H > 0 && s.W > 0 && s.Cout > 0, "dcn_v2: empty tensor");
-    C2M_CHECK_ARG(s.kh > 0 && s.kw > 0 && s.sh > 0 && s.sw > 0 && s.dh > 0 && s.dw > 0, "dcn_v2: bad kernel geometry");
-    C2M_CHECK_ARG(s.dg > 0 && s.C % s.dg == 0, "dcn_v2: channels (%d) not divisible by deformable_group (%d)", s.C, s.dg);
-    a.Ho = (s.H + 2 * s.ph - (s.dh * (s.kh - 1) + 1)) / s.sh + 1;
-    a.Wo = (s.W + 2 * s.pw - (s.dw * (s.kw - 1) + 1)) / s.sw + 1;
-    C2M_CHECK_ARG(a.Ho > 0 && a.Wo > 0, "dcn_v2: empty output (%d x %d)", a.Ho, a.Wo);
-    a.T = s.kh * s.kw;
-    const int cpg = s.C / s.dg;
-    a.CB = cpg < MAXCB ? cpg : MAXCB;
+    C2M_CHECK_ARG(s.Cout > 0, "dcn_v2: empty tensor");
+    if (int rc = dcn_geometry(&s, "dcn_v2", a.g)) return rc;
+    a.CB = a.g.cpg < MAXCB ? a.g.cpg : MAXCB;
     if (s.Cout <= 16) return launch_no<1>(a, st);
     if (s.Cout <= 32) return launch_no<2>(a, st);
     if (s.Cout <= 64) return launch_no<4>(a, st);

@@ -2,8 +2,9 @@
 //
 // Replaces CorrespondenceGenerationArch.index_to_flow + the tensor_shift / repeat_interleave
 // cascade (mmsr/models/archs/corres_generation_arch.py:29-46,70-104; arch_util.py:291-315): ~40
-// tiny elementwise kernels and a meshgrid per image become one launch per scale for the batch.
-#include "c2m_common.cuh"
+// tiny elementwise kernels and a meshgrid per image become one launch per scale for the batch.  The
+// decode itself is pyramid_flow (dcn_sampling.cuh), which the fused DCN forward also calls.
+#include "dcn_sampling.cuh"
 
 namespace c2m {
 
@@ -11,21 +12,8 @@ __global__ void offset_pyramid_kernel(const long long *__restrict__ idx, int gh,
                                       float2 *__restrict__ out) {
     const int HS = (gh + 2) * s, WS = (gw + 2) * s;
     const int b = blockIdx.z, k = blockIdx.y;
-    const int i = k / 3, j = k % 3;
-    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < HS * WS; e += gridDim.x * blockDim.x) {
-        const int Y = e / WS, X = e % WS;
-        float2 f = make_float2(0.f, 0.f);
-        const int ys = Y - s * i, xs = X - s * j;
-        if (ys >= 0 && xs >= 0) {
-            const int y = ys / s, x = xs / s;
-            if (y < gh && x < gw) {
-                const long long v = idx[((long long)b * gh + y) * gw + x];
-                f.x = (float)(s * ((int)(v % ref_gw) - x));
-                f.y = (float)(s * ((int)(v / ref_gw) - y));
-            }
-        }
-        out[((long long)b * 9 + k) * HS * WS + e] = f;
-    }
+    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < HS * WS; e += gridDim.x * blockDim.x)
+        out[((long long)b * 9 + k) * HS * WS + e] = pyramid_flow(idx, b, gh, gw, ref_gw, s, e / WS, e % WS, k / 3, k % 3);
 }
 
 }  // namespace c2m
