@@ -2,14 +2,5 @@
 (mmsr/models/archs/DCNv2/src/vision.cpp:3-8; imported as `import _ext as _backend` at
 mmsr/models/archs/DCNv2/dcn_v2.py:6).  Same names, positional signatures and error behaviour;
 the arithmetic runs in libc2m_sm100.so through the C ABI (include/c2m_sm100.h)."""
-from c2m_b200.ops import dcn_v2_backward, dcn_v2_forward  # noqa: F401
-
-
-def dcn_v2_psroi_pooling_forward(*args, **kwargs):
-    """DCNv2/src/dcn_v2.h:75-108 — unused by any C2-Matching arch."""
-    raise NotImplementedError('_ext.dcn_v2_psroi_pooling_forward is not part of the C2-Matching hot path')
-
-
-def dcn_v2_psroi_pooling_backward(*args, **kwargs):
-    """DCNv2/src/dcn_v2.h:110-144 — unused by any C2-Matching arch."""
-    raise NotImplementedError('_ext.dcn_v2_psroi_pooling_backward is not part of the C2-Matching hot path')
+from c2m_b200.ops import (dcn_v2_backward, dcn_v2_forward, dcn_v2_psroi_pooling_backward,  # noqa: F401
+                          dcn_v2_psroi_pooling_forward)

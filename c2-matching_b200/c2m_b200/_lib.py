@@ -48,6 +48,17 @@ class DcnTcArgs(ctypes.Structure):
                 ('mask', ctypes.c_void_p)]
 
 
+class PsroiShape(ctypes.Structure):
+    """c2m_psroi_shape (include/c2m_sm100.h)."""
+    _fields_ = [(n, ctypes.c_int) for n in ('B', 'C', 'H', 'W', 'R', 'no_trans', 'num_classes')] + \
+               [('spatial_scale', ctypes.c_float), ('trans_std', ctypes.c_float)] + \
+               [(n, ctypes.c_int) for n in ('output_dim', 'group_size', 'pooled_size', 'part_size', 'sample_per_part')]
+
+
+_psroi_fwd = (ctypes.c_int, [ctypes.c_void_p] * 3 + [ctypes.POINTER(PsroiShape)] + [ctypes.c_void_p] * 3)
+_psroi_bwd = (ctypes.c_int, [ctypes.c_void_p] * 5 + [ctypes.POINTER(PsroiShape)] + [ctypes.c_void_p] * 3 +
+              [ctypes.c_size_t, ctypes.c_void_p])
+
 SYMBOLS = {
     'c2m_abi_version': (ctypes.c_int, []),
     'c2m_last_error': (ctypes.c_char_p, []),
@@ -80,6 +91,11 @@ SYMBOLS = {
     'c2m_dcn_v2_fused_forward_f32': (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_i64p] + [ctypes.c_int] * 4 +
                                      [c_f32p, c_f32p, ctypes.c_float, c_f32p, ctypes.POINTER(DcnShape),
                                       ctypes.c_void_p]),
+    'c2m_psroi_pooling_workspace_bytes': (ctypes.c_size_t, [ctypes.POINTER(PsroiShape), ctypes.c_int]),
+    'c2m_psroi_pooling_forward_f32': _psroi_fwd,
+    'c2m_psroi_pooling_forward_f64': _psroi_fwd,
+    'c2m_psroi_pooling_backward_f32': _psroi_bwd,
+    'c2m_psroi_pooling_backward_f64': _psroi_bwd,
 }
 
 

@@ -572,3 +572,91 @@ def dcn_v2_backward(input, weight, bias, offset, mask, grad_output, kernel_h, ke
     finally:
         torch.backends.cuda.matmul.allow_tf32 = prev
     return [grad_input, grad_offset, grad_mask, grad_weight, grad_bias]
+
+
+# ------------------------------------------------------------------------------------------------
+# Deformable PS-ROI pooling (completes the `_ext` ABI)
+def _psroi_prepare(input, bbox, trans, no_trans, spatial_scale, output_dim, group_size, pooled_size, part_size,
+                   sample_per_part, trans_std):
+    """Validates the tensors (the size / channel rules are checked again by the library) and returns the contiguous
+    operands and the c2m_psroi_shape."""
+    if not isinstance(input, torch.Tensor):
+        raise TypeError('input must be a Tensor')
+    dtype = input.dtype
+    if dtype not in (torch.float32, torch.float64):
+        raise RuntimeError(f'input must be torch.float32 or torch.float64, got {dtype}')
+    _require_cuda('input', input, dtype)
+    _require_cuda('bbox', bbox, dtype)
+    if not no_trans:
+        _require_cuda('trans', trans, dtype)
+    if input.dim() != 4:
+        raise RuntimeError(f'input must be [B, C, H, W], got shape {tuple(input.shape)}')
+    if bbox.dim() != 2 or bbox.shape[1] != 5:
+        raise RuntimeError(f'bbox must be [R, 5], got shape {tuple(bbox.shape)}')
+    if bbox.device != input.device or (not no_trans and trans.device != input.device):
+        raise RuntimeError('input, bbox and trans must be on the same device')
+    if min(pooled_size, part_size, sample_per_part) < 1:
+        raise RuntimeError(f'pooled_size, part_size and sample_per_part must be >= 1, got {pooled_size}, '
+                           f'{part_size}, {sample_per_part}')
+    B, C, H, W = input.shape
+    R = bbox.shape[0]
+    K = 1
+    if not no_trans:
+        if (trans.dim() != 4 or trans.shape[0] != R or trans.shape[1] < 2 or trans.shape[1] % 2 or
+                tuple(trans.shape[2:]) != (part_size, part_size)):
+            raise RuntimeError(f'trans must be [R, 2K, part_size, part_size] = [{R}, 2K, {part_size}, {part_size}] '
+                               f'with K >= 1, got shape {tuple(trans.shape)}')
+        K = trans.shape[1] // 2
+    s = _lib.PsroiShape(B=B, C=C, H=H, W=W, R=R, no_trans=int(bool(no_trans)), num_classes=K,
+                        spatial_scale=spatial_scale, trans_std=trans_std, output_dim=output_dim,
+                        group_size=group_size, pooled_size=pooled_size, part_size=part_size,
+                        sample_per_part=sample_per_part)
+    return s, input.contiguous(), bbox.contiguous(), None if no_trans else trans.contiguous()
+
+
+def _psroi_sfx(dtype):
+    return 'f32' if dtype == torch.float32 else 'f64'
+
+
+def dcn_v2_psroi_pooling_forward(input, bbox, trans, no_trans, spatial_scale, output_dim, group_size, pooled_size,
+                                 part_size, sample_per_part, trans_std):
+    """`_ext.dcn_v2_psroi_pooling_forward` (DCNv2/src/dcn_v2.h:75-108; call site dcn_v2.py:280-283) ->
+    (output, output_count), both [R, output_dim, pooled_size, pooled_size] in the input's dtype."""
+    s, x, bbox, trans = _psroi_prepare(input, bbox, trans, no_trans, spatial_scale, output_dim, group_size,
+                                       pooled_size, part_size, sample_per_part, trans_std)
+    out = torch.empty(s.R, output_dim, pooled_size, pooled_size, dtype=x.dtype, device=x.device)
+    count = torch.empty_like(out)
+    fn = f'c2m_psroi_pooling_forward_{_psroi_sfx(x.dtype)}'
+    with torch.cuda.device(x.device):
+        _lib.check(getattr(_lib.lib(), fn)(x.data_ptr(), bbox.data_ptr(), None if trans is None else trans.data_ptr(),
+                                           s, out.data_ptr(), count.data_ptr(), _stream()), fn)
+    return out, count
+
+
+def dcn_v2_psroi_pooling_backward(out_grad, input, bbox, trans, top_count, no_trans, spatial_scale, output_dim,
+                                  group_size, pooled_size, part_size, sample_per_part, trans_std):
+    """`_ext.dcn_v2_psroi_pooling_backward` (DCNv2/src/dcn_v2.h:110-144; call site dcn_v2.py:291-304) ->
+    (grad_input, grad_trans).  grad_input is scattered with atomics (summation order not fixed); grad_trans is
+    reduced in a fixed order and is the same bit for bit on every run.  With no_trans, grad_trans is
+    zeros_like(trans)."""
+    s, x, bbox, tr = _psroi_prepare(input, bbox, trans, no_trans, spatial_scale, output_dim, group_size, pooled_size,
+                                    part_size, sample_per_part, trans_std)
+    _require_cuda('out_grad', out_grad, x.dtype)
+    _require_cuda('top_count', top_count, x.dtype)
+    want = (s.R, output_dim, pooled_size, pooled_size)
+    if tuple(out_grad.shape) != want or tuple(top_count.shape) != want:
+        raise RuntimeError(f'out_grad and top_count must be {want}, got {tuple(out_grad.shape)} and '
+                           f'{tuple(top_count.shape)}')
+    gout, cnt = out_grad.contiguous(), top_count.contiguous()
+    L = _lib.lib()
+    fn = f'c2m_psroi_pooling_backward_{_psroi_sfx(x.dtype)}'
+    with torch.cuda.device(x.device):
+        grad_input = torch.zeros_like(x)
+        grad_trans = torch.zeros_like(trans) if tr is None else torch.zeros_like(tr)
+        nbytes = L.c2m_psroi_pooling_workspace_bytes(s, x.element_size())
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device) if nbytes else None
+        _lib.check(getattr(L, fn)(gout.data_ptr(), x.data_ptr(), bbox.data_ptr(), None if tr is None else tr.data_ptr(),
+                                  cnt.data_ptr(), s, grad_input.data_ptr(),
+                                  None if tr is None else grad_trans.data_ptr(),
+                                  None if ws is None else ws.data_ptr(), nbytes, _stream()), fn)
+    return grad_input, grad_trans

@@ -1,5 +1,7 @@
 """DCNv2 module layer with the reference's class names and state-dict keys
-(mmsr/models/archs/DCNv2/dcn_v2.py), forward-only, on top of the drop-in `_ext`.
+(mmsr/models/archs/DCNv2/dcn_v2.py) on top of the drop-in `_ext`: the deformable convolutions
+(`DCNv2`, `DCN`, `DCN_sep`, `DCN_sep_pre_multi_offset`) and the deformable PS-ROI pooling modules
+(`DCNv2Pooling`, `DCNPooling`), forward and backward through `_ext`.
 
 `DCN_sep_pre_multi_offset` — the only variant C2-Matching instantiates
 (ref_restoration_arch.py:5) — runs its whole tail (offset add + reorder, sigmoid, deformable
@@ -171,3 +173,87 @@ class DCN_sep_pre_multi_offset(_WithOffsetConv):
         out = _ops.dcn_v2_fused_forward(x, om, self.weight, self.bias, self.deformable_groups,
                                         lrelu_slope=lrelu_slope, channels_last_out=channels_last_out, **kw)
         return _ops.psa_from_f32(out) if want_psa else out
+
+
+class _DCNv2Pooling(torch.autograd.Function):
+    """The reference's pooling Function (dcn_v2.py:256-307): forward and backward both cross the `_ext` boundary;
+    gradients flow to `input` and `offset` (the translations), not to `rois`."""
+
+    @staticmethod
+    def forward(ctx, input, rois, offset, spatial_scale, pooled_size, output_dim, no_trans, group_size=1,
+                part_size=None, sample_per_part=4, trans_std=.0):
+        ctx.args = (int(no_trans), spatial_scale, output_dim, group_size, pooled_size,
+                    pooled_size if part_size is None else part_size, sample_per_part, trans_std)
+        output, output_count = _backend.dcn_v2_psroi_pooling_forward(input, rois, offset, *ctx.args)
+        ctx.save_for_backward(input, rois, offset, output_count)
+        return output
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_output):
+        input, rois, offset, output_count = ctx.saved_tensors
+        grad_input, grad_offset = _backend.dcn_v2_psroi_pooling_backward(grad_output.contiguous(), input, rois, offset,
+                                                                         output_count, *ctx.args)
+        return grad_input, None, grad_offset, None, None, None, None, None, None, None, None
+
+
+dcn_v2_pooling = _DCNv2Pooling.apply
+
+
+class DCNv2Pooling(nn.Module):
+    """dcn_v2.py:313-341: pools with the given per-ROI translations `offset` [R, 2K, part, part] (ignored when
+    no_trans)."""
+
+    def __init__(self, spatial_scale, pooled_size, output_dim, no_trans, group_size=1, part_size=None,
+                 sample_per_part=4, trans_std=.0):
+        super().__init__()
+        self.spatial_scale = spatial_scale
+        self.pooled_size = pooled_size
+        self.output_dim = output_dim
+        self.no_trans = no_trans
+        self.group_size = group_size
+        self.part_size = pooled_size if part_size is None else part_size
+        self.sample_per_part = sample_per_part
+        self.trans_std = trans_std
+
+    def _pool(self, input, rois, offset, no_trans):
+        return dcn_v2_pooling(input, rois, offset, self.spatial_scale, self.pooled_size, self.output_dim, no_trans,
+                              self.group_size, self.part_size, self.sample_per_part, self.trans_std)
+
+    def forward(self, input, rois, offset):
+        assert input.shape[1] == self.output_dim
+        if self.no_trans:
+            offset = input.new()
+        return self._pool(input, rois, offset, self.no_trans)
+
+
+class DCNPooling(DCNv2Pooling):
+    """dcn_v2.py:344-411: unless no_trans, predicts one translation and one sigmoid modulation per bin from a first,
+    untranslated pooling through `offset_mask_fc` (last layer zero-initialised, so training starts from plain pooling),
+    then pools again with the translations and multiplies by the modulation."""
+
+    def __init__(self, spatial_scale, pooled_size, output_dim, no_trans, group_size=1, part_size=None,
+                 sample_per_part=4, trans_std=.0, deform_fc_dim=1024):
+        super().__init__(spatial_scale, pooled_size, output_dim, no_trans, group_size, part_size, sample_per_part,
+                         trans_std)
+        self.deform_fc_dim = deform_fc_dim
+        if not no_trans:
+            bins = self.pooled_size * self.pooled_size
+            self.offset_mask_fc = nn.Sequential(
+                nn.Linear(bins * self.output_dim, self.deform_fc_dim), nn.ReLU(inplace=True),
+                nn.Linear(self.deform_fc_dim, self.deform_fc_dim), nn.ReLU(inplace=True),
+                nn.Linear(self.deform_fc_dim, bins * 3))
+            with torch.no_grad():
+                self.offset_mask_fc[4].weight.zero_()
+                self.offset_mask_fc[4].bias.zero_()
+
+    def forward(self, input, rois):
+        offset = input.new()
+        if self.no_trans:
+            return self._pool(input, rois, offset, self.no_trans)
+        n = rois.shape[0]
+        roi = self._pool(input, rois, offset, True)
+        offset_mask = self.offset_mask_fc(roi.view(n, -1)).view(n, 3, self.pooled_size, self.pooled_size)
+        o1, o2, mask = torch.chunk(offset_mask, 3, dim=1)
+        offset = torch.cat((o1, o2), dim=1)
+        return self._pool(input, rois, offset, self.no_trans) * torch.sigmoid(mask)

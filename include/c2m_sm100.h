@@ -18,6 +18,9 @@
  *                                      mmsr/models/archs/corres_generation_arch.py:56-58)
  *   c2m_offset_pyramid_f32          <- index_to_flow + 9-shift x scale pyramid
  *                                      mmsr/models/archs/corres_generation_arch.py:29-46,70-104
+ *   c2m_psroi_pooling_{forward,backward}_{f32,f64}
+ *                                   <- `_ext.dcn_v2_psroi_pooling_forward` / `_backward`
+ *                                      src/dcn_v2.h:75-144, src/cuda/dcn_v2_psroi_pooling_cuda.cu:58-419
  *
  * The Python binding a reference maintainer would add is shown in INTEGRATION.md.
  */
@@ -191,6 +194,46 @@ int c2m_dcn_v2_col2im_coord_f32(const float *gcol, const float *x, const float *
                                 c2m_stream_t stream);
 int c2m_dcn_v2_col2im_f32(const float *gcol, const float *offset, const float *mask, const c2m_dcn_shape *shape,
                           float *grad_input, c2m_stream_t stream);
+
+/* --- deformable PS-ROI pooling (`_ext.dcn_v2_psroi_pooling_forward` / `_backward`) -------------------------------
+ * mmsr/models/archs/DCNv2/src/vision.cpp:3-8 (pybind export), src/dcn_v2.h:75-144 (dispatch),
+ * src/cuda/dcn_v2_psroi_pooling_cuda.cu:58-419 (kernels and host side); called by dcn_v2.py:256-411.
+ * Tensors are contiguous and all of one dtype T (f32 or f64 entry points):
+ *   input [B,C,H,W]; bbox [R,5] rows (batch, x1, y1, x2, y2); trans [R, 2*num_classes, part_size, part_size]
+ *   (unused and may be NULL when no_trans); out, count [R, output_dim, pooled_size, pooled_size].
+ * ROI n: start = round(x1) * spatial_scale - 0.5, end = (round(x2) + 1) * spatial_scale - 0.5 (round half away from
+ * zero), size = max(end - start, 0.1); bin (ph, pw) of size/pooled_size, S = sample_per_part samples per axis at
+ *   start + p * bin + trans[n, cls, {0,1}, part(ph), part(pw)] * trans_std * size + i * bin / S,
+ * part(p) = floor(T(p) / pooled_size * part_size), cls = c / (output_dim / num_classes).  A sample outside
+ * [-0.5, W-0.5] x [-0.5, H-0.5] is dropped; a kept one is clamped to [0, W-1] x [0, H-1] and blends its floor / ceil
+ * corners.  out = mean of the kept samples (0 if none), count = their number.  spatial_scale and trans_std are
+ * float for both dtypes (as in the reference).
+ * Rejected with C2M_ERR_INVALID (the reference reads out of bounds): C != output_dim, group_size != 1, num_classes
+ * not dividing output_dim, pooled_size / part_size / sample_per_part < 1, sample_per_part > 45.  A batch index
+ * int(bbox[n,0]) outside [0,B) gives out 0, count 0 and no gradient.
+ * Backward: grad_input [B,C,H,W] is ACCUMULATED with atomics and grad_trans (shape of trans) is written in a fixed
+ * summation order (bitwise reproducible); the caller zero-fills both.  Each gradient term is divided by top_count.
+ * The workspace (c2m_psroi_pooling_workspace_bytes(shape, sizeof(T)) bytes, 0 when no_trans) holds one partial
+ * trans gradient per output element. */
+typedef struct {
+    int B, C, H, W, R;
+    int no_trans, num_classes;
+    float spatial_scale, trans_std;
+    int output_dim, group_size, pooled_size, part_size, sample_per_part;
+} c2m_psroi_shape;
+
+size_t c2m_psroi_pooling_workspace_bytes(const c2m_psroi_shape *shape, int elem_bytes);
+int c2m_psroi_pooling_forward_f32(const float *input, const float *bbox, const float *trans,
+                                  const c2m_psroi_shape *shape, float *out, float *count, c2m_stream_t stream);
+int c2m_psroi_pooling_forward_f64(const double *input, const double *bbox, const double *trans,
+                                  const c2m_psroi_shape *shape, double *out, double *count, c2m_stream_t stream);
+int c2m_psroi_pooling_backward_f32(const float *out_grad, const float *input, const float *bbox, const float *trans,
+                                   const float *top_count, const c2m_psroi_shape *shape, float *grad_input,
+                                   float *grad_trans, void *ws, size_t ws_bytes, c2m_stream_t stream);
+int c2m_psroi_pooling_backward_f64(const double *out_grad, const double *input, const double *bbox,
+                                   const double *trans, const double *top_count, const c2m_psroi_shape *shape,
+                                   double *grad_input, double *grad_trans, void *ws, size_t ws_bytes,
+                                   c2m_stream_t stream);
 
 /* number of kernels this library has launched since load (bench.py's gpu_launches) */
 unsigned long long c2m_launch_count(void);
