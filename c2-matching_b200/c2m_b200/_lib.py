@@ -55,6 +55,11 @@ class PsroiShape(ctypes.Structure):
                [(n, ctypes.c_int) for n in ('output_dim', 'group_size', 'pooled_size', 'part_size', 'sample_per_part')]
 
 
+_dshape = ctypes.POINTER(DcnShape)
+_deform_fwd = (ctypes.c_int, [ctypes.c_void_p] * 5 + [ctypes.c_int, ctypes.c_void_p, _dshape, ctypes.c_void_p])
+_deform_im2col = (ctypes.c_int, [ctypes.c_void_p] * 3 + [_dshape, ctypes.c_void_p, ctypes.c_void_p])
+_deform_coord = (ctypes.c_int, [ctypes.c_void_p] * 4 + [_dshape] + [ctypes.c_void_p] * 3)
+_deform_col2im = (ctypes.c_int, [ctypes.c_void_p] * 3 + [_dshape, ctypes.c_void_p, ctypes.c_void_p])
 _psroi_fwd = (ctypes.c_int, [ctypes.c_void_p] * 3 + [ctypes.POINTER(PsroiShape)] + [ctypes.c_void_p] * 3)
 _psroi_bwd = (ctypes.c_int, [ctypes.c_void_p] * 5 + [ctypes.POINTER(PsroiShape)] + [ctypes.c_void_p] * 3 +
               [ctypes.c_size_t, ctypes.c_void_p])
@@ -96,6 +101,14 @@ SYMBOLS = {
     'c2m_psroi_pooling_forward_f64': _psroi_fwd,
     'c2m_psroi_pooling_backward_f32': _psroi_bwd,
     'c2m_psroi_pooling_backward_f64': _psroi_bwd,
+    'c2m_deform_conv_forward_f32': _deform_fwd,
+    'c2m_deform_conv_forward_f64': _deform_fwd,
+    'c2m_deform_conv_im2col_f32': _deform_im2col,
+    'c2m_deform_conv_im2col_f64': _deform_im2col,
+    'c2m_deform_conv_col2im_coord_f32': _deform_coord,
+    'c2m_deform_conv_col2im_coord_f64': _deform_coord,
+    'c2m_deform_conv_col2im_f32': _deform_col2im,
+    'c2m_deform_conv_col2im_f64': _deform_col2im,
 }
 
 

@@ -1,4 +1,5 @@
-"""Torch-facing wrappers over the C ABI.  Inputs must be CUDA fp32 tensors; outputs are
+"""Torch-facing wrappers over the C ABI.  Inputs must be CUDA fp32 tensors (fp32 or fp64 for the PS-ROI pooling and
+grouped deformable convolution entries); outputs are
 allocated here with torch (caller-owned in ABI terms) and raw pointers + the current stream
 are handed to the library."""
 import torch
@@ -660,3 +661,138 @@ def dcn_v2_psroi_pooling_backward(out_grad, input, bbox, trans, top_count, no_tr
                                   None if tr is None else grad_trans.data_ptr(),
                                   None if ws is None else ws.data_ptr(), nbytes, _stream()), fn)
     return grad_input, grad_trans
+
+
+# ------------------------------------------------------------------------------------------------
+# Grouped deformable convolution, v1 and modulated (`deform_conv_cuda`, mmsr/models/archs/dcn/src)
+_DEFORM_DTYPES = {torch.float32: 'f32', torch.float64: 'f64'}
+
+
+def _deform_check(input, weight, offset, mask, kernel_h, kernel_w, groups, deformable_group, **more):
+    """Validates dtype, channel / kernel shapes, then devices; returns (B, C, H, W, Cout, dtype suffix)."""
+    if not isinstance(input, torch.Tensor):
+        raise TypeError('input must be a Tensor')
+    dtype = input.dtype
+    if dtype not in _DEFORM_DTYPES:
+        raise RuntimeError(f'deformable convolution supports torch.float32 and torch.float64, got {dtype}')
+    if input.dim() != 4:
+        raise RuntimeError(f'input must be [B, C, H, W], got shape {tuple(input.shape)}')
+    if weight.dim() != 4 or weight.shape[2] != kernel_h or weight.shape[3] != kernel_w:
+        raise RuntimeError(f'Input shape and kernel shape wont match: ({kernel_h} x {kernel_w} vs '
+                           f'{tuple(weight.shape[2:])}).')
+    B, C, H, W = input.shape
+    cout = weight.shape[0]
+    if groups < 1 or C != weight.shape[1] * groups:
+        raise RuntimeError(f'Input shape and kernel channels wont match: ({C} vs {weight.shape[1]} x {groups} groups).')
+    if cout % groups:
+        raise RuntimeError(f'output channels ({cout}) must be divisible by groups ({groups})')
+    if deformable_group < 1 or C % deformable_group:
+        raise RuntimeError(f'input channels ({C}) must be divisible by deformable groups ({deformable_group})')
+    tensors = dict(input=input, weight=weight, offset=offset, mask=mask, **more)
+    for n, t in tensors.items():
+        if t is not None:
+            _require_cuda(n, t, dtype)
+            if t.device != input.device:
+                raise RuntimeError(f'{n} is on {t.device}, input on {input.device}')
+    return B, C, H, W, cout, _DEFORM_DTYPES[dtype]
+
+
+def deform_conv_forward(input, weight, offset, mask, bias, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w,
+                        dilation_h, dilation_w, groups, deformable_group):
+    """Grouped deformable convolution, fp32 or fp64: mask None is DCNv1 (modulation 1), bias None adds nothing.
+    weight [Cout, C/groups, kh, kw]; offset [B, 2*dg*kh*kw, Ho, Wo]; mask [B, dg*kh*kw, Ho, Wo].
+
+    A modulated fp32 call with groups == 1 is exactly `_ext.dcn_v2_forward` (dcn_v2_forward above, zero bias when
+    bias is None), so eligible 3x3 shapes run on the tensor cores there."""
+    B, C, H, W, cout, sfx = _deform_check(input, weight, offset, mask, kernel_h, kernel_w, groups, deformable_group,
+                                          bias=bias)
+    Ho, Wo = _out_hw(H, W, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w)
+    if Ho < 1 or Wo < 1:
+        raise RuntimeError(f'convolution input is too small (output would be {Ho} x {Wo})')
+    T = kernel_h * kernel_w
+    if tuple(offset.shape) != (B, 2 * deformable_group * T, Ho, Wo) or (
+            mask is not None and tuple(mask.shape) != (B, deformable_group * T, Ho, Wo)):
+        raise RuntimeError(f'offset/mask shape mismatch: {tuple(offset.shape)}, '
+                           f'{None if mask is None else tuple(mask.shape)} for output {Ho}x{Wo}')
+    if bias is not None and tuple(bias.shape) != (cout,):
+        raise RuntimeError(f'bias must be [{cout}], got shape {tuple(bias.shape)}')
+    if mask is not None and sfx == 'f32' and groups == 1:
+        if bias is None:
+            bias = torch.zeros(cout, dtype=input.dtype, device=input.device)
+        return dcn_v2_forward(input, weight, bias, offset, mask, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w,
+                              dilation_h, dilation_w, deformable_group)
+    x = _dense_nchw_or_nhwc(input)
+    out = torch.empty(B, cout, Ho, Wo, dtype=x.dtype, device=x.device)
+    s = _shape(x, cout, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w,
+               deformable_group, out)
+    offset = offset.contiguous()
+    mask = mask.contiguous() if mask is not None else None
+    weight = weight.contiguous()
+    bias = bias.contiguous() if bias is not None else None
+    fn = f'c2m_deform_conv_forward_{sfx}'
+    with torch.cuda.device(x.device):
+        _lib.check(getattr(_lib.lib(), fn)(x.data_ptr(), offset.data_ptr(), mask.data_ptr() if mask is not None else None,
+                                           weight.data_ptr(), bias.data_ptr() if bias is not None else None, groups,
+                                           out.data_ptr(), s, _stream()), fn)
+    return out
+
+
+def deform_conv_backward(input, weight, offset, mask, grad_output, kernel_h, kernel_w, stride_h, stride_w, pad_h,
+                         pad_w, dilation_h, dilation_w, groups, deformable_group, need_input=True, need_weight=True):
+    """Gradients of deform_conv_forward -> (grad_input, grad_offset, grad_mask, grad_weight, grad_bias).
+
+    Follows dcn_v2_backward: the deformable pieces are libc2m_sm100 kernels and the two GEMMs are grouped
+    torch.matmul over [groups, ...] views in full fp32 / fp64 (TF32 off):
+        gcol_g = W_g^T gout_g,   grad_W_g = sum_b gout_g col_g^T.
+    grad_mask is None when mask is None.  need_input=False skips grad_input / grad_offset / grad_mask (None),
+    need_weight=False skips grad_weight / grad_bias (None)."""
+    B, C, H, W, cout, sfx = _deform_check(input, weight, offset, mask, kernel_h, kernel_w, groups, deformable_group,
+                                          grad_output=grad_output)
+    x, w = input.contiguous(), weight.contiguous()
+    offset, gout = offset.contiguous(), grad_output.contiguous()
+    mask = mask.contiguous() if mask is not None else None
+    Ho, Wo = _out_hw(H, W, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w)
+    T, P = kernel_h * kernel_w, Ho * Wo
+    if tuple(gout.shape) != (B, cout, Ho, Wo):
+        raise RuntimeError(f'grad_output has shape {tuple(gout.shape)}, expected {(B, cout, Ho, Wo)}')
+    if tuple(offset.shape) != (B, 2 * deformable_group * T, Ho, Wo) or (
+            mask is not None and tuple(mask.shape) != (B, deformable_group * T, Ho, Wo)):
+        raise RuntimeError(f'offset/mask shape mismatch: {tuple(offset.shape)}, '
+                           f'{None if mask is None else tuple(mask.shape)} for output {Ho}x{Wo}')
+    s = _shape(x, cout, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w, deformable_group,
+               gout)
+    L = _lib.lib()
+    mp = mask.data_ptr() if mask is not None else None
+    G, cin_g, cout_g = groups, C // groups, cout // groups
+    grad_input = grad_offset = grad_mask = grad_weight = grad_bias = None
+    prev = torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = False
+    try:
+        with torch.cuda.device(x.device):
+            wg = w.view(G, cout_g, cin_g * T)
+            gg = gout.view(B, G, cout_g, P)
+            columns = None
+            if need_input:
+                gcol = torch.matmul(wg.transpose(1, 2), gg).contiguous()            # [B, G, Cin_g*T, P] = [B, C*T, P]
+                grad_offset = torch.empty_like(offset)
+                grad_mask = torch.empty_like(mask) if mask is not None else None
+                fn = f'c2m_deform_conv_col2im_coord_{sfx}'
+                _lib.check(getattr(L, fn)(gcol.data_ptr(), x.data_ptr(), offset.data_ptr(), mp, s,
+                                          grad_offset.data_ptr(),
+                                          grad_mask.data_ptr() if grad_mask is not None else None, _stream()), fn)
+                grad_input = torch.zeros_like(x)
+                fn = f'c2m_deform_conv_col2im_{sfx}'
+                _lib.check(getattr(L, fn)(gcol.data_ptr(), offset.data_ptr(), mp, s, grad_input.data_ptr(), _stream()),
+                           fn)
+                columns = gcol                                                      # reuse the buffer
+            if need_weight:
+                if columns is None:
+                    columns = torch.empty(B, C * T, P, dtype=x.dtype, device=x.device)
+                fn = f'c2m_deform_conv_im2col_{sfx}'
+                _lib.check(getattr(L, fn)(x.data_ptr(), offset.data_ptr(), mp, s, columns.data_ptr(), _stream()), fn)
+                cg = columns.view(B, G, cin_g * T, P)
+                grad_weight = torch.matmul(gg, cg.transpose(2, 3)).sum(0).view_as(w)
+                grad_bias = gout.sum(dim=(0, 2, 3))
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = prev
+    return grad_input, grad_offset, grad_mask, grad_weight, grad_bias

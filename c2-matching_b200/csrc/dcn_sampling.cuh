@@ -1,6 +1,7 @@
 // The deformable sampling rule of the CUDA-core DCN kernels (dcn_v2.cu, dcn_bwd.cu) and the index-map
 // decode (offsets.cu), stated once.  Arithmetic follows dmcn_im2col_bilinear (dcn_v2_im2col_cuda.cu:25-54,
 // 125-195) operation for operation; keep each expression's order, the kernels' results depend on it bit for bit.
+// The sampling rule is templated on the scalar type: float serves `_ext` and both dtypes serve deform_conv_cuda.
 #pragma once
 #include "c2m_common.cuh"
 
@@ -23,34 +24,41 @@ static inline int dcn_geometry(const c2m_dcn_shape *s, const char *who, DcnGeom 
 }
 
 // Sampling point of tap k at output pixel p (row-major, Wo wide) moved by the final offset (off_h, off_w);
-// false outside -1 < h < H, -1 < w < W, where the sample is 0.
-__device__ __forceinline__ bool dcn_sample_point(const c2m_dcn_shape &s, int Wo, int k, int p, float off_h,
-                                                 float off_w, float &h_im, float &w_im) {
+// false outside -1 < h < H, -1 < w < W, where the sample is 0.  T is the scalar type (float or double) positions are
+// computed in, as the reference's `scalar_t` kernels do.
+template <typename T>
+__device__ __forceinline__ bool dcn_sample_point(const c2m_dcn_shape &s, int Wo, int k, int p, T off_h, T off_w,
+                                                 T &h_im, T &w_im) {
     const int ho = p / Wo, wo = p % Wo, i = k / s.kw, j = k % s.kw;
-    h_im = (float)(ho * s.sh - s.ph + i * s.dh) + off_h;
-    w_im = (float)(wo * s.sw - s.pw + j * s.dw) + off_w;
-    return h_im > -1.f && w_im > -1.f && h_im < (float)s.H && w_im < (float)s.W;
+    h_im = (T)(ho * s.sh - s.ph + i * s.dh) + off_h;
+    w_im = (T)(wo * s.sw - s.pw + j * s.dw) + off_w;
+    return h_im > (T)-1 && w_im > (T)-1 && h_im < (T)s.H && w_im < (T)s.W;
 }
 
-__device__ __forceinline__ float dcn_blend(const float (&w)[4], float v0, float v1, float v2, float v3) {
+template <typename T>
+__device__ __forceinline__ T dcn_blend(const T (&w)[4], T v0, T v1, T v2, T v3) {
     return w[0] * v0 + w[1] * v1 + w[2] * v2 + w[3] * v3;
 }
 
+__device__ __forceinline__ float dcn_floor(float v) { return floorf(v); }
+__device__ __forceinline__ double dcn_floor(double v) { return floor(v); }
+
 // Bilinear corners (low, low), (low, high), (high, low), (high, high) in (row, column) of an in-window point;
 // a corner outside the image is not `ok`.  Offsets are row * ys + column * xs.
+template <typename T>
 struct DcnCorners {
     bool ok[4];
-    float w[4];     // hh*hw, hh*lw, lh*hw, lh*lw with hh = 1 - lh, hw = 1 - lw
-    float lh, lw;
+    T w[4];         // hh*hw, hh*lw, lh*hw, lh*lw with hh = 1 - lh, hw = 1 - lw
+    T lh, lw;
     int o[4];
 
     template <typename S>
-    __device__ __forceinline__ DcnCorners(float h_im, float w_im, int H, int W, S ys, S xs) {
-        const int h_low = (int)floorf(h_im), w_low = (int)floorf(w_im);
+    __device__ __forceinline__ DcnCorners(T h_im, T w_im, int H, int W, S ys, S xs) {
+        const int h_low = (int)dcn_floor(h_im), w_low = (int)dcn_floor(w_im);
         const int h_high = h_low + 1, w_high = w_low + 1;
         lh = h_im - h_low;
         lw = w_im - w_low;
-        const float hh = 1.f - lh, hw = 1.f - lw;
+        const T hh = (T)1 - lh, hw = (T)1 - lw;
         const bool t0 = h_low >= 0, t1 = h_high <= H - 1, l0 = w_low >= 0, l1 = w_high <= W - 1;
         ok[0] = t0 && l0; w[0] = hh * hw; o[0] = (int)(h_low * ys + w_low * xs);
         ok[1] = t0 && l1; w[1] = hh * lw; o[1] = (int)(h_low * ys + w_high * xs);

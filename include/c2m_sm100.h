@@ -21,6 +21,10 @@
  *   c2m_psroi_pooling_{forward,backward}_{f32,f64}
  *                                   <- `_ext.dcn_v2_psroi_pooling_forward` / `_backward`
  *                                      src/dcn_v2.h:75-144, src/cuda/dcn_v2_psroi_pooling_cuda.cu:58-419
+ *   c2m_deform_conv_{forward,im2col,col2im_coord,col2im}_{f32,f64}
+ *                                   <- `deform_conv_cuda` (DCNv1 and grouped DCNv2)
+ *                                      mmsr/models/archs/dcn/src/deform_conv_cuda.cpp:151-695,
+ *                                      src/deform_conv_cuda_kernel.cu
  *
  * The Python binding a reference maintainer would add is shown in INTEGRATION.md.
  */
@@ -194,6 +198,37 @@ int c2m_dcn_v2_col2im_coord_f32(const float *gcol, const float *x, const float *
                                 c2m_stream_t stream);
 int c2m_dcn_v2_col2im_f32(const float *gcol, const float *offset, const float *mask, const c2m_dcn_shape *shape,
                           float *grad_input, c2m_stream_t stream);
+
+/* --- grouped deformable convolution, v1 and modulated (`deform_conv_cuda`, mmsr/models/archs/dcn/src) ---------------
+ * The c2m_dcn_v2_* contract above in fp32 or fp64 (every tensor of one call in that dtype), generalised two ways:
+ *   groups: weight [Cout, C/groups, kh, kw]; output channel o reads the input channels of its conv group
+ *           o / (Cout/groups).  Conv groups and deformable groups partition C independently.
+ *   mask == NULL: modulation 1 (DCNv1, deform_conv_forward_cuda); then grad_mask must be NULL too.
+ * Rejected with C2M_ERR_INVALID: groups < 1, C or Cout not divisible by groups, and the c2m_dcn_v2_* shape errors.
+ * x and out use the shape's element strides in the forward; the backward pieces take NCHW-contiguous tensors, as the
+ * c2m_dcn_v2_* ones do (gcol / columns [B, C*kh*kw, Ho*Wo]; conv groups enter only the caller's GEMMs).
+ * Positions are computed in the dtype, like the reference's `scalar_t` kernels; fp32 with a mask and groups == 1 is
+ * bit for bit c2m_dcn_v2_forward_f32 / _im2col_f32 / _col2im_coord_f32 / _col2im_f32. */
+int c2m_deform_conv_forward_f32(const float *x, const float *offset, const float *mask, const float *weight,
+                                const float *bias, int groups, float *out, const c2m_dcn_shape *shape,
+                                c2m_stream_t stream);
+int c2m_deform_conv_forward_f64(const double *x, const double *offset, const double *mask, const double *weight,
+                                const double *bias, int groups, double *out, const c2m_dcn_shape *shape,
+                                c2m_stream_t stream);
+int c2m_deform_conv_im2col_f32(const float *x, const float *offset, const float *mask, const c2m_dcn_shape *shape,
+                               float *columns, c2m_stream_t stream);
+int c2m_deform_conv_im2col_f64(const double *x, const double *offset, const double *mask, const c2m_dcn_shape *shape,
+                               double *columns, c2m_stream_t stream);
+int c2m_deform_conv_col2im_coord_f32(const float *gcol, const float *x, const float *offset, const float *mask,
+                                     const c2m_dcn_shape *shape, float *grad_offset, float *grad_mask,
+                                     c2m_stream_t stream);
+int c2m_deform_conv_col2im_coord_f64(const double *gcol, const double *x, const double *offset, const double *mask,
+                                     const c2m_dcn_shape *shape, double *grad_offset, double *grad_mask,
+                                     c2m_stream_t stream);
+int c2m_deform_conv_col2im_f32(const float *gcol, const float *offset, const float *mask, const c2m_dcn_shape *shape,
+                               float *grad_input, c2m_stream_t stream);
+int c2m_deform_conv_col2im_f64(const double *gcol, const double *offset, const double *mask,
+                               const c2m_dcn_shape *shape, double *grad_input, c2m_stream_t stream);
 
 /* --- deformable PS-ROI pooling (`_ext.dcn_v2_psroi_pooling_forward` / `_backward`) -------------------------------
  * mmsr/models/archs/DCNv2/src/vision.cpp:3-8 (pybind export), src/dcn_v2.h:75-144 (dispatch),

@@ -34,6 +34,16 @@ y3 = _ext.dcn_v2_forward(x, w, b, off, msk, 3, 3, 1, 1, 1, 1, 1, 1, 8)
 mp = ops.psa_maxpool2(xp)
 xi = ops.psa_interleave(xp)
 back = ops.psa_to_f32(a)
+# grouped deformable convolution, v1 and modulated, fp32 and fp64, forward and backward (3 conv groups of 4 input
+# channels against 2 deformable groups of 6, Cout_g = 7: a partial NO block)
+from mmsr.models.archs.dcn import deform_conv, modulated_deform_conv
+for dt in (torch.float32, torch.float64):
+    xg = seeding.randn(10, (2, 12, 9, 11)).to(dev, dt).requires_grad_(True)
+    wg = seeding.randn(11, (21, 4, 3, 3), 0.2).to(dev, dt).requires_grad_(True)
+    og = seeding.randn(12, (2, 36, 9, 11), 2.0).to(dev, dt).requires_grad_(True)
+    mg = torch.sigmoid(seeding.randn(13, (2, 18, 9, 11))).to(dev, dt).requires_grad_(True)
+    deform_conv(xg, og, wg, 1, 1, 1, 3, 2).sum().backward()
+    modulated_deform_conv(xg, og, mg, wg, None, 1, 1, 1, 3, 2).sum().backward()
 # a search that overflows its candidate lists (constant features: every score ties) -> exhaustive re-scan kernels
 flat = torch.ones(1, 64, 20, 22, device=dev)
 os.environ['C2M_CORR_EXACT_TIES'] = '1'          # no budget: the exhaustive pass must run under the sanitizer
