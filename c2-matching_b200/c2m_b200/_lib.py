@@ -63,6 +63,10 @@ _deform_col2im = (ctypes.c_int, [ctypes.c_void_p] * 3 + [_dshape, ctypes.c_void_
 _psroi_fwd = (ctypes.c_int, [ctypes.c_void_p] * 3 + [ctypes.POINTER(PsroiShape)] + [ctypes.c_void_p] * 3)
 _psroi_bwd = (ctypes.c_int, [ctypes.c_void_p] * 5 + [ctypes.POINTER(PsroiShape)] + [ctypes.c_void_p] * 3 +
               [ctypes.c_size_t, ctypes.c_void_p])
+_deform_col2im_det = (ctypes.c_int, [ctypes.c_void_p] * 3 + [_dshape] + [ctypes.c_void_p] * 2 +
+                      [ctypes.c_size_t, ctypes.c_void_p])
+_psroi_grad_det = (ctypes.c_int, [ctypes.c_void_p] * 4 + [ctypes.POINTER(PsroiShape)] + [ctypes.c_void_p] * 2 +
+                   [ctypes.c_size_t, ctypes.c_void_p])
 
 SYMBOLS = {
     'c2m_abi_version': (ctypes.c_int, []),
@@ -109,6 +113,13 @@ SYMBOLS = {
     'c2m_deform_conv_col2im_coord_f64': _deform_coord,
     'c2m_deform_conv_col2im_f32': _deform_col2im,
     'c2m_deform_conv_col2im_f64': _deform_col2im,
+    'c2m_dcn_col2im_det_workspace_bytes': (ctypes.c_size_t, [_dshape, ctypes.c_int]),
+    'c2m_dcn_v2_col2im_det_f32': _deform_col2im_det,
+    'c2m_deform_conv_col2im_det_f32': _deform_col2im_det,
+    'c2m_deform_conv_col2im_det_f64': _deform_col2im_det,
+    'c2m_psroi_grad_input_det_workspace_bytes': (ctypes.c_size_t, [ctypes.POINTER(PsroiShape), ctypes.c_int]),
+    'c2m_psroi_pooling_grad_input_det_f32': _psroi_grad_det,
+    'c2m_psroi_pooling_grad_input_det_f64': _psroi_grad_det,
 }
 
 

@@ -55,6 +55,50 @@ def _workspace(nbytes, device):
     return buf
 
 
+# ------------------------------------------------------------------------------------------------
+# Ordered input gradients.  With torch.use_deterministic_algorithms(True) (warn_only or not) the three backward entries
+# below compute grad_input with the c2m_*_det entry points, which add every element's contributions in one fixed order
+# (include/c2m_sm100.h, "ordered input gradients"); otherwise the atomic scatters run.
+DET_WORKSPACE_CAP = 1 << 30      # planes per pass are capped so that the workspace stays near this size (>= one plane)
+det_workspace_peak = 0           # largest ordered-gather workspace allocated so far, in bytes (tools/ read and reset it)
+
+
+def deterministic():
+    return torch.are_deterministic_algorithms_enabled()
+
+
+def _det_workspace(query, shape, nplanes, device):
+    """Workspace for an ordered gather: as many planes per pass as fit in DET_WORKSPACE_CAP, at least one.  Call with
+    `device` current (the size query asks CUB, which reads the current device)."""
+    global det_workspace_peak
+    L = _lib.lib()
+    one = query(shape, 1)
+    if one == 0:
+        raise C2MError('ordered input gradient: ' + L.c2m_last_error().decode(errors='replace'))
+    planes = max(1, min(nplanes, DET_WORKSPACE_CAP // one))
+    nbytes = query(shape, planes) if planes > 1 else one
+    if nbytes == 0:
+        raise C2MError('ordered input gradient: ' + L.c2m_last_error().decode(errors='replace'))
+    det_workspace_peak = max(det_workspace_peak, int(nbytes))
+    return torch.empty(int(nbytes), dtype=torch.uint8, device=device)
+
+
+def _col2im(fn_atomic, fn_det, gcol, offset, mask_ptr, s, x):
+    """grad_input of the deformable convolution from gcol: the ordered gather when deterministic algorithms are on,
+    else the atomic scatter into zeros."""
+    L = _lib.lib()
+    if deterministic():
+        grad_input = torch.empty_like(x)
+        ws = _det_workspace(L.c2m_dcn_col2im_det_workspace_bytes, s, s.B * s.dg, x.device)
+        _lib.check(getattr(L, fn_det)(gcol.data_ptr(), offset.data_ptr(), mask_ptr, s, grad_input.data_ptr(),
+                                      ws.data_ptr(), ws.numel(), _stream()), fn_det)
+        return grad_input
+    grad_input = torch.zeros_like(x)
+    _lib.check(getattr(L, fn_atomic)(gcol.data_ptr(), offset.data_ptr(), mask_ptr, s, grad_input.data_ptr(), _stream()),
+               fn_atomic)
+    return grad_input
+
+
 def corr_argmax(feat_in, feat_ref, patch_size=3, input_stride=1, ref_stride=1, is_norm=True,
                 norm_input=False, l2norm=False, force_generic=False):
     """Batched correlation + argmax.  feat_in [B,C,h,w], feat_ref [B,C,hr,wr] ->
@@ -562,9 +606,8 @@ def dcn_v2_backward(input, weight, bias, offset, mask, grad_output, kernel_h, ke
             _lib.check(L.c2m_dcn_v2_col2im_coord_f32(gcol.data_ptr(), x.data_ptr(), offset.data_ptr(), mask.data_ptr(),
                                                      s, grad_offset.data_ptr(), grad_mask.data_ptr(), _stream()),
                        'c2m_dcn_v2_col2im_coord_f32')
-            grad_input = torch.zeros_like(x)
-            _lib.check(L.c2m_dcn_v2_col2im_f32(gcol.data_ptr(), offset.data_ptr(), mask.data_ptr(), s,
-                                               grad_input.data_ptr(), _stream()), 'c2m_dcn_v2_col2im_f32')
+            grad_input = _col2im('c2m_dcn_v2_col2im_f32', 'c2m_dcn_v2_col2im_det_f32', gcol, offset,
+                                 mask.data_ptr(), s, x)
             columns = gcol                                                        # reuse the buffer
             _lib.check(L.c2m_dcn_v2_im2col_f32(x.data_ptr(), offset.data_ptr(), mask.data_ptr(), s, columns.data_ptr(),
                                                _stream()), 'c2m_dcn_v2_im2col_f32')
@@ -637,8 +680,9 @@ def dcn_v2_psroi_pooling_forward(input, bbox, trans, no_trans, spatial_scale, ou
 def dcn_v2_psroi_pooling_backward(out_grad, input, bbox, trans, top_count, no_trans, spatial_scale, output_dim,
                                   group_size, pooled_size, part_size, sample_per_part, trans_std):
     """`_ext.dcn_v2_psroi_pooling_backward` (DCNv2/src/dcn_v2.h:110-144; call site dcn_v2.py:291-304) ->
-    (grad_input, grad_trans).  grad_input is scattered with atomics (summation order not fixed); grad_trans is
-    reduced in a fixed order and is the same bit for bit on every run.  With no_trans, grad_trans is
+    (grad_input, grad_trans).  grad_input is scattered with atomics (summation order not fixed), or, when torch's
+    deterministic algorithms are enabled, gathered in a fixed order; grad_trans is reduced in a fixed order and is the
+    same bit for bit on every run.  With no_trans, grad_trans is
     zeros_like(trans)."""
     s, x, bbox, tr = _psroi_prepare(input, bbox, trans, no_trans, spatial_scale, output_dim, group_size, pooled_size,
                                     part_size, sample_per_part, trans_std)
@@ -651,15 +695,27 @@ def dcn_v2_psroi_pooling_backward(out_grad, input, bbox, trans, top_count, no_tr
     gout, cnt = out_grad.contiguous(), top_count.contiguous()
     L = _lib.lib()
     fn = f'c2m_psroi_pooling_backward_{_psroi_sfx(x.dtype)}'
+    det = deterministic()
     with torch.cuda.device(x.device):
-        grad_input = torch.zeros_like(x)
         grad_trans = torch.zeros_like(trans) if tr is None else torch.zeros_like(tr)
-        nbytes = L.c2m_psroi_pooling_workspace_bytes(s, x.element_size())
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device) if nbytes else None
-        _lib.check(getattr(L, fn)(gout.data_ptr(), x.data_ptr(), bbox.data_ptr(), None if tr is None else tr.data_ptr(),
-                                  cnt.data_ptr(), s, grad_input.data_ptr(),
-                                  None if tr is None else grad_trans.data_ptr(),
-                                  None if ws is None else ws.data_ptr(), nbytes, _stream()), fn)
+        if not det or tr is not None:
+            # grad_trans (and, unless deterministic, grad_input) from the backward kernel; in deterministic mode its
+            # scattered grad_input goes to a scratch buffer and is discarded
+            grad_input = torch.zeros_like(x)
+            nbytes = L.c2m_psroi_pooling_workspace_bytes(s, x.element_size())
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device) if nbytes else None
+            _lib.check(getattr(L, fn)(gout.data_ptr(), x.data_ptr(), bbox.data_ptr(),
+                                      None if tr is None else tr.data_ptr(), cnt.data_ptr(), s, grad_input.data_ptr(),
+                                      None if tr is None else grad_trans.data_ptr(),
+                                      None if ws is None else ws.data_ptr(), nbytes, _stream()), fn)
+        if det:
+            grad_input = torch.empty_like(x)
+            fn = f'c2m_psroi_pooling_grad_input_det_{_psroi_sfx(x.dtype)}'
+            ws = _det_workspace(L.c2m_psroi_grad_input_det_workspace_bytes, s, s.B * (1 if no_trans else s.num_classes),
+                                x.device) if s.R and grad_input.numel() else None
+            _lib.check(getattr(L, fn)(gout.data_ptr(), bbox.data_ptr(), None if tr is None else tr.data_ptr(),
+                                      cnt.data_ptr(), s, grad_input.data_ptr(), None if ws is None else ws.data_ptr(),
+                                      0 if ws is None else ws.numel(), _stream()), fn)
     return grad_input, grad_trans
 
 
@@ -780,10 +836,8 @@ def deform_conv_backward(input, weight, offset, mask, grad_output, kernel_h, ker
                 _lib.check(getattr(L, fn)(gcol.data_ptr(), x.data_ptr(), offset.data_ptr(), mp, s,
                                           grad_offset.data_ptr(),
                                           grad_mask.data_ptr() if grad_mask is not None else None, _stream()), fn)
-                grad_input = torch.zeros_like(x)
-                fn = f'c2m_deform_conv_col2im_{sfx}'
-                _lib.check(getattr(L, fn)(gcol.data_ptr(), offset.data_ptr(), mp, s, grad_input.data_ptr(), _stream()),
-                           fn)
+                grad_input = _col2im(f'c2m_deform_conv_col2im_{sfx}', f'c2m_deform_conv_col2im_det_{sfx}', gcol,
+                                     offset, mp, s, x)
                 columns = gcol                                                      # reuse the buffer
             if need_weight:
                 if columns is None:

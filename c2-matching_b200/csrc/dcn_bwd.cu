@@ -18,6 +18,7 @@
 // (deformable_im2col / col2im / col2im_coord, dcn/src/deform_conv_cuda_kernel.cu:116-434) are these formulas with
 // m = 1, and their 5x5-window scatter reaches the same <= 4 corners.  Conv groups enter only the two GEMMs.
 #include "dcn_sampling.cuh"
+#include "det_gather.cuh"
 
 namespace c2m {
 
@@ -105,7 +106,125 @@ __global__ void dcn_col2im_kernel(const scalar_t *__restrict__ gcol, const scala
     }
 }
 
+// ---- ordered input gradient (det_gather.cuh).  Plane q = (image b, deformable group g) = b * dg + g; its entries are
+// id = (k * P + p) * 4 + corner (corners in DcnCorners order), so ascending id is ascending tap, output pixel, corner.
+
+__device__ __forceinline__ float dcn_add_rn(float a, float b) { return __fadd_rn(a, b); }
+__device__ __forceinline__ double dcn_add_rn(double a, double b) { return __dadd_rn(a, b); }
+
+// one thread per (plane of the pass, tap, p): the four entries of the sampling point
+template <typename scalar_t>
+__global__ void dcn_col2im_emit_kernel(const scalar_t *__restrict__ offset, const c2m_dcn_shape s, const DcnGeom d,
+                                       int q0, int np, uint32_t *__restrict__ keys, uint32_t *__restrict__ ids) {
+    const int T = d.T, P = d.Ho * d.Wo, HW = s.H * s.W;
+    const long long n = (long long)np * T * P;
+    for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x) {
+        const int p = (int)(e % P), k = (int)((e / P) % T), ql = (int)(e / ((long long)P * T));
+        const long long j = (long long)(q0 + ql) * T + k;
+        const uint32_t key0 = (uint32_t)ql * (uint32_t)(HW + 1), id0 = (uint32_t)(k * P + p) * 4u;
+        uint32_t key[4] = {key0 + HW, key0 + HW, key0 + HW, key0 + HW};
+        scalar_t h_im, w_im;
+        if (dcn_sample_point(s, d.Wo, k, p, offset[2 * j * P + p], offset[(2 * j + 1) * P + p], h_im, w_im)) {
+            const DcnCorners<scalar_t> q(h_im, w_im, s.H, s.W, s.W, 1);
+#pragma unroll
+            for (int c = 0; c < 4; ++c)
+                if (q.ok[c]) key[c] = key0 + (uint32_t)q.o[c];
+        }
+        const long long base = (long long)ql * T * P * 4 + id0;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            keys[base + c] = key[c];
+            ids[base + c] = id0 + c;
+        }
+    }
+}
+
+constexpr int DCN_GATHER_CH = 4;   // channels of a deformable group one gather thread accumulates
+
+// one thread per (plane of the pass, run of DCN_GATHER_CH channels of its group, input pixel): walks the pixel's
+// sorted entries, recomputes each one's sampling point once and adds its contribution to every channel of the run,
+// ((gcol * m) * hh) * hw and so on as in dcn_col2im_kernel, with correctly rounded adds from +0.  Writes every element.
+template <typename scalar_t>
+__global__ void dcn_col2im_gather_kernel(const scalar_t *__restrict__ gcol, const scalar_t *__restrict__ offset,
+                                         const scalar_t *__restrict__ mask, const c2m_dcn_shape s, const DcnGeom d,
+                                         int q0, int np, const uint32_t *__restrict__ seg,
+                                         const uint32_t *__restrict__ ids, scalar_t *__restrict__ gx) {
+    const int T = d.T, P = d.Ho * d.Wo, cpg = d.cpg, HW = s.H * s.W;
+    const int runs = ceil_div(cpg, DCN_GATHER_CH);
+    const long long n = (long long)np * runs * HW;
+    for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x) {
+        const int pix = (int)(e % HW), r = (int)((e / HW) % runs), ql = (int)(e / ((long long)HW * runs));
+        const int q = q0 + ql, b = q / s.dg, c0 = (q % s.dg) * cpg + r * DCN_GATHER_CH;
+        const int nc = min(DCN_GATHER_CH, cpg - r * DCN_GATHER_CH);
+        scalar_t acc[DCN_GATHER_CH];
+#pragma unroll
+        for (int i = 0; i < DCN_GATHER_CH; ++i) acc[i] = (scalar_t)0;
+        const uint32_t key = (uint32_t)ql * (uint32_t)(HW + 1) + (uint32_t)pix;
+        for (uint32_t it = seg[key], end = seg[key + 1]; it < end; ++it) {
+            const uint32_t id = ids[it], kp = id >> 2, corner = id & 3u;
+            const int k = (int)(kp / (uint32_t)P), p = (int)(kp % (uint32_t)P);
+            const long long j = (long long)q * T + k;
+            scalar_t h_im, w_im;
+            dcn_sample_point(s, d.Wo, k, p, offset[2 * j * P + p], offset[(2 * j + 1) * P + p], h_im, w_im);
+            const DcnCorners<scalar_t> cq(h_im, w_im, s.H, s.W, s.W, 1);
+            const scalar_t wa = corner < 2 ? (scalar_t)1 - cq.lh : cq.lh;
+            const scalar_t wb = (corner & 1u) ? cq.lw : (scalar_t)1 - cq.lw;
+            const scalar_t m = mask ? mask[j * P + p] : (scalar_t)1;
+            const scalar_t *gc = gcol + (((long long)b * s.C + c0) * T + k) * P + p;
+#pragma unroll
+            for (int i = 0; i < DCN_GATHER_CH; ++i)
+                if (i < nc) acc[i] = dcn_add_rn(acc[i], gc[(long long)i * T * P] * m * wa * wb);
+        }
+        scalar_t *out = gx + ((long long)b * s.C + c0) * HW + pix;
+#pragma unroll
+        for (int i = 0; i < DCN_GATHER_CH; ++i)
+            if (i < nc) out[(long long)i * HW] = acc[i];
+    }
+}
+
 static inline int blocks_for(long long n) { long long b = (n + 255) / 256; return (int)(b > 132 * 16 ? 132 * 16 : b); }
+
+// Entries and keys of one plane; false (error set) when a plane exceeds the 32-bit entry id.
+static bool dcn_det_plane(const c2m_dcn_shape *shape, const DcnGeom &d, const char *who, long long &entries,
+                          long long &keys) {
+    entries = 4ll * d.T * d.Ho * d.Wo;
+    keys = (long long)shape->H * shape->W + 1;
+    if (entries > 0xFFFFFFFFll || keys > 0xFFFFFFFFll) {
+        set_error("%s: a plane of %lld entries exceeds the 32-bit entry id", who, entries);
+        return false;
+    }
+    return true;
+}
+
+template <typename scalar_t>
+static int col2im_det(const scalar_t *gcol, const scalar_t *offset, const scalar_t *mask, const c2m_dcn_shape *shape,
+                      scalar_t *grad_input, void *ws, size_t ws_bytes, c2m_stream_t stream) {
+    DcnGeom d;
+    if (int rc = dcn_geometry(shape, "dcn ordered col2im", d)) return rc;
+    long long E, K;
+    if (!dcn_det_plane(shape, d, "dcn ordered col2im", E, K)) return C2M_ERR_INVALID;
+    const long long nplanes = (long long)shape->B * shape->dg;
+    C2M_CHECK_ARG(ws, "dcn ordered col2im: null workspace");
+    const int np = det_planes_per_pass(ws_bytes, nplanes, E, K);
+    C2M_CHECK_ARG(np >= 1, "dcn ordered col2im: workspace of %zu bytes holds no plane (%zu needed)", ws_bytes,
+                  det_workspace_bytes(1, nplanes, E, K, "dcn ordered col2im"));
+    const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const int runs = ceil_div(d.cpg, DCN_GATHER_CH);
+    DetLayout L;
+    C2M_CUDA(det_layout(ws, np * E, np * K, L));
+    for (long long q0 = 0; q0 < nplanes; q0 += np) {
+        const int n = (int)(nplanes - q0 < np ? nplanes - q0 : np);
+        dcn_col2im_emit_kernel<<<blocks_for((long long)n * d.T * d.Ho * d.Wo), 256, 0, st>>>(
+            offset, *shape, d, (int)q0, n, L.keys[0], L.vals[0]);
+        C2M_LAUNCH_CHECK("dcn_col2im_emit_kernel");
+        int sorted;
+        if (int rc = det_sort_segments(L, (uint32_t)(n * E), (uint32_t)(n * K), sorted, st)) return rc;
+        dcn_col2im_gather_kernel<<<blocks_for((long long)n * runs * shape->H * shape->W), 256, 0, st>>>(
+            gcol, offset, mask, *shape, d, (int)q0, n, L.seg, L.vals[sorted], grad_input);
+        C2M_LAUNCH_CHECK("dcn_col2im_gather_kernel");
+    }
+    return C2M_OK;
+}
 
 template <typename scalar_t>
 static int im2col(const scalar_t *x, const scalar_t *offset, const scalar_t *mask, const c2m_dcn_shape *shape,
@@ -187,3 +306,30 @@ extern "C" int c2m_dcn_v2_col2im_f32(const float *gcol, const float *offset, con
 
 C2M_DEFORM_CONV_BWD(float, f32)
 C2M_DEFORM_CONV_BWD(double, f64)
+
+// ordered input gradient: grad_input written (not accumulated), in the order of col2im_det
+extern "C" size_t c2m_dcn_col2im_det_workspace_bytes(const c2m_dcn_shape *shape, int planes) {
+    DcnGeom d;
+    if (dcn_geometry(shape, "dcn_col2im_det_workspace_bytes", d)) return 0;
+    long long E, K;
+    if (!dcn_det_plane(shape, d, "dcn_col2im_det_workspace_bytes", E, K)) return 0;
+    return det_workspace_bytes(planes, (long long)shape->B * shape->dg, E, K, "dcn_col2im_det_workspace_bytes");
+}
+
+extern "C" int c2m_dcn_v2_col2im_det_f32(const float *gcol, const float *offset, const float *mask,
+                                         const c2m_dcn_shape *shape, float *grad_input, void *ws, size_t ws_bytes,
+                                         c2m_stream_t stream) {
+    C2M_CHECK_ARG(gcol && offset && mask && grad_input, "dcn_v2_col2im_det: null pointer");
+    return col2im_det(gcol, offset, mask, shape, grad_input, ws, ws_bytes, stream);
+}
+
+#define C2M_DEFORM_CONV_COL2IM_DET(T, SFX)                                                                          \
+    extern "C" int c2m_deform_conv_col2im_det_##SFX(const T *gcol, const T *offset, const T *mask,                  \
+                                                    const c2m_dcn_shape *shape, T *grad_input, void *ws,            \
+                                                    size_t ws_bytes, c2m_stream_t stream) {                         \
+        C2M_CHECK_ARG(gcol && offset && grad_input, "deform_conv_col2im_det: null pointer");                        \
+        return col2im_det(gcol, offset, mask, shape, grad_input, ws, ws_bytes, stream);                             \
+    }
+
+C2M_DEFORM_CONV_COL2IM_DET(float, f32)
+C2M_DEFORM_CONV_COL2IM_DET(double, f64)

@@ -14,13 +14,15 @@
 //
 // Backward: grad_input is scattered with atomicAdd (summation order arbitrary).  grad_trans is reproducible bit for bit:
 // each (ROI, channel, bin) writes its partial sum over samples to a caller-owned workspace, and a second kernel adds the
-// partials of each (ROI, class, part cell) in a fixed order (bins ascending, then channels ascending).
+// partials of each (ROI, class, part cell) in a fixed order (bins ascending, then channels ascending).  With torch's
+// deterministic algorithms on, grad_input comes instead from the ordered gather below (det_gather.cuh).
 //
 // Deliberate differences from the reference, which reads out of bounds in each case: C != output_dim, group_size != 1,
 // a class count that does not divide output_dim and pooled_size / part_size / sample_per_part below 1 are rejected
 // (C2M_ERR_INVALID); an ROI whose batch index, truncated toward zero, lies outside [0, B) pools to 0 with count 0 and
 // receives no gradient.
 #include "c2m_common.cuh"
+#include "det_gather.cuh"
 
 namespace c2m {
 
@@ -88,6 +90,26 @@ __device__ __forceinline__ void psroi_sample(T w, T h, int H, int W, int &code, 
     code = ((y0 * W + x0) << 2) | (x1 != x0 ? 1 : 0) | (y1 != y0 ? 2 : 0);
 }
 
+// Position (w, h) of sample (ih, iw) of bin (ph, pw) of ROI n (geometry r) for class cls, translated by trans unless
+// no_trans; psroi_sample turns it into corners.
+template <typename T>
+__device__ __forceinline__ void psroi_position(const PsroiRoi<T> &r, const T *trans, const c2m_psroi_shape &s, int n,
+                                               int cls, int ph, int pw, int ih, int iw, T &w, T &h) {
+    const int P = s.pooled_size, part = s.part_size;
+    T tx = (T)0, ty = (T)0;
+    if (!s.no_trans) {
+        const int pcell = psroi_part<T>(ph, P, part) * part + psroi_part<T>(pw, P, part);
+        const long long t0 = (((long long)n * s.num_classes + cls) * 2) * part * part + pcell;
+        const T tstd = (T)s.trans_std;
+        tx = rn_mul(trans[t0], tstd);
+        ty = rn_mul(trans[t0 + (long long)part * part], tstd);
+    }
+    const T ws = rn_add(rn_add(rn_mul((T)pw, r.bin_w), r.start_w), rn_mul(tx, r.width));
+    const T hs = rn_add(rn_add(rn_mul((T)ph, r.bin_h), r.start_h), rn_mul(ty, r.height));
+    w = rn_add(ws, rn_mul((T)iw, r.sub_w));
+    h = rn_add(hs, rn_mul((T)ih, r.sub_h));
+}
+
 // Shared-memory sample table of `nb` bins starting at bin0, S*S samples each: sample s = ih * S + iw of bin j at
 // s * nb + j, so the threads of a warp, which walk consecutive bins, read consecutive words (no bank conflicts).  The
 // ROI's translation for (class, part cell) is read from trans unless no_trans.
@@ -104,7 +126,7 @@ struct PsroiTable {
 
     __device__ void fill(const PsroiRoi<T> &r, const T *trans, const c2m_psroi_shape &s, int n, int cls, int bin0,
                          int nb) {
-        const int P = s.pooled_size, S = s.sample_per_part, SS = S * S, part = s.part_size;
+        const int P = s.pooled_size, S = s.sample_per_part, SS = S * S;
         for (int i = threadIdx.x; i < nb * SS; i += blockDim.x) {
             const int bin = bin0 + i % nb, ph = bin / P, pw = bin % P, ih = (i / nb) / S, iw = (i / nb) % S;
             if (r.b < 0) {
@@ -112,18 +134,8 @@ struct PsroiTable {
                 lx[i] = ly[i] = (T)0;
                 continue;
             }
-            T tx = (T)0, ty = (T)0;
-            if (!s.no_trans) {
-                const int pcell = psroi_part<T>(ph, P, part) * part + psroi_part<T>(pw, P, part);
-                const long long t0 = (((long long)n * s.num_classes + cls) * 2) * part * part + pcell;
-                const T tstd = (T)s.trans_std;
-                tx = rn_mul(trans[t0], tstd);
-                ty = rn_mul(trans[t0 + (long long)part * part], tstd);
-            }
-            const T ws = rn_add(rn_add(rn_mul((T)pw, r.bin_w), r.start_w), rn_mul(tx, r.width));
-            const T hs = rn_add(rn_add(rn_mul((T)ph, r.bin_h), r.start_h), rn_mul(ty, r.height));
-            const T w = rn_add(ws, rn_mul((T)iw, r.sub_w));
-            const T h = rn_add(hs, rn_mul((T)ih, r.sub_h));
+            T w, h;
+            psroi_position(r, trans, s, n, cls, ph, pw, ih, iw, w, h);
             psroi_sample(w, h, s.H, s.W, code[i], lx[i], ly[i]);
         }
     }
@@ -268,6 +280,100 @@ __global__ void psroi_trans_grad_kernel(const T *__restrict__ ws, const c2m_psro
     }
 }
 
+// ---- ordered grad_input (det_gather.cuh).  Plane q = (image b, class cls) = b * K + cls; its entries are
+// id = ((n * PP + bin) * SS + sample) * 4 + corner with corners floor, +dy, +dx, +dx+dy, so ascending id is ascending
+// ROI, bin (row-major), sample (row-major), corner.  Entries of ROIs of other images, dropped samples and corners that
+// coincide with the floor corner get the "no pixel" key.
+
+// one thread per (plane of the pass, ROI, bin, sample)
+template <typename T>
+__global__ void psroi_grad_emit_kernel(const T *__restrict__ bbox, const T *__restrict__ trans,
+                                       const c2m_psroi_shape s, int q0, int np, uint32_t *__restrict__ keys,
+                                       uint32_t *__restrict__ ids) {
+    const int P = s.pooled_size, PP = P * P, S = s.sample_per_part, SS = S * S, HW = s.H * s.W;
+    const long long per = (long long)s.R * PP * SS, total = np * per;
+    for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total;
+         e += (long long)gridDim.x * blockDim.x) {
+        const long long local = e % per;
+        const int si = (int)(local % SS), bin = (int)((local / SS) % PP), n = (int)(local / ((long long)SS * PP));
+        const int ql = (int)(e / per), q = q0 + ql, b = q / s.num_classes, cls = q % s.num_classes;
+        const uint32_t key0 = (uint32_t)ql * (uint32_t)(HW + 1);
+        uint32_t key[4] = {key0 + HW, key0 + HW, key0 + HW, key0 + HW};
+        const PsroiRoi<T> roi(bbox + (long long)n * 5, s);
+        if (roi.b == b) {
+            int code;
+            T lx, ly;
+            T w, h;
+            psroi_position(roi, trans, s, n, cls, bin / P, bin % P, si / S, si % S, w, h);
+            psroi_sample(w, h, s.H, s.W, code, lx, ly);
+            if (code >= 0) {
+                int o, dx, dy;
+                psroi_corners(code, s.W, o, dx, dy);
+                key[0] = key0 + (uint32_t)o;
+                if (dy) key[1] = key0 + (uint32_t)(o + dy);
+                if (dx) key[2] = key0 + (uint32_t)(o + dx);
+                if (dx && dy) key[3] = key0 + (uint32_t)(o + dx + dy);
+            }
+        }
+        const uint32_t id0 = (uint32_t)local * 4u;
+        const long long base = ql * per * 4 + id0;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            keys[base + c] = key[c];
+            ids[base + c] = id0 + c;
+        }
+    }
+}
+
+constexpr int PS_GATHER_CH = 4;    // channels of a class one gather thread accumulates
+
+// one thread per (plane of the pass, run of PS_GATHER_CH channels of its class, input pixel): walks the pixel's sorted
+// entries, recomputes each sample once and adds (hx * hy) * (out_grad / count) and so on, as psroi_bwd_kernel, to
+// every channel of the run whose count is positive, with correctly rounded adds from +0.  Writes every element.
+template <typename T>
+__global__ void psroi_grad_gather_kernel(const T *__restrict__ gout, const T *__restrict__ bbox,
+                                         const T *__restrict__ trans, const T *__restrict__ top_count,
+                                         const c2m_psroi_shape s, int q0, int np, const uint32_t *__restrict__ seg,
+                                         const uint32_t *__restrict__ ids, T *__restrict__ gx) {
+    const int P = s.pooled_size, PP = P * P, S = s.sample_per_part, SS = S * S, HW = s.H * s.W;
+    const int cpc = s.output_dim / s.num_classes, runs = ceil_div(cpc, PS_GATHER_CH);
+    const long long total = (long long)np * runs * HW;
+    for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total;
+         e += (long long)gridDim.x * blockDim.x) {
+        const int pix = (int)(e % HW), r = (int)((e / HW) % runs), ql = (int)(e / ((long long)HW * runs));
+        const int q = q0 + ql, b = q / s.num_classes, cls = q % s.num_classes;
+        const int c0 = cls * cpc + r * PS_GATHER_CH, nc = min(PS_GATHER_CH, cpc - r * PS_GATHER_CH);
+        T acc[PS_GATHER_CH];
+#pragma unroll
+        for (int i = 0; i < PS_GATHER_CH; ++i) acc[i] = (T)0;
+        const uint32_t key = (uint32_t)ql * (uint32_t)(HW + 1) + (uint32_t)pix;
+        for (uint32_t it = seg[key], end = seg[key + 1]; it < end; ++it) {
+            const uint32_t id = ids[it], t = id >> 2, corner = id & 3u;
+            const int si = (int)(t % (uint32_t)SS), bin = (int)((t / (uint32_t)SS) % (uint32_t)PP);
+            const int n = (int)(t / ((uint32_t)SS * (uint32_t)PP));
+            const PsroiRoi<T> roi(bbox + (long long)n * 5, s);
+            int code;
+            T lx, ly;
+            T w, h;
+            psroi_position(roi, trans, s, n, cls, bin / P, bin % P, si / S, si % S, w, h);
+            psroi_sample(w, h, s.H, s.W, code, lx, ly);
+            const T hx = (T)1 - lx, hy = (T)1 - ly;
+            const T wgt = corner == 0 ? hx * hy : corner == 1 ? hx * ly : corner == 2 ? lx * hy : lx * ly;
+            const long long oi0 = ((long long)n * s.output_dim + c0) * PP + bin;
+#pragma unroll
+            for (int i = 0; i < PS_GATHER_CH; ++i) {
+                if (i >= nc) continue;
+                const T cnt = top_count[oi0 + (long long)i * PP];
+                if (cnt > (T)0) acc[i] = rn_add(acc[i], wgt * (gout[oi0 + (long long)i * PP] / cnt));
+            }
+        }
+        T *out = gx + ((long long)b * s.C + c0) * HW + pix;
+#pragma unroll
+        for (int i = 0; i < PS_GATHER_CH; ++i)
+            if (i < nc) out[(long long)i * HW] = acc[i];
+    }
+}
+
 static int psroi_check(const c2m_psroi_shape *s, const char *what) {
     C2M_CHECK_ARG(s, "%s: null shape", what);
     C2M_CHECK_ARG(s->B >= 0 && s->C >= 0 && s->H >= 0 && s->W >= 0 && s->R >= 0 && s->output_dim >= 0,
@@ -361,6 +467,56 @@ static int psroi_backward(const T *gout, const T *x, const T *bbox, const T *tra
     return C2M_OK;
 }
 
+// Entries and keys of one (image, class) plane; false (error set) when a plane exceeds the 32-bit entry id.
+static bool psroi_det_plane(const c2m_psroi_shape &s, const char *who, long long &entries, long long &keys) {
+    entries = 4ll * s.R * s.pooled_size * s.pooled_size * s.sample_per_part * s.sample_per_part;
+    keys = (long long)s.H * s.W + 1;
+    if (entries > 0xFFFFFFFFll || keys > 0xFFFFFFFFll) {
+        set_error("%s: a plane of %lld entries exceeds the 32-bit entry id", who, entries);
+        return false;
+    }
+    return true;
+}
+
+template <typename T>
+static int psroi_grad_input_det(const T *gout, const T *bbox, const T *trans, const T *top_count,
+                                const c2m_psroi_shape *shape, T *grad_input, void *ws, size_t ws_bytes,
+                                c2m_stream_t stream) {
+    const char *who = "psroi_pooling_grad_input_det";
+    if (int rc = psroi_check(shape, who)) return rc;
+    const c2m_psroi_shape s = psroi_effective(*shape);
+    const long long nx = (long long)s.B * s.C * s.H * s.W;
+    if (nx == 0) return C2M_OK;
+    C2M_CHECK_ARG(grad_input, "%s: null pointer", who);
+    const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if (s.R == 0) {                                       // no ROI: every element is +0
+        C2M_CUDA(cudaMemsetAsync(grad_input, 0, (size_t)nx * sizeof(T), st));
+        return C2M_OK;
+    }
+    C2M_CHECK_ARG(gout && bbox && top_count && (s.no_trans || trans) && ws, "%s: null pointer", who);
+    long long E, K;
+    if (!psroi_det_plane(s, who, E, K)) return C2M_ERR_INVALID;
+    const long long nplanes = (long long)s.B * s.num_classes;
+    const int np = det_planes_per_pass(ws_bytes, nplanes, E, K);
+    C2M_CHECK_ARG(np >= 1, "%s: workspace of %zu bytes holds no plane (%zu needed)", who, ws_bytes,
+                  det_workspace_bytes(1, nplanes, E, K, who));
+    const int runs = ceil_div(s.output_dim / s.num_classes, PS_GATHER_CH);
+    DetLayout L;
+    C2M_CUDA(det_layout(ws, np * E, np * K, L));
+    auto blocks = [](long long n) { const long long b = (n + 255) / 256; return (int)(b < 132 * 16 ? b : 132 * 16); };
+    for (long long q0 = 0; q0 < nplanes; q0 += np) {
+        const int n = (int)(nplanes - q0 < np ? nplanes - q0 : np);
+        psroi_grad_emit_kernel<T><<<blocks(n * E / 4), 256, 0, st>>>(bbox, trans, s, (int)q0, n, L.keys[0], L.vals[0]);
+        C2M_LAUNCH_CHECK("psroi_grad_emit_kernel");
+        int sorted;
+        if (int rc = det_sort_segments(L, (uint32_t)(n * E), (uint32_t)(n * K), sorted, st)) return rc;
+        psroi_grad_gather_kernel<T><<<blocks((long long)n * runs * s.H * s.W), 256, 0, st>>>(
+            gout, bbox, trans, top_count, s, (int)q0, n, L.seg, L.vals[sorted], grad_input);
+        C2M_LAUNCH_CHECK("psroi_grad_gather_kernel");
+    }
+    return C2M_OK;
+}
+
 }  // namespace c2m
 
 using namespace c2m;
@@ -394,4 +550,27 @@ extern "C" int c2m_psroi_pooling_backward_f64(const double *out_grad, const doub
                                               const c2m_psroi_shape *shape, double *grad_input, double *grad_trans,
                                               void *ws, size_t ws_bytes, c2m_stream_t stream) {
     return psroi_backward(out_grad, input, bbox, trans, top_count, shape, grad_input, grad_trans, ws, ws_bytes, stream);
+}
+
+extern "C" size_t c2m_psroi_grad_input_det_workspace_bytes(const c2m_psroi_shape *shape, int planes) {
+    const char *who = "psroi_grad_input_det_workspace_bytes";
+    if (psroi_check(shape, who)) return 0;
+    const c2m_psroi_shape s = psroi_effective(*shape);
+    long long E, K;
+    if (!psroi_det_plane(s, who, E, K)) return 0;
+    return det_workspace_bytes(planes, (long long)s.B * s.num_classes, E, K, who);
+}
+
+extern "C" int c2m_psroi_pooling_grad_input_det_f32(const float *out_grad, const float *bbox, const float *trans,
+                                                    const float *top_count, const c2m_psroi_shape *shape,
+                                                    float *grad_input, void *ws, size_t ws_bytes,
+                                                    c2m_stream_t stream) {
+    return psroi_grad_input_det(out_grad, bbox, trans, top_count, shape, grad_input, ws, ws_bytes, stream);
+}
+
+extern "C" int c2m_psroi_pooling_grad_input_det_f64(const double *out_grad, const double *bbox, const double *trans,
+                                                    const double *top_count, const c2m_psroi_shape *shape,
+                                                    double *grad_input, void *ws, size_t ws_bytes,
+                                                    c2m_stream_t stream) {
+    return psroi_grad_input_det(out_grad, bbox, trans, top_count, shape, grad_input, ws, ws_bytes, stream);
 }

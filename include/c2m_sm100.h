@@ -230,6 +230,32 @@ int c2m_deform_conv_col2im_f32(const float *gcol, const float *offset, const flo
 int c2m_deform_conv_col2im_f64(const double *gcol, const double *offset, const double *mask,
                                const c2m_dcn_shape *shape, double *grad_input, c2m_stream_t stream);
 
+/* --- ordered input gradients (used when torch's deterministic algorithms are enabled) -----------------------------
+ * Same results as the col2im / PS-ROI grad_input scatters above, except that every element of grad_input is a sum in
+ * one fixed order, so it is the same bit for bit on every run, and that grad_input is WRITTEN (every element, +0
+ * where nothing contributes), not accumulated.  Each contribution is the scatter's own expression; an element starts
+ * at +0 and adds its contributions with correctly rounded adds in this order:
+ *   DCN (c2m_dcn_v2_col2im_det_f32, c2m_deform_conv_col2im_det_{f32,f64}; arguments as c2m_*_col2im_*): over the
+ *     sampling points of deformable group c / (C/dg) of image b, ascending tap, then output pixel, then corner
+ *     (low-low, low-high, high-low, high-high); in-image corners only.
+ *   PS-ROI (c2m_psroi_pooling_grad_input_det_{f32,f64}; arguments as the backward, without input and grad_trans): over
+ *     the ROIs with batch index b, ascending ROI, then bin (row-major), then sample (row-major), then corner (floor,
+ *     +y, +x, +x+y), skipping dropped samples, corners that coincide with the floor corner and outputs with count <= 0.
+ * A plane is one (image, deformable group) for DCN and one (image, class) for PS-ROI.  The workspace is caller-owned:
+ * c2m_*_det_workspace_bytes(shape, planes) is the size that processes `planes` planes per pass (clamped to
+ * [1, planes in the call]); the entry points process as many planes per pass as ws_bytes holds, at least one.  The
+ * one-plane size does not depend on B.  A plane of 2^32 or more contributions is rejected (C2M_ERR_INVALID; the
+ * queries return 0).  The size queries ask CUB for its sort storage and so need a current CUDA device. */
+size_t c2m_dcn_col2im_det_workspace_bytes(const c2m_dcn_shape *shape, int planes);
+int c2m_dcn_v2_col2im_det_f32(const float *gcol, const float *offset, const float *mask, const c2m_dcn_shape *shape,
+                              float *grad_input, void *ws, size_t ws_bytes, c2m_stream_t stream);
+int c2m_deform_conv_col2im_det_f32(const float *gcol, const float *offset, const float *mask,
+                                   const c2m_dcn_shape *shape, float *grad_input, void *ws, size_t ws_bytes,
+                                   c2m_stream_t stream);
+int c2m_deform_conv_col2im_det_f64(const double *gcol, const double *offset, const double *mask,
+                                   const c2m_dcn_shape *shape, double *grad_input, void *ws, size_t ws_bytes,
+                                   c2m_stream_t stream);
+
 /* --- deformable PS-ROI pooling (`_ext.dcn_v2_psroi_pooling_forward` / `_backward`) -------------------------------
  * mmsr/models/archs/DCNv2/src/vision.cpp:3-8 (pybind export), src/dcn_v2.h:75-144 (dispatch),
  * src/cuda/dcn_v2_psroi_pooling_cuda.cu:58-419 (kernels and host side); called by dcn_v2.py:256-411.
@@ -269,6 +295,15 @@ int c2m_psroi_pooling_backward_f64(const double *out_grad, const double *input, 
                                    const double *trans, const double *top_count, const c2m_psroi_shape *shape,
                                    double *grad_input, double *grad_trans, void *ws, size_t ws_bytes,
                                    c2m_stream_t stream);
+
+/* ordered PS-ROI grad_input: see "ordered input gradients" above */
+size_t c2m_psroi_grad_input_det_workspace_bytes(const c2m_psroi_shape *shape, int planes);
+int c2m_psroi_pooling_grad_input_det_f32(const float *out_grad, const float *bbox, const float *trans,
+                                         const float *top_count, const c2m_psroi_shape *shape, float *grad_input,
+                                         void *ws, size_t ws_bytes, c2m_stream_t stream);
+int c2m_psroi_pooling_grad_input_det_f64(const double *out_grad, const double *bbox, const double *trans,
+                                         const double *top_count, const c2m_psroi_shape *shape, double *grad_input,
+                                         void *ws, size_t ws_bytes, c2m_stream_t stream);
 
 /* number of kernels this library has launched since load (bench.py's gpu_launches) */
 unsigned long long c2m_launch_count(void);
