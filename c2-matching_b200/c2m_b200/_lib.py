@@ -81,9 +81,6 @@ SYMBOLS = {
     'c2m_conv3x3': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
     'c2m_psa_interleave': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 4 + [ctypes.c_void_p] * 2),
     'c2m_psa_maxpool2': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 4 + [ctypes.c_void_p] * 3),
-    'c2m_dcn_v2_im2col_f32': (ctypes.c_int, [c_f32p] * 3 + [ctypes.POINTER(DcnShape), c_f32p, ctypes.c_void_p]),
-    'c2m_dcn_v2_col2im_coord_f32': (ctypes.c_int, [c_f32p] * 4 + [ctypes.POINTER(DcnShape), c_f32p, c_f32p, ctypes.c_void_p]),
-    'c2m_dcn_v2_col2im_f32': (ctypes.c_int, [c_f32p] * 3 + [ctypes.POINTER(DcnShape), c_f32p, ctypes.c_void_p]),
     'c2m_dcn_tc_supported': (ctypes.c_int, [ctypes.c_int] * 3),
     'c2m_dcn_tc_packed_weight_bytes': (ctypes.c_size_t, [ctypes.c_int] * 3),
     'c2m_dcn_tc_pack_weights_f32': (ctypes.c_int, [c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
@@ -96,7 +93,6 @@ SYMBOLS = {
                                                                                  ctypes.c_void_p, ctypes.c_size_t,
                                                                                  ctypes.c_void_p]),
     'c2m_offset_pyramid_f32': (ctypes.c_int, [c_i64p] + [ctypes.c_int] * 5 + [c_f32p, ctypes.c_void_p]),
-    'c2m_dcn_v2_forward_f32': (ctypes.c_int, [c_f32p] * 6 + [ctypes.POINTER(DcnShape), ctypes.c_void_p]),
     'c2m_dcn_v2_fused_forward_f32': (ctypes.c_int, [c_f32p, c_f32p, c_f32p, c_i64p] + [ctypes.c_int] * 4 +
                                      [c_f32p, c_f32p, ctypes.c_float, c_f32p, ctypes.POINTER(DcnShape),
                                       ctypes.c_void_p]),
@@ -114,7 +110,6 @@ SYMBOLS = {
     'c2m_deform_conv_col2im_f32': _deform_col2im,
     'c2m_deform_conv_col2im_f64': _deform_col2im,
     'c2m_dcn_col2im_det_workspace_bytes': (ctypes.c_size_t, [_dshape, ctypes.c_int]),
-    'c2m_dcn_v2_col2im_det_f32': _deform_col2im_det,
     'c2m_deform_conv_col2im_det_f32': _deform_col2im_det,
     'c2m_deform_conv_col2im_det_f64': _deform_col2im_det,
     'c2m_psroi_grad_input_det_workspace_bytes': (ctypes.c_size_t, [ctypes.POINTER(PsroiShape), ctypes.c_int]),
@@ -127,7 +122,7 @@ class C2MError(RuntimeError):
     pass
 
 
-EXPECTED_ABI = 5      # c2m_abi_version() the ctypes structs above mirror (include/c2m_sm100.h)
+EXPECTED_ABI = 6      # c2m_abi_version() the ctypes structs above mirror (include/c2m_sm100.h)
 
 
 def lib():

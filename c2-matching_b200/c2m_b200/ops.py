@@ -83,19 +83,20 @@ def _det_workspace(query, shape, nplanes, device):
     return torch.empty(int(nbytes), dtype=torch.uint8, device=device)
 
 
-def _col2im(fn_atomic, fn_det, gcol, offset, mask_ptr, s, x):
+def _col2im(sfx, gcol, offset, mask_ptr, s, x):
     """grad_input of the deformable convolution from gcol: the ordered gather when deterministic algorithms are on,
     else the atomic scatter into zeros."""
     L = _lib.lib()
     if deterministic():
         grad_input = torch.empty_like(x)
         ws = _det_workspace(L.c2m_dcn_col2im_det_workspace_bytes, s, s.B * s.dg, x.device)
-        _lib.check(getattr(L, fn_det)(gcol.data_ptr(), offset.data_ptr(), mask_ptr, s, grad_input.data_ptr(),
-                                      ws.data_ptr(), ws.numel(), _stream()), fn_det)
+        fn = f'c2m_deform_conv_col2im_det_{sfx}'
+        _lib.check(getattr(L, fn)(gcol.data_ptr(), offset.data_ptr(), mask_ptr, s, grad_input.data_ptr(),
+                                  ws.data_ptr(), ws.numel(), _stream()), fn)
         return grad_input
     grad_input = torch.zeros_like(x)
-    _lib.check(getattr(L, fn_atomic)(gcol.data_ptr(), offset.data_ptr(), mask_ptr, s, grad_input.data_ptr(), _stream()),
-               fn_atomic)
+    fn = f'c2m_deform_conv_col2im_{sfx}'
+    _lib.check(getattr(L, fn)(gcol.data_ptr(), offset.data_ptr(), mask_ptr, s, grad_input.data_ptr(), _stream()), fn)
     return grad_input
 
 
@@ -209,15 +210,9 @@ def dcn_v2_forward(input, weight, bias, offset, mask, kernel_h, kernel_w, stride
         # in one pass, final offsets / mask read as given, fp32 NCHW out.  The FFMA kernel below stays the general
         # path (any kernel size / stride / dilation / group width).
         return dcn_v2_fused_tc(x, offset.contiguous(), weight, bias, deformable_group, final_mask=mask.contiguous())
-    out = torch.empty(B, weight.shape[0], Ho, Wo, dtype=torch.float32, device=x.device)
-    s = _shape(x, weight.shape[0], kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w,
-               deformable_group, out)
-    with torch.cuda.device(x.device):
-        rc = _lib.lib().c2m_dcn_v2_forward_f32(x.data_ptr(), offset.contiguous().data_ptr(),
-                                               mask.contiguous().data_ptr(), weight.contiguous().data_ptr(),
-                                               bias.contiguous().data_ptr(), out.data_ptr(), s, _stream())
-        _lib.check(rc, 'c2m_dcn_v2_forward_f32')
-    return out
+    return _deform_forward(x, weight, offset, mask, bias, Ho, Wo,
+                           (kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w), 1,
+                           deformable_group)
 
 
 def dcn_v2_fused_forward(x, om, weight, bias, deformable_group, pre_offset=None, idx=None, pre_scale=1,
@@ -578,9 +573,8 @@ def dcn_v2_fused_tc(x, om, weight, bias, deformable_group, pre_offset=None, idx=
 def dcn_v2_backward(input, weight, bias, offset, mask, grad_output, kernel_h, kernel_w, stride_h, stride_w, pad_h,
                     pad_w, dilation_h, dilation_w, deformable_group):
     """`_ext.dcn_v2_backward` (DCNv2/src/dcn_v2.h:41-72; call site dcn_v2.py:38-47) ->
-    [grad_input, grad_offset, grad_mask, grad_weight, grad_bias].  The deformable pieces
-    (im2col, coordinate/mask gradient, input scatter) are libc2m_sm100 kernels; the two dense
-    GEMMs are torch.matmul in full fp32."""
+    [grad_input, grad_offset, grad_mask, grad_weight, grad_bias]: the groups = 1 case of deform_conv_backward,
+    behind `_ext`'s own checks."""
     for n, t in (('input', input), ('weight', weight), ('bias', bias), ('offset', offset), ('mask', mask),
                  ('grad_output', grad_output)):
         _require_cuda(n, t)
@@ -589,33 +583,11 @@ def dcn_v2_backward(input, weight, bias, offset, mask, grad_output, kernel_h, ke
     B, C, H, W = x.shape
     cout = w.shape[0]
     Ho, Wo = _out_hw(H, W, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w)
-    T, P = kernel_h * kernel_w, Ho * Wo
     if tuple(gout.shape) != (B, cout, Ho, Wo):
         raise RuntimeError(f'grad_output has shape {tuple(gout.shape)}, expected {(B, cout, Ho, Wo)}')
     s = _shape(x, cout, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w, deformable_group,
                gout)
-    L = _lib.lib()
-    prev = torch.backends.cuda.matmul.allow_tf32
-    torch.backends.cuda.matmul.allow_tf32 = False
-    try:
-        with torch.cuda.device(x.device):
-            w2 = w.view(cout, C * T)
-            g2 = gout.view(B, cout, P)
-            gcol = torch.matmul(w2.t(), g2).contiguous()                          # [B, C*T, P]
-            grad_offset, grad_mask = torch.empty_like(offset), torch.empty_like(mask)
-            _lib.check(L.c2m_dcn_v2_col2im_coord_f32(gcol.data_ptr(), x.data_ptr(), offset.data_ptr(), mask.data_ptr(),
-                                                     s, grad_offset.data_ptr(), grad_mask.data_ptr(), _stream()),
-                       'c2m_dcn_v2_col2im_coord_f32')
-            grad_input = _col2im('c2m_dcn_v2_col2im_f32', 'c2m_dcn_v2_col2im_det_f32', gcol, offset,
-                                 mask.data_ptr(), s, x)
-            columns = gcol                                                        # reuse the buffer
-            _lib.check(L.c2m_dcn_v2_im2col_f32(x.data_ptr(), offset.data_ptr(), mask.data_ptr(), s, columns.data_ptr(),
-                                               _stream()), 'c2m_dcn_v2_im2col_f32')
-            grad_weight = torch.matmul(g2, columns.transpose(1, 2)).sum(0).view_as(w)
-            grad_bias = gout.sum(dim=(0, 2, 3))
-    finally:
-        torch.backends.cuda.matmul.allow_tf32 = prev
-    return [grad_input, grad_offset, grad_mask, grad_weight, grad_bias]
+    return list(_deform_backward(x, w, offset, mask, gout, s, 1, True, True))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -777,15 +749,21 @@ def deform_conv_forward(input, weight, offset, mask, bias, kernel_h, kernel_w, s
             bias = torch.zeros(cout, dtype=input.dtype, device=input.device)
         return dcn_v2_forward(input, weight, bias, offset, mask, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w,
                               dilation_h, dilation_w, deformable_group)
-    x = _dense_nchw_or_nhwc(input)
-    out = torch.empty(B, cout, Ho, Wo, dtype=x.dtype, device=x.device)
-    s = _shape(x, cout, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w,
-               deformable_group, out)
-    offset = offset.contiguous()
+    return _deform_forward(_dense_nchw_or_nhwc(input), weight, offset, mask, bias, Ho, Wo,
+                           (kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w), groups,
+                           deformable_group)
+
+
+def _deform_forward(x, weight, offset, mask, bias, Ho, Wo, geom, groups, deformable_group):
+    """The CUDA-core forward (c2m_deform_conv_forward_*) on checked tensors of one dtype; x dense NCHW or channels-last,
+    geom = (kh, kw, sh, sw, ph, pw, dh, dw), mask / bias may be None."""
+    cout = weight.shape[0]
+    out = torch.empty(x.shape[0], cout, Ho, Wo, dtype=x.dtype, device=x.device)
+    s = _shape(x, cout, *geom, deformable_group, out)
+    offset, weight = offset.contiguous(), weight.contiguous()
     mask = mask.contiguous() if mask is not None else None
-    weight = weight.contiguous()
     bias = bias.contiguous() if bias is not None else None
-    fn = f'c2m_deform_conv_forward_{sfx}'
+    fn = f'c2m_deform_conv_forward_{_DEFORM_DTYPES[x.dtype]}'
     with torch.cuda.device(x.device):
         _lib.check(getattr(_lib.lib(), fn)(x.data_ptr(), offset.data_ptr(), mask.data_ptr() if mask is not None else None,
                                            weight.data_ptr(), bias.data_ptr() if bias is not None else None, groups,
@@ -797,18 +775,18 @@ def deform_conv_backward(input, weight, offset, mask, grad_output, kernel_h, ker
                          pad_w, dilation_h, dilation_w, groups, deformable_group, need_input=True, need_weight=True):
     """Gradients of deform_conv_forward -> (grad_input, grad_offset, grad_mask, grad_weight, grad_bias).
 
-    Follows dcn_v2_backward: the deformable pieces are libc2m_sm100 kernels and the two GEMMs are grouped
-    torch.matmul over [groups, ...] views in full fp32 / fp64 (TF32 off):
+    The deformable pieces are libc2m_sm100 kernels and the two GEMMs are grouped torch.matmul over [groups, ...] views
+    in full fp32 / fp64 (TF32 off):
         gcol_g = W_g^T gout_g,   grad_W_g = sum_b gout_g col_g^T.
     grad_mask is None when mask is None.  need_input=False skips grad_input / grad_offset / grad_mask (None),
     need_weight=False skips grad_weight / grad_bias (None)."""
-    B, C, H, W, cout, sfx = _deform_check(input, weight, offset, mask, kernel_h, kernel_w, groups, deformable_group,
-                                          grad_output=grad_output)
+    B, C, H, W, cout, _ = _deform_check(input, weight, offset, mask, kernel_h, kernel_w, groups, deformable_group,
+                                        grad_output=grad_output)
     x, w = input.contiguous(), weight.contiguous()
     offset, gout = offset.contiguous(), grad_output.contiguous()
     mask = mask.contiguous() if mask is not None else None
     Ho, Wo = _out_hw(H, W, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w)
-    T, P = kernel_h * kernel_w, Ho * Wo
+    T = kernel_h * kernel_w
     if tuple(gout.shape) != (B, cout, Ho, Wo):
         raise RuntimeError(f'grad_output has shape {tuple(gout.shape)}, expected {(B, cout, Ho, Wo)}')
     if tuple(offset.shape) != (B, 2 * deformable_group * T, Ho, Wo) or (
@@ -817,6 +795,15 @@ def deform_conv_backward(input, weight, offset, mask, grad_output, kernel_h, ker
                            f'{None if mask is None else tuple(mask.shape)} for output {Ho}x{Wo}')
     s = _shape(x, cout, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w, deformable_group,
                gout)
+    return _deform_backward(x, w, offset, mask, gout, s, groups, need_input, need_weight)
+
+
+def _deform_backward(x, w, offset, mask, gout, s, groups, need_input, need_weight):
+    """deform_conv_backward on checked, contiguous tensors of one dtype and their DcnShape `s`."""
+    B, C = x.shape[:2]
+    cout = w.shape[0]
+    T, P = s.kh * s.kw, gout.shape[2] * gout.shape[3]
+    sfx = _DEFORM_DTYPES[x.dtype]
     L = _lib.lib()
     mp = mask.data_ptr() if mask is not None else None
     G, cin_g, cout_g = groups, C // groups, cout // groups
@@ -836,8 +823,7 @@ def deform_conv_backward(input, weight, offset, mask, grad_output, kernel_h, ker
                 _lib.check(getattr(L, fn)(gcol.data_ptr(), x.data_ptr(), offset.data_ptr(), mp, s,
                                           grad_offset.data_ptr(),
                                           grad_mask.data_ptr() if grad_mask is not None else None, _stream()), fn)
-                grad_input = _col2im(f'c2m_deform_conv_col2im_{sfx}', f'c2m_deform_conv_col2im_det_{sfx}', gcol,
-                                     offset, mp, s, x)
+                grad_input = _col2im(sfx, gcol, offset, mp, s, x)
                 columns = gcol                                                      # reuse the buffer
             if need_weight:
                 if columns is None:

@@ -54,6 +54,12 @@ void prof_end(void *handle, cudaStream_t st);
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 __host__ __device__ static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
+// Blocks of 256 threads for a grid-stride loop over n items: one per 256 items, at most 16 per SM of an H100.
+static inline int grid_blocks(long long n) {
+    const long long b = (n + 255) / 256;
+    return (int)(b < 132 * 16 ? b : 132 * 16);
+}
+
 // number of SMs of the current device (the persistent kernels launch at most one CTA per SM)
 static inline cudaError_t sm_count(int &sms) {
     int dev = 0;

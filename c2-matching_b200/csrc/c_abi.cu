@@ -122,7 +122,9 @@ static void carve(CorrWorkspace &ws, const CorrGeom &g, uint8_t *base) {
 
 using namespace c2m;
 
-extern "C" int c2m_abi_version(void) { return 5; }   // 5: c2m_dcn_tc_args without x_hi / x_lo; 4: .x_il + c2m_psa_interleave; 3: .mask; 2: out_f32_octets / om_octets
+// 6: no fp32 c2m_dcn_v2_* twins of c2m_deform_conv_*; 5: c2m_dcn_tc_args without x_hi / x_lo; 4: .x_il +
+// c2m_psa_interleave; 3: .mask; 2: out_f32_octets / om_octets
+extern "C" int c2m_abi_version(void) { return 6; }
 extern "C" const char *c2m_last_error(void) { return g_err; }
 extern "C" unsigned long long c2m_launch_count(void) { return g_launches.load(); }
 

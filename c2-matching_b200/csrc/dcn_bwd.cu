@@ -5,18 +5,18 @@
 // decomposition — column-gradient GEMM, coordinate/mask gradient, input-gradient scatter, column
 // matrix for the weight gradient — with the two dense GEMMs left to the caller (torch.matmul) and
 // the three deformable pieces written here:
-//   c2m_dcn_v2_im2col_f32        columns[b, c*T+k, p] = mask * bilinear(x)          (:125-195)
-//   c2m_dcn_v2_col2im_coord_f32  grad_offset / grad_mask from gcol                   (:256-327, 83-123)
-//   c2m_dcn_v2_col2im_f32        grad_input += scatter of gcol * mask                (:197-254, 56-80)
+//   c2m_deform_conv_im2col_*        columns[b, c*T+k, p] = mask * bilinear(x)       (:125-195)
+//   c2m_deform_conv_col2im_coord_*  grad_offset / grad_mask from gcol                (:256-327, 83-123)
+//   c2m_deform_conv_col2im_*        grad_input += scatter of gcol * mask             (:197-254, 56-80)
 // Unlike the reference, batch is a grid dimension (no host loop), grad_input scatter touches only
 // the (<= 4) contributing corners instead of a 5x5 window, and launch errors are returned.
 // Sampling points, corners and the shape check are the forward's (dcn_sampling.cuh); a corner
 // outside the image is skipped here, where the forward loads element 0 with weight 0.
 //
-// The kernels are templated on the scalar type and also serve `deform_conv_cuda` (mmsr/models/archs/dcn):
-// a null mask is a modulation of 1 and then no grad_mask is written.  The reference's DCNv1 kernels
-// (deformable_im2col / col2im / col2im_coord, dcn/src/deform_conv_cuda_kernel.cu:116-434) are these formulas with
-// m = 1, and their 5x5-window scatter reaches the same <= 4 corners.  Conv groups enter only the two GEMMs.
+// The kernels are templated on the scalar type and serve `_ext` (fp32, with a mask) and `deform_conv_cuda`
+// (mmsr/models/archs/dcn): a null mask is a modulation of 1 and then no grad_mask is written.  The reference's DCNv1
+// kernels (deformable_im2col / col2im / col2im_coord, dcn/src/deform_conv_cuda_kernel.cu:116-434) are these formulas
+// with m = 1, and their 5x5-window scatter reaches the same <= 4 corners.  Conv groups enter only the two GEMMs.
 #include "dcn_sampling.cuh"
 #include "det_gather.cuh"
 
@@ -182,48 +182,28 @@ __global__ void dcn_col2im_gather_kernel(const scalar_t *__restrict__ gcol, cons
     }
 }
 
-static inline int blocks_for(long long n) { long long b = (n + 255) / 256; return (int)(b > 132 * 16 ? 132 * 16 : b); }
-
-// Entries and keys of one plane; false (error set) when a plane exceeds the 32-bit entry id.
-static bool dcn_det_plane(const c2m_dcn_shape *shape, const DcnGeom &d, const char *who, long long &entries,
-                          long long &keys) {
-    entries = 4ll * d.T * d.Ho * d.Wo;
-    keys = (long long)shape->H * shape->W + 1;
-    if (entries > 0xFFFFFFFFll || keys > 0xFFFFFFFFll) {
-        set_error("%s: a plane of %lld entries exceeds the 32-bit entry id", who, entries);
-        return false;
-    }
-    return true;
-}
-
 template <typename scalar_t>
 static int col2im_det(const scalar_t *gcol, const scalar_t *offset, const scalar_t *mask, const c2m_dcn_shape *shape,
                       scalar_t *grad_input, void *ws, size_t ws_bytes, c2m_stream_t stream) {
     DcnGeom d;
     if (int rc = dcn_geometry(shape, "dcn ordered col2im", d)) return rc;
-    long long E, K;
-    if (!dcn_det_plane(shape, d, "dcn ordered col2im", E, K)) return C2M_ERR_INVALID;
-    const long long nplanes = (long long)shape->B * shape->dg;
-    C2M_CHECK_ARG(ws, "dcn ordered col2im: null workspace");
-    const int np = det_planes_per_pass(ws_bytes, nplanes, E, K);
-    C2M_CHECK_ARG(np >= 1, "dcn ordered col2im: workspace of %zu bytes holds no plane (%zu needed)", ws_bytes,
-                  det_workspace_bytes(1, nplanes, E, K, "dcn ordered col2im"));
+    const long long E = 4ll * d.T * d.Ho * d.Wo, K = (long long)shape->H * shape->W + 1;
+    if (!det_plane_fits(E, K, "dcn ordered col2im")) return C2M_ERR_INVALID;
     const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const int runs = ceil_div(d.cpg, DCN_GATHER_CH);
-    DetLayout L;
-    C2M_CUDA(det_layout(ws, np * E, np * K, L));
-    for (long long q0 = 0; q0 < nplanes; q0 += np) {
-        const int n = (int)(nplanes - q0 < np ? nplanes - q0 : np);
-        dcn_col2im_emit_kernel<<<blocks_for((long long)n * d.T * d.Ho * d.Wo), 256, 0, st>>>(
-            offset, *shape, d, (int)q0, n, L.keys[0], L.vals[0]);
+    auto emit = [&](int q0, int n, uint32_t *keys, uint32_t *ids) -> int {
+        dcn_col2im_emit_kernel<<<grid_blocks((long long)n * d.T * d.Ho * d.Wo), 256, 0, st>>>(offset, *shape, d, q0, n,
+                                                                                             keys, ids);
         C2M_LAUNCH_CHECK("dcn_col2im_emit_kernel");
-        int sorted;
-        if (int rc = det_sort_segments(L, (uint32_t)(n * E), (uint32_t)(n * K), sorted, st)) return rc;
-        dcn_col2im_gather_kernel<<<blocks_for((long long)n * runs * shape->H * shape->W), 256, 0, st>>>(
-            gcol, offset, mask, *shape, d, (int)q0, n, L.seg, L.vals[sorted], grad_input);
+        return C2M_OK;
+    };
+    auto gather = [&](int q0, int n, const uint32_t *seg, const uint32_t *ids) -> int {
+        dcn_col2im_gather_kernel<<<grid_blocks((long long)n * runs * shape->H * shape->W), 256, 0, st>>>(
+            gcol, offset, mask, *shape, d, q0, n, seg, ids, grad_input);
         C2M_LAUNCH_CHECK("dcn_col2im_gather_kernel");
-    }
-    return C2M_OK;
+        return C2M_OK;
+    };
+    return det_passes(ws, ws_bytes, (long long)shape->B * shape->dg, E, K, "dcn ordered col2im", st, emit, gather);
 }
 
 template <typename scalar_t>
@@ -231,7 +211,7 @@ static int im2col(const scalar_t *x, const scalar_t *offset, const scalar_t *mas
                   scalar_t *columns, c2m_stream_t stream) {
     DcnGeom d;
     if (int rc = dcn_geometry(shape, "dcn backward", d)) return rc;
-    dcn_im2col_kernel<<<blocks_for((long long)shape->B * shape->C * d.Ho * d.Wo), 256, 0,
+    dcn_im2col_kernel<<<grid_blocks((long long)shape->B * shape->C * d.Ho * d.Wo), 256, 0,
                         reinterpret_cast<cudaStream_t>(stream)>>>(x, offset, mask, *shape, d, columns);
     C2M_LAUNCH_CHECK("dcn_im2col_kernel");
     return C2M_OK;
@@ -242,7 +222,7 @@ static int col2im_coord(const scalar_t *gcol, const scalar_t *x, const scalar_t 
                         const c2m_dcn_shape *shape, scalar_t *grad_offset, scalar_t *grad_mask, c2m_stream_t stream) {
     DcnGeom d;
     if (int rc = dcn_geometry(shape, "dcn backward", d)) return rc;
-    dcn_col2im_coord_kernel<<<blocks_for((long long)shape->B * shape->dg * d.T * d.Ho * d.Wo), 256, 0,
+    dcn_col2im_coord_kernel<<<grid_blocks((long long)shape->B * shape->dg * d.T * d.Ho * d.Wo), 256, 0,
                               reinterpret_cast<cudaStream_t>(stream)>>>(gcol, x, offset, mask, *shape, d, grad_offset,
                                                                         grad_mask);
     C2M_LAUNCH_CHECK("dcn_col2im_coord_kernel");
@@ -254,7 +234,7 @@ static int col2im(const scalar_t *gcol, const scalar_t *offset, const scalar_t *
                   scalar_t *grad_input, c2m_stream_t stream) {
     DcnGeom d;
     if (int rc = dcn_geometry(shape, "dcn backward", d)) return rc;
-    dcn_col2im_kernel<<<blocks_for((long long)shape->B * shape->C * d.T * d.Ho * d.Wo), 256, 0,
+    dcn_col2im_kernel<<<grid_blocks((long long)shape->B * shape->C * d.T * d.Ho * d.Wo), 256, 0,
                         reinterpret_cast<cudaStream_t>(stream)>>>(gcol, offset, mask, *shape, d, grad_input);
     C2M_LAUNCH_CHECK("dcn_col2im_kernel");
     return C2M_OK;
@@ -264,26 +244,7 @@ static int col2im(const scalar_t *gcol, const scalar_t *offset, const scalar_t *
 
 using namespace c2m;
 
-extern "C" int c2m_dcn_v2_im2col_f32(const float *x, const float *offset, const float *mask, const c2m_dcn_shape *shape,
-                                     float *columns, c2m_stream_t stream) {
-    C2M_CHECK_ARG(x && offset && mask && columns, "dcn_v2_im2col: null pointer");
-    return im2col(x, offset, mask, shape, columns, stream);
-}
-
-extern "C" int c2m_dcn_v2_col2im_coord_f32(const float *gcol, const float *x, const float *offset, const float *mask,
-                                           const c2m_dcn_shape *shape, float *grad_offset, float *grad_mask,
-                                           c2m_stream_t stream) {
-    C2M_CHECK_ARG(gcol && x && offset && mask && grad_offset && grad_mask, "dcn_v2_col2im_coord: null pointer");
-    return col2im_coord(gcol, x, offset, mask, shape, grad_offset, grad_mask, stream);
-}
-
-extern "C" int c2m_dcn_v2_col2im_f32(const float *gcol, const float *offset, const float *mask, const c2m_dcn_shape *shape,
-                                     float *grad_input, c2m_stream_t stream) {
-    C2M_CHECK_ARG(gcol && offset && mask && grad_input, "dcn_v2_col2im: null pointer");
-    return col2im(gcol, offset, mask, shape, grad_input, stream);
-}
-
-// deform_conv_cuda: mask may be NULL (DCNv1), and grad_mask is NULL exactly when mask is
+// mask may be NULL (DCNv1), and grad_mask is NULL exactly when mask is
 #define C2M_DEFORM_CONV_BWD(T, SFX)                                                                                 \
     extern "C" int c2m_deform_conv_im2col_##SFX(const T *x, const T *offset, const T *mask,                         \
                                                 const c2m_dcn_shape *shape, T *columns, c2m_stream_t stream) {      \
@@ -311,16 +272,9 @@ C2M_DEFORM_CONV_BWD(double, f64)
 extern "C" size_t c2m_dcn_col2im_det_workspace_bytes(const c2m_dcn_shape *shape, int planes) {
     DcnGeom d;
     if (dcn_geometry(shape, "dcn_col2im_det_workspace_bytes", d)) return 0;
-    long long E, K;
-    if (!dcn_det_plane(shape, d, "dcn_col2im_det_workspace_bytes", E, K)) return 0;
+    const long long E = 4ll * d.T * d.Ho * d.Wo, K = (long long)shape->H * shape->W + 1;
+    if (!det_plane_fits(E, K, "dcn_col2im_det_workspace_bytes")) return 0;
     return det_workspace_bytes(planes, (long long)shape->B * shape->dg, E, K, "dcn_col2im_det_workspace_bytes");
-}
-
-extern "C" int c2m_dcn_v2_col2im_det_f32(const float *gcol, const float *offset, const float *mask,
-                                         const c2m_dcn_shape *shape, float *grad_input, void *ws, size_t ws_bytes,
-                                         c2m_stream_t stream) {
-    C2M_CHECK_ARG(gcol && offset && mask && grad_input, "dcn_v2_col2im_det: null pointer");
-    return col2im_det(gcol, offset, mask, shape, grad_input, ws, ws_bytes, stream);
 }
 
 #define C2M_DEFORM_CONV_COL2IM_DET(T, SFX)                                                                          \

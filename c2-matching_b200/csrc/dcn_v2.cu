@@ -266,35 +266,29 @@ static int dcn_launch(DcnArgs<scalar_t> a, const char *who, cudaStream_t st) {
 template <typename scalar_t>
 static int deform_forward(const scalar_t *x, const scalar_t *offset, const scalar_t *mask, const scalar_t *weight,
                           const scalar_t *bias, int groups, scalar_t *out, const c2m_dcn_shape *shape,
-                          c2m_stream_t stream, const char *who) {
+                          c2m_stream_t stream) {
     DcnArgs<scalar_t> a = {};
     a.x = x; a.offset = offset; a.mask = mask; a.weight = weight; a.bias = bias; a.out = out;
     a.s = *shape;
     a.slope = 1.f;
     a.groups = groups;
-    return dcn_launch(a, who, reinterpret_cast<cudaStream_t>(stream));
+    return dcn_launch(a, "deform_conv", reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // namespace c2m
-
-extern "C" int c2m_dcn_v2_forward_f32(const float *x, const float *offset, const float *mask, const float *weight,
-                                      const float *bias, float *out, const c2m_dcn_shape *shape, c2m_stream_t stream) {
-    C2M_CHECK_ARG(x && offset && mask && weight && out && shape, "dcn_v2_forward: null pointer");
-    return c2m::deform_forward(x, offset, mask, weight, bias, 1, out, shape, stream, "dcn_v2");
-}
 
 extern "C" int c2m_deform_conv_forward_f32(const float *x, const float *offset, const float *mask,
                                            const float *weight, const float *bias, int groups, float *out,
                                            const c2m_dcn_shape *shape, c2m_stream_t stream) {
     C2M_CHECK_ARG(x && offset && weight && out && shape, "deform_conv_forward: null pointer");
-    return c2m::deform_forward(x, offset, mask, weight, bias, groups, out, shape, stream, "deform_conv");
+    return c2m::deform_forward(x, offset, mask, weight, bias, groups, out, shape, stream);
 }
 
 extern "C" int c2m_deform_conv_forward_f64(const double *x, const double *offset, const double *mask,
                                            const double *weight, const double *bias, int groups, double *out,
                                            const c2m_dcn_shape *shape, c2m_stream_t stream) {
     C2M_CHECK_ARG(x && offset && weight && out && shape, "deform_conv_forward: null pointer");
-    return c2m::deform_forward(x, offset, mask, weight, bias, groups, out, shape, stream, "deform_conv");
+    return c2m::deform_forward(x, offset, mask, weight, bias, groups, out, shape, stream);
 }
 
 extern "C" int c2m_dcn_v2_fused_forward_f32(const float *x, const float *om, const float *pre, const int64_t *idx,

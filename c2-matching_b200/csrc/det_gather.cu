@@ -58,14 +58,19 @@ int det_sort_segments(DetLayout &L, uint32_t n, uint32_t nkeys, int &sorted, cud
     C2M_CUDA(cub::DeviceRadixSort::SortPairs(L.temp, temp_bytes, k, v, n, 0, key_bits(nkeys), st));
     C2M_LAUNCH_CHECK("cub::DeviceRadixSort::SortPairs");
     sorted = k.selector;
-    const long long blocks = ((long long)nkeys + 255) / 256;
-    det_segments_kernel<<<(int)(blocks < 132 * 16 ? blocks : 132 * 16), 256, 0, st>>>(k.Current(), n, nkeys, L.seg);
+    det_segments_kernel<<<grid_blocks(nkeys), 256, 0, st>>>(k.Current(), n, nkeys, L.seg);
     C2M_LAUNCH_CHECK("det_segments_kernel");
     return C2M_OK;
 }
 
 static bool pass_fits_32bit(long long planes, long long entries_per_plane, long long keys_per_plane) {
     return planes * entries_per_plane <= 0xFFFFFFFFll && planes * keys_per_plane <= 0xFFFFFFFFll;
+}
+
+bool det_plane_fits(long long entries, long long keys, const char *who) {
+    if (pass_fits_32bit(1, entries, keys)) return true;
+    set_error("%s: a plane of %lld entries exceeds the 32-bit entry id", who, entries);
+    return false;
 }
 
 size_t det_workspace_bytes(long long planes, long long nplanes, long long entries_per_plane, long long keys_per_plane,

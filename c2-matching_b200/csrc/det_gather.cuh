@@ -39,4 +39,29 @@ int det_planes_per_pass(size_t ws_bytes, long long nplanes, long long entries_pe
 size_t det_workspace_bytes(long long planes, long long nplanes, long long entries_per_plane, long long keys_per_plane,
                            const char *who);
 
+// False, with the error set, when one plane of `entries` entries and `keys` keys exceeds the 32-bit entry id.
+bool det_plane_fits(long long entries, long long keys, const char *who);
+
+// Steps 1-4 over `nplanes` planes of E entries and K keys each, as many planes per pass as ws_bytes holds:
+// emit(q0, n, keys, ids) writes the pairs of planes [q0, q0 + n), gather(q0, n, seg, ids) adds them up from the
+// segment starts and the sorted ids.  Both return a status.
+template <typename Emit, typename Gather>
+int det_passes(void *ws, size_t ws_bytes, long long nplanes, long long E, long long K, const char *who,
+               cudaStream_t st, Emit emit, Gather gather) {
+    C2M_CHECK_ARG(ws, "%s: null workspace", who);
+    const int np = det_planes_per_pass(ws_bytes, nplanes, E, K);
+    C2M_CHECK_ARG(np >= 1, "%s: workspace of %zu bytes holds no plane (%zu needed)", who, ws_bytes,
+                  det_workspace_bytes(1, nplanes, E, K, who));
+    DetLayout L;
+    C2M_CUDA(det_layout(ws, np * E, np * K, L));
+    for (long long q0 = 0; q0 < nplanes; q0 += np) {
+        const int n = (int)(nplanes - q0 < np ? nplanes - q0 : np);
+        if (int rc = emit((int)q0, n, L.keys[0], L.vals[0])) return rc;
+        int sorted;
+        if (int rc = det_sort_segments(L, (uint32_t)(n * E), (uint32_t)(n * K), sorted, st)) return rc;
+        if (int rc = gather((int)q0, n, L.seg, L.vals[sorted])) return rc;
+    }
+    return C2M_OK;
+}
+
 }  // namespace c2m

@@ -460,22 +460,10 @@ static int psroi_backward(const T *gout, const T *x, const T *bbox, const T *tra
     C2M_LAUNCH_CHECK("psroi_bwd_kernel");
     if (!s.no_trans) {
         const long long cells = (long long)s.R * s.num_classes * s.part_size * s.part_size;
-        const int blocks = (int)((cells + 255) / 256 < 132 * 16 ? (cells + 255) / 256 : 132 * 16);
-        psroi_trans_grad_kernel<T><<<blocks, 256, 0, st>>>(static_cast<const T *>(ws), s, grad_trans);
+        psroi_trans_grad_kernel<T><<<grid_blocks(cells), 256, 0, st>>>(static_cast<const T *>(ws), s, grad_trans);
         C2M_LAUNCH_CHECK("psroi_trans_grad_kernel");
     }
     return C2M_OK;
-}
-
-// Entries and keys of one (image, class) plane; false (error set) when a plane exceeds the 32-bit entry id.
-static bool psroi_det_plane(const c2m_psroi_shape &s, const char *who, long long &entries, long long &keys) {
-    entries = 4ll * s.R * s.pooled_size * s.pooled_size * s.sample_per_part * s.sample_per_part;
-    keys = (long long)s.H * s.W + 1;
-    if (entries > 0xFFFFFFFFll || keys > 0xFFFFFFFFll) {
-        set_error("%s: a plane of %lld entries exceeds the 32-bit entry id", who, entries);
-        return false;
-    }
-    return true;
 }
 
 template <typename T>
@@ -494,27 +482,22 @@ static int psroi_grad_input_det(const T *gout, const T *bbox, const T *trans, co
         return C2M_OK;
     }
     C2M_CHECK_ARG(gout && bbox && top_count && (s.no_trans || trans) && ws, "%s: null pointer", who);
-    long long E, K;
-    if (!psroi_det_plane(s, who, E, K)) return C2M_ERR_INVALID;
-    const long long nplanes = (long long)s.B * s.num_classes;
-    const int np = det_planes_per_pass(ws_bytes, nplanes, E, K);
-    C2M_CHECK_ARG(np >= 1, "%s: workspace of %zu bytes holds no plane (%zu needed)", who, ws_bytes,
-                  det_workspace_bytes(1, nplanes, E, K, who));
+    const long long E = 4ll * s.R * s.pooled_size * s.pooled_size * s.sample_per_part * s.sample_per_part;
+    const long long K = (long long)s.H * s.W + 1;
+    if (!det_plane_fits(E, K, who)) return C2M_ERR_INVALID;
     const int runs = ceil_div(s.output_dim / s.num_classes, PS_GATHER_CH);
-    DetLayout L;
-    C2M_CUDA(det_layout(ws, np * E, np * K, L));
-    auto blocks = [](long long n) { const long long b = (n + 255) / 256; return (int)(b < 132 * 16 ? b : 132 * 16); };
-    for (long long q0 = 0; q0 < nplanes; q0 += np) {
-        const int n = (int)(nplanes - q0 < np ? nplanes - q0 : np);
-        psroi_grad_emit_kernel<T><<<blocks(n * E / 4), 256, 0, st>>>(bbox, trans, s, (int)q0, n, L.keys[0], L.vals[0]);
+    auto emit = [&](int q0, int n, uint32_t *keys, uint32_t *ids) -> int {
+        psroi_grad_emit_kernel<T><<<grid_blocks(n * E / 4), 256, 0, st>>>(bbox, trans, s, q0, n, keys, ids);
         C2M_LAUNCH_CHECK("psroi_grad_emit_kernel");
-        int sorted;
-        if (int rc = det_sort_segments(L, (uint32_t)(n * E), (uint32_t)(n * K), sorted, st)) return rc;
-        psroi_grad_gather_kernel<T><<<blocks((long long)n * runs * s.H * s.W), 256, 0, st>>>(
-            gout, bbox, trans, top_count, s, (int)q0, n, L.seg, L.vals[sorted], grad_input);
+        return C2M_OK;
+    };
+    auto gather = [&](int q0, int n, const uint32_t *seg, const uint32_t *ids) -> int {
+        psroi_grad_gather_kernel<T><<<grid_blocks((long long)n * runs * s.H * s.W), 256, 0, st>>>(
+            gout, bbox, trans, top_count, s, q0, n, seg, ids, grad_input);
         C2M_LAUNCH_CHECK("psroi_grad_gather_kernel");
-    }
-    return C2M_OK;
+        return C2M_OK;
+    };
+    return det_passes(ws, ws_bytes, (long long)s.B * s.num_classes, E, K, who, st, emit, gather);
 }
 
 }  // namespace c2m
@@ -556,8 +539,9 @@ extern "C" size_t c2m_psroi_grad_input_det_workspace_bytes(const c2m_psroi_shape
     const char *who = "psroi_grad_input_det_workspace_bytes";
     if (psroi_check(shape, who)) return 0;
     const c2m_psroi_shape s = psroi_effective(*shape);
-    long long E, K;
-    if (!psroi_det_plane(s, who, E, K)) return 0;
+    const long long E = 4ll * s.R * s.pooled_size * s.pooled_size * s.sample_per_part * s.sample_per_part;
+    const long long K = (long long)s.H * s.W + 1;
+    if (!det_plane_fits(E, K, who)) return 0;
     return det_workspace_bytes(planes, (long long)s.B * s.num_classes, E, K, who);
 }
 

@@ -8,9 +8,13 @@
  * of the tensors' device under the GIL, DCNv2/src/cuda/dcn_v2_cuda.cu:107,139).
  *
  * Reference interfaces replaced (paths relative to the reference repo root):
- *   c2m_dcn_v2_forward_f32          <- `_ext.dcn_v2_forward`
+ *   c2m_deform_conv_{forward,im2col,col2im_coord,col2im,col2im_det}_{f32,f64}
+ *                                   <- `_ext.dcn_v2_forward` / `_ext.dcn_v2_backward`
  *                                      mmsr/models/archs/DCNv2/src/vision.cpp:3-8 (pybind export),
- *                                      src/dcn_v2.h:9-39 (dispatch), src/cuda/dcn_v2_cuda.cu:42-172
+ *                                      src/dcn_v2.h:9-72 (dispatch), src/cuda/dcn_v2_cuda.cu:42-335;
+ *                                      and `deform_conv_cuda` (DCNv1 and grouped DCNv2)
+ *                                      mmsr/models/archs/dcn/src/deform_conv_cuda.cpp:151-695,
+ *                                      src/deform_conv_cuda_kernel.cu
  *   c2m_dcn_v2_fused_forward_f32    <- DCN_sep_pre_multi_offset.forward (everything after the
  *                                      conv_offset_mask conv) mmsr/models/archs/DCNv2/dcn_v2.py:229-253
  *   c2m_corr_argmax_f32             <- feature_match_index  mmsr/models/archs/ref_map_util.py:26-86
@@ -21,10 +25,6 @@
  *   c2m_psroi_pooling_{forward,backward}_{f32,f64}
  *                                   <- `_ext.dcn_v2_psroi_pooling_forward` / `_backward`
  *                                      src/dcn_v2.h:75-144, src/cuda/dcn_v2_psroi_pooling_cuda.cu:58-419
- *   c2m_deform_conv_{forward,im2col,col2im_coord,col2im}_{f32,f64}
- *                                   <- `deform_conv_cuda` (DCNv1 and grouped DCNv2)
- *                                      mmsr/models/archs/dcn/src/deform_conv_cuda.cpp:151-695,
- *                                      src/deform_conv_cuda_kernel.cu
  *
  * The Python binding a reference maintainer would add is shown in INTEGRATION.md.
  */
@@ -50,7 +50,9 @@ enum {
     C2M_ERR_UNSUPPORTED = 4   /* no sm_90 device / driver entry point missing */
 };
 
-int c2m_abi_version(void);      /* 5 since c2m_dcn_tc_args takes only x_il (4: .x_il / c2m_psa_interleave; 3: .mask; 2: out_f32_octets / om_octets) */
+int c2m_abi_version(void);      /* 6 since the fp32 c2m_dcn_v2_* twins of c2m_deform_conv_* are gone (5: c2m_dcn_tc_args
+                                 * takes only x_il; 4: .x_il / c2m_psa_interleave; 3: .mask; 2: out_f32_octets /
+                                 * om_octets) */
 const char *c2m_last_error(void);
 
 /* --- correlation / index_map --------------------------------------------------------------
@@ -82,16 +84,31 @@ int c2m_corr_argmax_f32(const float *fin, const float *fref, int B, int C, int h
 int c2m_offset_pyramid_f32(const int64_t *idx, int B, int gh, int gw, int ref_gw, int scale, float *out,
                            c2m_stream_t stream);
 
-/* --- modulated deformable convolution v2, forward -----------------------------------------
- * out[b,o,p] = bias[o] + sum_{c,i,j} W[o,c,i,j] * mask[b,g(c)*kh*kw+i*kw+j,p] *
+/* --- deformable convolution on the CUDA cores, v1 and modulated, with conv groups -------------------------------
+ * (`_ext.dcn_v2_forward` / `_backward` call the fp32 entries with groups = 1 and a mask; `deform_conv_cuda`,
+ * mmsr/models/archs/dcn/src, calls all of them.)
+ * out[b,o,p] = bias[o] + sum_{c,i,j} W[o,c',i,j] * mask[b,g(c)*kh*kw+i*kw+j,p] *
  *              bilinear(x[b,c], ho*sh-ph+i*dh+off_y, wo*sw-pw+j*dw+off_x)
- * off_y/off_x = offset[b, 2*(g*kh*kw+i*kw+j) (+1), p];  sample is 0 unless
- * -1 < y < H and -1 < x < W; g(c) = c / (C/dg).   All tensors fp32.
- * x  : [B,C,H,W]; element (b,c,y,x) at x[b*xs_b + c*xs_c + y*xs_y + x*xs_x]  (element strides,
- *      so NCHW-contiguous and channels-last storage are both accepted)
- * out: [B,Cout,Ho,Wo]; element strides os_b, os_c, os_y, os_x likewise.
- * offset [B,2*dg*kh*kw,Ho,Wo], mask [B,dg*kh*kw,Ho,Wo], weight [Cout,C,kh,kw], bias [Cout] or NULL:
- * contiguous.
+ * over the input channels c of o's conv group, c' = c - (first channel of that group);
+ * off_y/off_x = offset[b, 2*(g(c)*kh*kw+i*kw+j) (+1), p];  sample is 0 unless
+ * -1 < y < H and -1 < x < W; g(c) = c / (C/dg).
+ *   groups: weight [Cout, C/groups, kh, kw]; output channel o reads the input channels of its conv group
+ *           o / (Cout/groups).  Conv groups and deformable groups partition C independently.
+ *   mask == NULL: modulation 1 (DCNv1); then grad_mask must be NULL too.  bias == NULL adds nothing.
+ * Every tensor of one call is fp32 (_f32) or fp64 (_f64); positions are computed in the dtype, like the reference's
+ * `scalar_t` kernels.
+ * Forward: x [B,C,H,W]; element (b,c,y,x) at x[b*xs_b + c*xs_c + y*xs_y + x*xs_x] (element strides, so
+ * NCHW-contiguous and channels-last storage are both accepted); out [B,Cout,Ho,Wo]: element strides os_b, os_c,
+ * os_y, os_x likewise.  offset [B,2*dg*kh*kw,Ho,Wo], mask [B,dg*kh*kw,Ho,Wo], weight, bias [Cout]: contiguous.
+ * Backward pieces: every tensor NCHW-contiguous; shape->x* / o* strides are ignored.  The two dense GEMMs are the
+ * caller's, per conv group:
+ *   columns [B, C*kh*kw, Ho*Wo] = mask * bilinear(x)                      (for grad_weight = gout x columns^T)
+ *   gcol    [B, C*kh*kw, Ho*Wo] = W^T x grad_output                       (computed by the caller)
+ *   grad_offset [B,2*dg*kh*kw,Ho,Wo], grad_mask [B,dg*kh*kw,Ho,Wo] written; grad_input [B,C,H,W] ACCUMULATED
+ *   (caller zero-fills it first), or written in a fixed order by c2m_deform_conv_col2im_det_* (see "ordered input
+ *   gradients" below).
+ * Rejected with C2M_ERR_INVALID: empty tensors or output, kernel sizes / strides / dilations < 1, C not divisible by
+ * dg, groups < 1, C or Cout not divisible by groups.
  */
 typedef struct {
     int B, C, H, W, Cout;
@@ -100,10 +117,29 @@ typedef struct {
     long long os_b, os_c, os_y, os_x;
 } c2m_dcn_shape;
 
-int c2m_dcn_v2_forward_f32(const float *x, const float *offset, const float *mask, const float *weight,
-                           const float *bias, float *out, const c2m_dcn_shape *shape, c2m_stream_t stream);
+int c2m_deform_conv_forward_f32(const float *x, const float *offset, const float *mask, const float *weight,
+                                const float *bias, int groups, float *out, const c2m_dcn_shape *shape,
+                                c2m_stream_t stream);
+int c2m_deform_conv_forward_f64(const double *x, const double *offset, const double *mask, const double *weight,
+                                const double *bias, int groups, double *out, const c2m_dcn_shape *shape,
+                                c2m_stream_t stream);
+int c2m_deform_conv_im2col_f32(const float *x, const float *offset, const float *mask, const c2m_dcn_shape *shape,
+                               float *columns, c2m_stream_t stream);
+int c2m_deform_conv_im2col_f64(const double *x, const double *offset, const double *mask, const c2m_dcn_shape *shape,
+                               double *columns, c2m_stream_t stream);
+int c2m_deform_conv_col2im_coord_f32(const float *gcol, const float *x, const float *offset, const float *mask,
+                                     const c2m_dcn_shape *shape, float *grad_offset, float *grad_mask,
+                                     c2m_stream_t stream);
+int c2m_deform_conv_col2im_coord_f64(const double *gcol, const double *x, const double *offset, const double *mask,
+                                     const c2m_dcn_shape *shape, double *grad_offset, double *grad_mask,
+                                     c2m_stream_t stream);
+int c2m_deform_conv_col2im_f32(const float *gcol, const float *offset, const float *mask, const c2m_dcn_shape *shape,
+                               float *grad_input, c2m_stream_t stream);
+int c2m_deform_conv_col2im_f64(const double *gcol, const double *offset, const double *mask,
+                               const c2m_dcn_shape *shape, double *grad_input, c2m_stream_t stream);
 
-/* Fused DCN_sep_pre_multi_offset tail: `om` = conv_offset_mask(feat) [B,3*dg*kh*kw,Ho,Wo] raw;
+/* Fused DCN_sep_pre_multi_offset tail, the forward above in fp32 with groups = 1, where
+ * `om` = conv_offset_mask(feat) [B,3*dg*kh*kw,Ho,Wo] raw;
  *   off_y = om[2j] + pre[...,1], off_x = om[2j+1] + pre[...,0], mask = sigmoid(om[2*dg*kh*kw + j]),
  *   j = g*kh*kw + k;  pre = pre_offset [B,kh*kw,Ho,Wo,2] (x,y) or NULL.
  * If pre == NULL and idx != NULL the pre-offsets are rebuilt on the fly from idx [B,gh,gw]
@@ -184,58 +220,12 @@ size_t c2m_dcn_tc_packed_weight_bytes(int C, int Cout, int dg);
 int c2m_dcn_tc_pack_weights_f32(const float *w, int C, int Cout, int dg, void *packed, c2m_stream_t stream);
 int c2m_dcn_v2_fused_tc(const c2m_dcn_tc_args *args, c2m_stream_t stream);
 
-/* --- DCNv2 backward building blocks (`_ext.dcn_v2_backward`, DCNv2/src/dcn_v2.h:41-72) -----------
- * All tensors fp32, NCHW-contiguous; shape->x* / o* strides are ignored here.
- *   columns [B, C*kh*kw, Ho*Wo] = mask * bilinear(x)                      (for grad_weight = gout x columns^T)
- *   gcol    [B, C*kh*kw, Ho*Wo] = W^T x grad_output                       (computed by the caller)
- *   grad_offset [B,2*dg*kh*kw,Ho,Wo], grad_mask [B,dg*kh*kw,Ho,Wo] written; grad_input [B,C,H,W] ACCUMULATED
- *   (caller zero-fills it first).
- */
-int c2m_dcn_v2_im2col_f32(const float *x, const float *offset, const float *mask, const c2m_dcn_shape *shape,
-                          float *columns, c2m_stream_t stream);
-int c2m_dcn_v2_col2im_coord_f32(const float *gcol, const float *x, const float *offset, const float *mask,
-                                const c2m_dcn_shape *shape, float *grad_offset, float *grad_mask,
-                                c2m_stream_t stream);
-int c2m_dcn_v2_col2im_f32(const float *gcol, const float *offset, const float *mask, const c2m_dcn_shape *shape,
-                          float *grad_input, c2m_stream_t stream);
-
-/* --- grouped deformable convolution, v1 and modulated (`deform_conv_cuda`, mmsr/models/archs/dcn/src) ---------------
- * The c2m_dcn_v2_* contract above in fp32 or fp64 (every tensor of one call in that dtype), generalised two ways:
- *   groups: weight [Cout, C/groups, kh, kw]; output channel o reads the input channels of its conv group
- *           o / (Cout/groups).  Conv groups and deformable groups partition C independently.
- *   mask == NULL: modulation 1 (DCNv1, deform_conv_forward_cuda); then grad_mask must be NULL too.
- * Rejected with C2M_ERR_INVALID: groups < 1, C or Cout not divisible by groups, and the c2m_dcn_v2_* shape errors.
- * x and out use the shape's element strides in the forward; the backward pieces take NCHW-contiguous tensors, as the
- * c2m_dcn_v2_* ones do (gcol / columns [B, C*kh*kw, Ho*Wo]; conv groups enter only the caller's GEMMs).
- * Positions are computed in the dtype, like the reference's `scalar_t` kernels; fp32 with a mask and groups == 1 is
- * bit for bit c2m_dcn_v2_forward_f32 / _im2col_f32 / _col2im_coord_f32 / _col2im_f32. */
-int c2m_deform_conv_forward_f32(const float *x, const float *offset, const float *mask, const float *weight,
-                                const float *bias, int groups, float *out, const c2m_dcn_shape *shape,
-                                c2m_stream_t stream);
-int c2m_deform_conv_forward_f64(const double *x, const double *offset, const double *mask, const double *weight,
-                                const double *bias, int groups, double *out, const c2m_dcn_shape *shape,
-                                c2m_stream_t stream);
-int c2m_deform_conv_im2col_f32(const float *x, const float *offset, const float *mask, const c2m_dcn_shape *shape,
-                               float *columns, c2m_stream_t stream);
-int c2m_deform_conv_im2col_f64(const double *x, const double *offset, const double *mask, const c2m_dcn_shape *shape,
-                               double *columns, c2m_stream_t stream);
-int c2m_deform_conv_col2im_coord_f32(const float *gcol, const float *x, const float *offset, const float *mask,
-                                     const c2m_dcn_shape *shape, float *grad_offset, float *grad_mask,
-                                     c2m_stream_t stream);
-int c2m_deform_conv_col2im_coord_f64(const double *gcol, const double *x, const double *offset, const double *mask,
-                                     const c2m_dcn_shape *shape, double *grad_offset, double *grad_mask,
-                                     c2m_stream_t stream);
-int c2m_deform_conv_col2im_f32(const float *gcol, const float *offset, const float *mask, const c2m_dcn_shape *shape,
-                               float *grad_input, c2m_stream_t stream);
-int c2m_deform_conv_col2im_f64(const double *gcol, const double *offset, const double *mask,
-                               const c2m_dcn_shape *shape, double *grad_input, c2m_stream_t stream);
-
 /* --- ordered input gradients (used when torch's deterministic algorithms are enabled) -----------------------------
  * Same results as the col2im / PS-ROI grad_input scatters above, except that every element of grad_input is a sum in
  * one fixed order, so it is the same bit for bit on every run, and that grad_input is WRITTEN (every element, +0
  * where nothing contributes), not accumulated.  Each contribution is the scatter's own expression; an element starts
  * at +0 and adds its contributions with correctly rounded adds in this order:
- *   DCN (c2m_dcn_v2_col2im_det_f32, c2m_deform_conv_col2im_det_{f32,f64}; arguments as c2m_*_col2im_*): over the
+ *   DCN (c2m_deform_conv_col2im_det_{f32,f64}; arguments as c2m_deform_conv_col2im_*): over the
  *     sampling points of deformable group c / (C/dg) of image b, ascending tap, then output pixel, then corner
  *     (low-low, low-high, high-low, high-high); in-image corners only.
  *   PS-ROI (c2m_psroi_pooling_grad_input_det_{f32,f64}; arguments as the backward, without input and grad_trans): over
@@ -247,8 +237,6 @@ int c2m_deform_conv_col2im_f64(const double *gcol, const double *offset, const d
  * one-plane size does not depend on B.  A plane of 2^32 or more contributions is rejected (C2M_ERR_INVALID; the
  * queries return 0).  The size queries ask CUB for its sort storage and so need a current CUDA device. */
 size_t c2m_dcn_col2im_det_workspace_bytes(const c2m_dcn_shape *shape, int planes);
-int c2m_dcn_v2_col2im_det_f32(const float *gcol, const float *offset, const float *mask, const c2m_dcn_shape *shape,
-                              float *grad_input, void *ws, size_t ws_bytes, c2m_stream_t stream);
 int c2m_deform_conv_col2im_det_f32(const float *gcol, const float *offset, const float *mask,
                                    const c2m_dcn_shape *shape, float *grad_input, void *ws, size_t ws_bytes,
                                    c2m_stream_t stream);

@@ -112,12 +112,13 @@ def test_deform_conv_col2im_det_equals_ordered_oracle(case, modulated, dtype):
 
 
 @pytest.mark.parametrize('case', [CASES[i] for i in (0, 1, 2, 5)], ids=_case_id)
-def test_ext_dcn_v2_col2im_det_equals_ordered_oracle(case):
+def test_ext_call_of_col2im_det_equals_ordered_oracle(case):
+    """c2m_deform_conv_col2im_det_f32 as `_ext.dcn_v2_backward` calls it: fp32 with a mask."""
     geo, B, C, Cout, groups, dg, H, W = case
     x, gcol, off, mask = _gcol(case, 600 + 10 * CASES.index(case), True, F32)
     want = ogo.deform_col2im(gcol, off, mask, x.shape, *geo, dg)
     got = _dcn_det_all(gcol.to(DEV), off.to(DEV), mask.to(DEV), tuple(x.shape), geo, dg, F32,
-                       'c2m_dcn_v2_col2im_det_f32')
+                       'c2m_deform_conv_col2im_det_f32')
     assert torch.equal(got.cpu(), want)
 
 
@@ -242,8 +243,8 @@ class _Spy:
             monkeypatch.setattr(L, n, wrap)
 
 
-_DCN_ENTRIES = ['c2m_dcn_v2_col2im_f32', 'c2m_dcn_v2_col2im_det_f32', 'c2m_deform_conv_col2im_f32',
-                'c2m_deform_conv_col2im_f64', 'c2m_deform_conv_col2im_det_f32', 'c2m_deform_conv_col2im_det_f64',
+_DCN_ENTRIES = ['c2m_deform_conv_col2im_f32', 'c2m_deform_conv_col2im_f64', 'c2m_deform_conv_col2im_det_f32',
+                'c2m_deform_conv_col2im_det_f64',
                 'c2m_psroi_pooling_backward_f32', 'c2m_psroi_pooling_backward_f64',
                 'c2m_psroi_pooling_grad_input_det_f32', 'c2m_psroi_pooling_grad_input_det_f64']
 
@@ -277,7 +278,7 @@ def _dcn_modules(kind, dtype):
                                         ('ModulatedDeformConv', F32), ('ModulatedDeformConv', F64)],
                          ids=['DCNv2', 'DeformConv-f32', 'DeformConv-f64', 'ModulatedDeformConv-f32',
                               'ModulatedDeformConv-f64'])
-def test_dcn_modules_take_the_selected_path(kind, dtype, deterministic, monkeypatch):
+def test_dcn_modules_take_the_selected_col2im_path(kind, dtype, deterministic, monkeypatch):
     m = _dcn_modules(kind, dtype)
     dg = m.deformable_groups
     B, H, W = 2, 9, 11
@@ -306,7 +307,7 @@ def test_dcn_modules_take_the_selected_path(kind, dtype, deterministic, monkeypa
 @pytest.mark.parametrize('deterministic', FLAG, ids=FLAG_IDS, indirect=True)
 @pytest.mark.parametrize('no_trans', [False, True])
 @pytest.mark.parametrize('dtype', [F32, F64], ids=['f32', 'f64'])
-def test_dcnv2_pooling_takes_the_selected_path(no_trans, dtype, deterministic, monkeypatch):
+def test_dcnv2_pooling_takes_the_selected_grad_input_path(no_trans, dtype, deterministic, monkeypatch):
     from mmsr.models.archs.DCNv2.dcn_v2 import DCNv2Pooling
     x, bbox, _ = _make(3, 2, 16, 20, 24, 12, 1, 7, 0.25, dtype)
     offs = (torch.randn(12, 2, 5, 5, generator=torch.Generator().manual_seed(2), dtype=F64) * 0.5).to(dtype)

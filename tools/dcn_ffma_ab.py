@@ -1,5 +1,5 @@
-"""A/B of the general FFMA DCN forward (`c2m_dcn_v2_forward_f32`, what `_ext.dcn_v2_forward` runs under
-C2M_EXT_DCN_TC=0) between this tree's library and another build of it, e.g. the parent commit's:
+"""A/B of the general FFMA DCN forward (`c2m_deform_conv_forward_f32` with groups = 1, what `_ext.dcn_v2_forward`
+runs under C2M_EXT_DCN_TC=0) between this tree's library and another build of it, e.g. the parent commit's:
 
     git worktree add /tmp/parent HEAD~1 && python /tmp/parent/c2-matching_b200/c2m_b200/build.py
     python tools/dcn_ffma_ab.py --other /tmp/parent/c2-matching_b200/lib/libc2m_sm100.so
@@ -33,7 +33,7 @@ def main():
     from c2m_b200 import _lib, ops
     libs = {'other': ctypes.CDLL(os.path.abspath(args.other)), 'this': ctypes.CDLL(_lib.LIB_PATH)}
     for lib in libs.values():
-        lib.c2m_dcn_v2_forward_f32.argtypes = [ctypes.c_void_p] * 6 + [ctypes.POINTER(_lib.DcnShape), ctypes.c_void_p]
+        lib.c2m_deform_conv_forward_f32.argtypes = _lib.SYMBOLS['c2m_deform_conv_forward_f32'][1]
     print(torch.cuda.get_device_name(0))
     dev, dg = 'cuda:0', 8
     gen = torch.Generator().manual_seed(3)
@@ -48,10 +48,11 @@ def main():
         s = ops._shape(x, C, 3, 3, 1, 1, 1, 1, 1, 1, dg, outs['this'])
 
         def run(k):
-            rc = libs[k].c2m_dcn_v2_forward_f32(x.data_ptr(), off.data_ptr(), m.data_ptr(), w.data_ptr(),
-                                                b.data_ptr(), outs[k].data_ptr(), ctypes.byref(s), ops._stream())
+            rc = libs[k].c2m_deform_conv_forward_f32(x.data_ptr(), off.data_ptr(), m.data_ptr(), w.data_ptr(),
+                                                     b.data_ptr(), 1, outs[k].data_ptr(), ctypes.byref(s),
+                                                     ops._stream())
             if rc:
-                raise RuntimeError(f'{k}: c2m_dcn_v2_forward_f32 returned {rc}')
+                raise RuntimeError(f'{k}: c2m_deform_conv_forward_f32 returned {rc}')
         for k in libs:
             for _ in range(3):
                 run(k)
