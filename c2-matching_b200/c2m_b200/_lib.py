@@ -45,7 +45,7 @@ class DcnTcArgs(ctypes.Structure):
                 ('out_hi', ctypes.c_void_p), ('out_lo', ctypes.c_void_p), ('sa_out', ctypes.c_int),
                 ('out_f32', ctypes.c_void_p), ('os_b', ctypes.c_longlong), ('os_c', ctypes.c_longlong),
                 ('os_y', ctypes.c_longlong), ('os_x', ctypes.c_longlong), ('om_octets', ctypes.c_int),
-                ('mask', ctypes.c_void_p)]
+                ('mask', ctypes.c_void_p), ('x_amax', ctypes.c_void_p), ('mask_amax', ctypes.c_void_p)]
 
 
 class PsroiShape(ctypes.Structure):
@@ -79,12 +79,16 @@ SYMBOLS = {
     'c2m_psa_to_f32': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 5 + [c_f32p, c_f32p] +
                        [ctypes.c_longlong] * 4 + [ctypes.c_void_p]),
     'c2m_conv3x3': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
-    'c2m_psa_interleave': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 4 + [ctypes.c_void_p] * 2),
     'c2m_psa_maxpool2': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 4 + [ctypes.c_void_p] * 3),
     'c2m_dcn_tc_supported': (ctypes.c_int, [ctypes.c_int] * 3),
     'c2m_dcn_tc_packed_weight_bytes': (ctypes.c_size_t, [ctypes.c_int] * 3),
     'c2m_dcn_tc_pack_weights_f32': (ctypes.c_int, [c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
     'c2m_dcn_v2_fused_tc': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
+    'c2m_dcn_tc_operand_bytes': (ctypes.c_size_t, [ctypes.c_int] * 5),
+    'c2m_dcn_tc_operand_psa': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 5 +
+                               [ctypes.c_void_p] * 2),
+    'c2m_dcn_tc_operand_f32': (ctypes.c_int, [c_f32p] + [ctypes.c_int] * 4 + [ctypes.c_longlong] * 4 +
+                               [ctypes.c_int, c_f32p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     'c2m_profile_enable': (ctypes.c_int, [ctypes.c_int]),
     'c2m_profile_collect': (ctypes.c_int, [ctypes.c_int, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_int),
                                            ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double)]),

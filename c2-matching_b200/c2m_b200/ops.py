@@ -322,18 +322,6 @@ def psa_to_f32(p, add=None, channels_last=False):
     return out
 
 
-def psa_interleave(p):
-    """PSA planes -> fp16 [B][ceil(C/8)][H][W][16] with the hi and lo octets of a pixel adjacent (the tensor-core DCN's
-    gather operand: one 32 B sector per corner fetch instead of two)."""
-    if p.sa != 0:
-        raise RuntimeError('psa_interleave: scale exponent must be 0')
-    out = torch.empty(p.B, (p.C + 7) // 8, p.H, p.W, 16, dtype=torch.float16, device=p.hi.device)
-    with torch.cuda.device(p.hi.device):
-        rc = _lib.lib().c2m_psa_interleave(p.hi.data_ptr(), p.lo.data_ptr(), p.B, p.C, p.H, p.W, out.data_ptr(), _stream())
-        _lib.check(rc, 'c2m_psa_interleave')
-    return out
-
-
 def psa_maxpool2(p):
     """nn.MaxPool2d(kernel_size=2, stride=2) on a PSA tensor."""
     out = PSA.empty(p.B, p.C, p.H // 2, p.W // 2, p.hi.device, p.sa)
@@ -508,17 +496,19 @@ def dcn_v2_fused_tc(x, om, weight, bias, deformable_group, pre_offset=None, idx=
     import ctypes
     om_oct = isinstance(om, OctF32)
     _require_cuda('om', om.data if om_oct else om)
-    if isinstance(x, PSA):
-        xp = x
+    xp = x if isinstance(x, PSA) else getattr(x, '_c2m_psa', None)
+    if xp is not None and xp.shape != tuple(x.shape):
+        xp = None
+    if xp is not None:
+        if xp.sa != 0:
+            raise RuntimeError('dcn_v2_fused_tc: PSA input must have scale exponent 0')
+        B, C, H, W = xp.shape
+        dev = xp.hi.device
     else:
         _require_cuda('x', x)
-        xp = getattr(x, '_c2m_psa', None)
-        if xp is None or xp.shape != tuple(x.shape):
-            xp = psa_from_f32(x)
-    if xp.sa != 0:
-        raise RuntimeError('dcn_v2_fused_tc: PSA input must have scale exponent 0')
-    B, C, H, W = xp.shape
-    dev = xp.hi.device
+        x = _dense_nchw_or_nhwc(x)
+        B, C, H, W = x.shape
+        dev = x.device
     cout = weight.shape[0]
     if final_mask is not None:
         _require_cuda('final_mask', final_mask)
@@ -529,11 +519,28 @@ def dcn_v2_fused_tc(x, om, weight, bias, deformable_group, pre_offset=None, idx=
     elif tuple(om.shape) != (B, 27 * deformable_group, H, W):
         raise RuntimeError(f'conv_offset_mask output has shape {tuple(om.shape)}')
     a = _lib.DcnTcArgs()
-    x_il = psa_interleave(xp)               # kept alive until the launch below is enqueued (same stream)
-    a.x_il = x_il.data_ptr()
+    # x_il (the interleaved operand and its zero tail) and the amax buffer are kept alive until the launch below is
+    # enqueued (same stream)
+    x_il = torch.empty(_lib.lib().c2m_dcn_tc_operand_bytes(B, C, H, W, deformable_group) // 2, dtype=torch.float16,
+                       device=dev)
     if final_mask is not None:
         final_mask = final_mask.contiguous()
         a.mask = final_mask.data_ptr()
+    with torch.cuda.device(dev):
+        if xp is not None:
+            rc = _lib.lib().c2m_dcn_tc_operand_psa(xp.hi.data_ptr(), xp.lo.data_ptr(), B, C, H, W, deformable_group,
+                                                   x_il.data_ptr(), _stream())
+            _lib.check(rc, 'c2m_dcn_tc_operand_psa')
+        else:
+            # an fp32 input of any magnitude: per-image operand (and final mask) exponents, taken on the device
+            amax = torch.empty(2 * B, dtype=torch.int32, device=dev)
+            rc = _lib.lib().c2m_dcn_tc_operand_f32(x.data_ptr(), B, C, H, W, *x.stride(), deformable_group,
+                                                   a.mask, x_il.data_ptr(), amax.data_ptr(), _stream())
+            _lib.check(rc, 'c2m_dcn_tc_operand_f32')
+            a.x_amax = amax.data_ptr()
+            if final_mask is not None:
+                a.mask_amax = amax.data_ptr() + 4 * B
+    a.x_il = x_il.data_ptr()
     if om_oct:
         a.om, a.om_octets = om.data.data_ptr(), 1
     else:

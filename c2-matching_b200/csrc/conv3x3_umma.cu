@@ -283,17 +283,6 @@ __global__ void psa_to_f32_kernel(const __half *__restrict__ hi, const __half *_
     }
 }
 
-// hi / lo planes -> one array with the two halves of a (pixel, octet) adjacent: [B][C8][H][W][hi 8 | lo 8] fp16.
-// The DCN gather fetches single (pixel, octet) corners from unrelated places: with separate planes every corner costs
-// two 32 B sectors (16 B used in each), interleaved it is one fully used sector and one 256-bit load.
-__global__ void psa_interleave_kernel(const uint4 *__restrict__ hi, const uint4 *__restrict__ lo, long long n,
-                                      uint4 *__restrict__ out) {
-    for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x) {
-        out[2 * e] = hi[e];
-        out[2 * e + 1] = lo[e];
-    }
-}
-
 // 2x2 / stride 2 max-pool on a PSA tensor (VGG pool1/pool2 between tensor-core convolutions): the
 // pooled map stays in the operand layout, no fp32 round trip through HBM.  max(hi+lo) is taken on
 // the reconstructed fp32 values and re-split (the re-split of an already-split value is exact).
@@ -418,19 +407,6 @@ extern "C" int c2m_psa_to_f32(const void *hi, const void *lo, int B, int C, int 
         reinterpret_cast<const __half *>(hi), reinterpret_cast<const __half *>(lo), C, C8, H, W, sa, add, out, os_b,
         os_c, os_y, os_x);
     C2M_LAUNCH_CHECK("psa_to_f32_kernel");
-    return C2M_OK;
-}
-
-extern "C" int c2m_psa_interleave(const void *hi, const void *lo, int B, int C, int H, int W, void *out, c2m_stream_t stream) {
-    C2M_CHECK_ARG(hi && lo && out && B > 0 && C > 0 && H > 0 && W > 0, "psa_interleave: bad argument");
-    C2M_CHECK_ARG(((reinterpret_cast<uintptr_t>(hi) | reinterpret_cast<uintptr_t>(lo)) & 15) == 0 &&
-                  (reinterpret_cast<uintptr_t>(out) & 31) == 0, "psa_interleave: planes must be 16 B, the output 32 B aligned");
-    const long long n = (long long)B * ((C + 7) / 8) * H * W;
-    int bx = (int)((n + 255) / 256);
-    if (bx > 4096) bx = 4096;
-    psa_interleave_kernel<<<bx, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-        reinterpret_cast<const uint4 *>(hi), reinterpret_cast<const uint4 *>(lo), n, reinterpret_cast<uint4 *>(out));
-    C2M_LAUNCH_CHECK("psa_interleave_kernel");
     return C2M_OK;
 }
 

@@ -48,9 +48,12 @@ struct DcnTc {
     int om_c8;
     const float *mask;         // non-null: FINAL modulation mask [B, dg*9, H, W] (no sigmoid) and `om` holds only the
                                // FINAL offsets [B, 2*dg*9, H, W] — the `_ext.dcn_v2_forward` contract
+    const unsigned *x_amax;    // [B] bits of the largest finite |x| of each image, or null: x_il holds x * 2^operand_exp
+    const unsigned *mask_amax; // [B] the same for the final mask, or null: the gather weights carry mask * 2^mask_exp
     const float *pre;          // [B, 9, H, W, 2] or null
     const long long *idx;      // [B, gh, gw] or null
     int gh, gw, ref_gw, pre_scale;
+    int z_end;                 // elements of x_il before its zero tail (B * C * H * W)
     int C, dg, cpg, opp;       // opp = octets per (g, tap) pair = cpg / 8
     int n_ko;                  // real K octets = C/8 * 9
     int L, lshift;             // K octets per gather thread and stage (1, 2 or 4), log2
@@ -63,6 +66,24 @@ struct DcnTc {
     float inv_ref_gw, inv_scale;   // reciprocals for the exact float-assisted integer divisions
 };
 }  // namespace
+
+// Per-image operand exponents of an fp32 boundary, from the bits of the image's largest finite magnitude (0 -> 0).
+// x: amax * 2^s in [2^11, 2^12), under fp16's 65504 with 16x headroom for the blend and well above its subnormals.
+// mask: max |mask| * 2^s in [1, 2), so the corner weights are at most 2.  Exponent arithmetic only: scaling an image
+// by 2^k shifts its exponent by -k and leaves the operand bit for bit the same.  Each exponent is clamped to +-120, so
+// 2^sa and 2^sm are normal floats.  Their sum with the weight exponent sw is not clamped: the epilogue's
+// 2^-(sa + sm + sw) leaves fp32's range (flushing the output to 0 or overflowing it) only when it exceeds 149 or
+// drops below -127.  Since amax(x) 2^sa is in [2^11, 2^12), amax(mask) 2^sm in [1, 2) and amax(w) 2^sw in
+// [2^13, 2^14), that happens only when amax(x) amax(mask) amax(w) is below 2^-121 or above 2^151: outputs at the
+// edge of fp32's range whatever computes them.
+__host__ __device__ __forceinline__ int amax_exp(unsigned bits, int top) {
+    if (bits == 0u) return 0;
+    const int e = (int)(bits >> 23) - 127;            // floor(log2 amax); a subnormal amax counts as 2^-127
+    const int s = top - e;
+    return s < -120 ? -120 : s > 120 ? 120 : s;
+}
+__device__ __forceinline__ int operand_exp(const unsigned *amax, int b) { return amax ? amax_exp(amax[b], 11) : 0; }
+__device__ __forceinline__ int mask_exp(const unsigned *amax, int b) { return amax ? amax_exp(amax[b], 0) : 0; }
 
 // exact n / d for 0 <= n < 2^23 with a precomputed float reciprocal (one multiply + fix-up instead
 // of the ~25-instruction integer division sequence; the gather loop is issue-bound)
@@ -169,7 +190,6 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
         // one warpgroup: the wgmmas of both 64-row halves of the tile (A rows 64.. start 8 core-matrix groups in),
         // then the accumulator goes through shared memory to the epilogue, one pixel per thread
         const int e = threadIdx.x - 128;
-        const float out_scale = ldexpf(1.f, -(p.sa_in + sw));
         const float res_scale = 1.f;
         const float so = ldexpf(1.f, p.sa_out);
         const bool fast = epilogue_fast_ok(q, p) && p.sa_out == 0;     // (this kernel does not pre-scale bias / factors)
@@ -182,6 +202,7 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
             const int b = item / tiles_img, tt = item - b * tiles_img;
             const int y = (tt / p.tiles_x) * T_R + e / T_C, x = (tt % p.tiles_x) * T_C + e % T_C;
             const bool ok = y < p.H && x < p.W;
+            const float out_scale = ldexpf(1.f, -(operand_exp(d.x_amax, b) + mask_exp(d.mask_amax, b) + sw));
             float acc0[N / 2], acc1[N / 2];                 // rows [0, 64) and [64, 128)
             for (int kc = 0; kc < p.nkc; ++kc) {
                 mbar_wait(&bfull[bst], bphase);
@@ -353,9 +374,14 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
             fetch(sg, sg < p.nkc, mt, y, xx, b, lv);
             for (int kc = sg; kc < p.nkc; kc += NG) {
                 // ---- sampling point of the unit's (pixel, g, tap): dcn_v2_im2col_cuda.cu:25-54,172-190
-                int o0 = 0, o1 = 0, o2 = 0, o3 = 0;
+                const int xoff = lv ? c_xoff : 0;           // belongs to kc (set_kc(kc) ran in this unit's fetch)
+                // A corner the sample does not read (outside the image, or the sample outside the window) points at
+                // x_il's zero tail: octet u of the run then reads zeros at z_end + u * P * 8, so it contributes exactly
+                // 0 whatever the image holds, at no cost per corner.  Offsets reach z_end < 2^31 (host-checked), so
+                // their doubling below is unsigned.
+                const int zo = d.z_end - (b * x_img + xoff);
+                int o0 = zo, o1 = zo, o2 = zo, o3 = zo;
                 float w0 = 0.f, w1 = 0.f, w2 = 0.f, w3 = 0.f;
-                const int xoff = c_xoff;                    // belongs to kc (set_kc(kc) ran in this unit's fetch)
                 if (lv) {
                     const float h_im = ((float)y + c_fy) + mt.off_h;
                     const float w_im = ((float)xx + c_fx) + mt.off_w;
@@ -366,7 +392,8 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
                         const float hh = 1.f - lh, hw = 1.f - lw;
                         const bool tv = h_low >= 0, bv = h_low + 1 <= p.H - 1, lvv = w_low >= 0, rv = w_low + 1 <= p.W - 1;
                         // sigmoid to ~2 ulp: the TC path is fp32-grade, not bit-exact; the mask is folded into the weights
-                        const float mk = d.mask ? mt.mr : __fdividef(1.f, 1.f + __expf(-mt.mr));
+                        const float mk = d.mask ? mt.mr * __int_as_float((127 + mask_exp(d.mask_amax, b)) << 23)
+                                                : __fdividef(1.f, 1.f + __expf(-mt.mr));
                         const int r0 = h_low * W8 + w_low * 8;
                         const float mh = hh * mk, ml = lh * mk;
                         if (tv && lvv) { o0 = r0; w0 = mh * hw; }
@@ -390,11 +417,11 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
                     const int po = u * P * 8;
                     uint4 ch0, ch1, ch2, ch3, cl0, cl1, cl2, cl3;
                     // element offsets double in the interleaved operand
-                    const __half *xi = d.x_il + 2 * ((size_t)b * x_img + (lv ? xoff : 0) + po);
-                    ldg_keep_v8(xi + 2 * o0, pol_keep, ch0, cl0);
-                    ldg_keep_v8(xi + 2 * o1, pol_keep, ch1, cl1);
-                    ldg_keep_v8(xi + 2 * o2, pol_keep, ch2, cl2);
-                    ldg_keep_v8(xi + 2 * o3, pol_keep, ch3, cl3);
+                    const __half *xi = d.x_il + 2 * ((size_t)b * x_img + xoff + po);
+                    ldg_keep_v8(xi + 2u * (unsigned)o0, pol_keep, ch0, cl0);
+                    ldg_keep_v8(xi + 2u * (unsigned)o1, pol_keep, ch1, cl1);
+                    ldg_keep_v8(xi + 2u * (unsigned)o2, pol_keep, ch2, cl2);
+                    ldg_keep_v8(xi + 2u * (unsigned)o3, pol_keep, ch3, cl3);
                     // ---- blend, modulate, split.  value = hi + lo: the hi halves are blended in fp32, the lo halves
                     // (|lo| <= 2^-11 |value|) in packed fp16 — their rounding lands at 2^-22 of the value
                     const __half2 *hp0 = reinterpret_cast<const __half2 *>(&ch0), *hp1 = reinterpret_cast<const __half2 *>(&ch1);
@@ -461,12 +488,81 @@ __global__ void dcn_wpack_kernel(const float *__restrict__ w, int C, int Cout, i
     }
 }
 
+// Largest finite |v| of each image as fp32 bits, for x (blockIdx.z = 0: image b at x + b * nx) and the final mask
+// (blockIdx.z = 1: image b at mask + b * nm) in one launch; amax[z * B + b] starts at 0.
+__global__ void amax_per_image_kernel(const float *__restrict__ x, long long nx, const float *__restrict__ mask,
+                                      long long nm, unsigned *__restrict__ amax) {
+    const int b = blockIdx.y, B = gridDim.y;
+    const long long n = blockIdx.z ? nm : nx;
+    const float *vb = (blockIdx.z ? mask : x) + (size_t)b * n;
+    float m = 0.f;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const float a = fabsf(vb[i]);
+        if (a < INFINITY) m = fmaxf(m, a);          // NaN and Inf do not set the scale
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(amax + blockIdx.z * B + b, __float_as_uint(m));
+}
+
+// The operand writers below also zero x_il's tail: `tail` pairs of 16-byte halves (hi | lo) after the B*C8*H*W
+// pixel octets, which the gather reads for corners it must not read from the image.
+
+// strided fp32 x -> x * 2^operand_exp(image) split into the interleaved operand [B][C8][H][W][hi 8 | lo 8]
+// (one thread = one (octet, pixel), pixel fastest: coalesced NCHW reads, one 32 B store)
+__global__ void dcn_operand_kernel(const float *__restrict__ x, int C, int C8, int H, int W, long long xs_b,
+                                   long long xs_c, long long xs_y, long long xs_x, const unsigned *__restrict__ amax,
+                                   long long tail, __half *__restrict__ out) {
+    const long long HW = (long long)H * W;
+    const long long n = (long long)C8 * HW;
+    const int b = blockIdx.y;
+    const long long n_here = b == gridDim.y - 1 ? n + tail : n;           // the last image's blocks write the tail
+    const float S = ldexpf(1.f, operand_exp(amax, b));
+    for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < n_here; e += (long long)gridDim.x * blockDim.x) {
+        uint4 *dst = reinterpret_cast<uint4 *>(out + ((size_t)b * n + e) * 16);
+        if (e >= n) {
+            dst[0] = dst[1] = make_uint4(0, 0, 0, 0);
+            continue;
+        }
+        const int oct = (int)(e / HW);
+        const long long pix = e % HW;
+        const int y = (int)(pix / W), xx = (int)(pix % W);
+        __align__(16) __half h8[16];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const int c = oct * 8 + j;
+            const float v = c < C ? x[b * xs_b + c * xs_c + y * xs_y + xx * xs_x] * S : 0.f;
+            const __half hh = __float2half_rn(v);
+            h8[j] = hh;
+            h8[8 + j] = __float2half_rn(v - __half2float(hh));
+        }
+        dst[0] = reinterpret_cast<const uint4 *>(h8)[0];
+        dst[1] = reinterpret_cast<const uint4 *>(h8)[1];
+    }
+}
+
+// PSA hi / lo planes -> the same interleaved operand (and its zero tail): one 32 B sector per corner fetch instead of
+// two 16 B halves in separate planes
+__global__ void dcn_operand_psa_kernel(const uint4 *__restrict__ hi, const uint4 *__restrict__ lo, long long n,
+                                       long long tail, uint4 *__restrict__ out) {
+    for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < n + tail; e += (long long)gridDim.x * blockDim.x) {
+        const bool body = e < n;
+        out[2 * e] = body ? hi[e] : make_uint4(0, 0, 0, 0);
+        out[2 * e + 1] = body ? lo[e] : make_uint4(0, 0, 0, 0);
+    }
+}
+
 static inline int d_pad16(int c) { return (c + 15) / 16 * 16; }
 // output channels per launch: a 128 x 64 fp32 accumulator is what the MMA warpgroup keeps in registers
 constexpr int D_NMAX = 64;
 static inline int d_slice_n(int cout) { return cout <= D_NMAX ? d_pad16(cout) : D_NMAX; }
 static inline int d_n_slice(int cout) { return (cout + D_NMAX - 1) / D_NMAX; }
 static inline int d_nkc(int C) { return ((C / 8) * 9 + KOCT - 1) / KOCT; }
+// K octets per gather thread: the (g, tap) run inside a 4-octet stage when C/dg/8 is a power of two
+static inline int d_run(int C, int dg) {
+    const int opp = C / dg / 8;
+    return (opp & (opp - 1)) ? 1 : (opp >= KOCT ? KOCT : opp);
+}
 
 }  // namespace c2m
 
@@ -490,6 +586,57 @@ extern "C" int c2m_dcn_tc_pack_weights_f32(const float *w, int C, int Cout, int 
     const long long total = (long long)ns * nkc * 2 * KOCT * N * 8;
     dcn_wpack_kernel<<<wpack_blocks(total), 256, 0, st>>>(w, C, Cout, dg, N, nkc, ns, reinterpret_cast<uint8_t *>(packed));
     C2M_LAUNCH_CHECK("dcn_wpack_kernel");
+    return C2M_OK;
+}
+
+// (pixel, octet) pairs of x_il's zero tail: the gather's L-octet runs read it at z_end + u * H * W * 8, u < L
+static inline long long d_tail(int C, int dg, int H, int W) { return (long long)(d_run(C, dg) - 1) * H * W + 1; }
+
+extern "C" size_t c2m_dcn_tc_operand_bytes(int B, int C, int H, int W, int dg) {
+    if (B <= 0 || H <= 0 || W <= 0 || !c2m_dcn_tc_supported(C, 1, dg)) return 0;
+    return ((size_t)B * (C / 8) * H * W + d_tail(C, dg, H, W)) * 32;
+}
+
+extern "C" int c2m_dcn_tc_operand_psa(const void *hi, const void *lo, int B, int C, int H, int W, int dg, void *x_il,
+                                      c2m_stream_t stream) {
+    C2M_CHECK_ARG(hi && lo && x_il && B > 0 && H > 0 && W > 0 && c2m_dcn_tc_supported(C, 1, dg),
+                  "dcn_tc_operand_psa: bad argument");
+    C2M_CHECK_ARG(((reinterpret_cast<uintptr_t>(hi) | reinterpret_cast<uintptr_t>(lo)) & 15) == 0 &&
+                  (reinterpret_cast<uintptr_t>(x_il) & 31) == 0, "dcn_tc_operand_psa: planes must be 16 B, x_il 32 B aligned");
+    const long long n = (long long)B * (C / 8) * H * W, tail = d_tail(C, dg, H, W);
+    const long long bx = (n + tail + 255) / 256;
+    dcn_operand_psa_kernel<<<(int)(bx > 4096 ? 4096 : bx), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+        reinterpret_cast<const uint4 *>(hi), reinterpret_cast<const uint4 *>(lo), n, tail, reinterpret_cast<uint4 *>(x_il));
+    C2M_LAUNCH_CHECK("dcn_operand_psa_kernel");
+    return C2M_OK;
+}
+
+extern "C" int c2m_dcn_tc_operand_f32(const float *x, int B, int C, int H, int W, long long xs_b, long long xs_c,
+                                      long long xs_y, long long xs_x, int dg, const float *mask, void *x_il,
+                                      unsigned *amax, c2m_stream_t stream) {
+    C2M_CHECK_ARG(x && x_il && amax && B > 0 && B <= 65535 && H > 0 && W > 0 && c2m_dcn_tc_supported(C, 1, dg),
+                  "dcn_tc_operand: bad argument");
+    C2M_CHECK_ARG((reinterpret_cast<uintptr_t>(x_il) & 31) == 0, "dcn_tc_operand: x_il must be 32 B aligned");
+    // image b must be the C*H*W elements from x + b * C*H*W on (dense NCHW or channels-last): its amax is taken flat.
+    // The stride of a dimension of size 1 is never used.
+    const long long n = (long long)C * H * W;
+    C2M_CHECK_ARG((C == 1 || xs_c > 0) && (H == 1 || xs_y > 0) && (W == 1 || xs_x > 0) && (B == 1 || xs_b == n) &&
+                  (C - 1) * xs_c + (H - 1) * xs_y + (W - 1) * xs_x + 1 == n,
+                  "dcn_tc_operand: x must be dense NCHW or channels-last");
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const int nz = mask ? 2 : 1;
+    const long long nm = (long long)dg * 9 * H * W;
+    C2M_CUDA(cudaMemsetAsync(amax, 0, sizeof(unsigned) * nz * B, st));
+    const long long ax = ((n > nm ? n : nm) + 2047) / 2048;
+    amax_per_image_kernel<<<dim3(ax > 256 ? 256 : (unsigned)ax, B, nz), 256, 0, st>>>(x, n, mask, nm, amax);
+    C2M_LAUNCH_CHECK("amax_per_image_kernel");
+    const int C8 = C / 8;
+    const long long m = (long long)C8 * H * W, tail = d_tail(C, dg, H, W);
+    const long long bx = (m + tail + 255) / 256;
+    dcn_operand_kernel<<<dim3((unsigned)(bx > 4096 ? 4096 : bx), B), 256, 0, st>>>(x, C, C8, H, W, B == 1 ? 0 : xs_b,
+                                                                                  xs_c, xs_y, xs_x, amax, tail,
+                                                                                  reinterpret_cast<__half *>(x_il));
+    C2M_LAUNCH_CHECK("dcn_operand_kernel");
     return C2M_OK;
 }
 
@@ -527,14 +674,17 @@ extern "C" int c2m_dcn_v2_fused_tc(const c2m_dcn_tc_args *a, c2m_stream_t stream
     C2M_CHECK_ARG(!a->mask || (!a->om_octets && !a->pre && !a->idx),
                   "dcn_v2_fused_tc: a final mask excludes octet-planar om and pre-offsets");
     d.mask = a->mask;
+    d.x_amax = a->x_amax;
+    d.mask_amax = a->mask_amax;
+    C2M_CHECK_ARG(!a->mask_amax || a->mask, "dcn_v2_fused_tc: mask_amax needs a final mask");
     d.om = a->om; d.pre = a->pre; d.idx = reinterpret_cast<const long long *>(a->idx);
     d.gh = a->gh; d.gw = a->gw; d.ref_gw = a->ref_gw; d.pre_scale = a->pre_scale;
+    d.z_end = (int)((long long)a->B * a->C * a->H * a->W);     // < 2^31: checked below, before any launch
     d.C = a->C; d.dg = a->dg; d.cpg = a->C / a->dg; d.opp = d.cpg / 8; d.n_ko = (a->C / 8) * 9;
     d.opp_shift = -1;
     for (int sft = 0; sft < 8; ++sft)
         if (d.opp == (1 << sft)) d.opp_shift = sft;
-    // K octets per gather thread: the (g, tap) run inside a 4-octet stage when C/dg/8 is a power of two
-    d.L = d.opp_shift < 0 ? 1 : (d.opp >= KOCT ? KOCT : d.opp);
+    d.L = d_run(a->C, a->dg);
     d.lshift = d.L == 4 ? 2 : d.L == 2 ? 1 : 0;
     d.inv_ref_gw = a->ref_gw > 0 ? 1.f / (float)a->ref_gw : 0.f;
     d.inv_scale = a->pre_scale > 0 ? 1.f / (float)a->pre_scale : 1.f;

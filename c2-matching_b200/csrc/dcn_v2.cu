@@ -21,8 +21,9 @@
 // 4tx..4tx+3 and channels ty+16i.  K is walked over the conv group's input channels in segments that never cross
 // a deformable-group boundary (conv groups and deformable groups partition C independently), one channel block at
 // a time: the sampling table (4 corner offsets + 4 weights + mask per (tap, pixel)) is computed once per
-// (deformable group, tap pass) and shared by all channels of the segment.  A corner outside the image is stored as
-// element 0 with weight 0, so the gather loads unconditionally.
+// (deformable group, tap pass) and shared by all channels of the segment.  A corner outside the image (and every corner
+// of a sample outside the window) is stored as offset -1 and reads as exactly 0: like the reference, the gather never
+// loads it, so a non-finite element elsewhere in the plane cannot reach the sample through a zero weight.
 #include <type_traits>
 
 #include "dcn_sampling.cuh"
@@ -70,6 +71,10 @@ struct Samp {
 __device__ __forceinline__ float dcn_fma(float a, float b, float c) { return fmaf(a, b, c); }
 __device__ __forceinline__ double dcn_fma(double a, double b, double c) { return fma(a, b, c); }
 
+// corner value: offset -1 marks a corner the sample does not read
+template <typename T>
+__device__ __forceinline__ T corner(const T *xc, int o) { return o >= 0 ? xc[o] : (T)0; }
+
 struct Double4 { double x, y, z, w; };
 __device__ __forceinline__ float4 col_load4(const float *p) { return *reinterpret_cast<const float4 *>(p); }
 __device__ __forceinline__ Double4 col_load4(const double *p) {
@@ -116,7 +121,7 @@ __global__ void __launch_bounds__(256, (dcn_min_ctas<scalar_t, NO>())) dcn_fwd_k
             // ---- sampling table for (tap, pixel), shared by the segment's channels
             for (int e = t; e < TB * TP; e += 256) {
                 const int tl = e / TP, pl = e % TP, tap = t0 + tl, p = p0 + pl;
-                Samp<scalar_t> sp = {};
+                Samp<scalar_t> sp = {{-1, -1, -1, -1}, {}, (scalar_t)0};
                 if (p < P) {
                     const int j = g * T + tap;
                     scalar_t off_h, off_w, m;
@@ -165,7 +170,8 @@ __global__ void __launch_bounds__(256, (dcn_min_ctas<scalar_t, NO>())) dcn_fwd_k
                         const int cl = e % CBn, rest = e / CBn, pl = rest % TP, tl = rest / TP;
                         const Samp<scalar_t> &sp = samp[tl * TP + pl];
                         const scalar_t *xc = xb + (c0 + cl);
-                        const scalar_t v = dcn_blend(sp.w, xc[sp.o[0]], xc[sp.o[1]], xc[sp.o[2]], xc[sp.o[3]]);
+                        const scalar_t v = dcn_blend(sp.w, corner(xc, sp.o[0]), corner(xc, sp.o[1]), corner(xc, sp.o[2]),
+                                                     corner(xc, sp.o[3]));
                         col[(cl * TB + tl) * TP + pl] = v * sp.m;
                     }
                 } else {
@@ -173,7 +179,8 @@ __global__ void __launch_bounds__(256, (dcn_min_ctas<scalar_t, NO>())) dcn_fwd_k
                         const int pl = e % TP, row = e / TP, cl = row / TB, tl = row % TB;
                         const Samp<scalar_t> &sp = samp[tl * TP + pl];
                         const scalar_t *xc = xb + (long long)(c0 + cl) * s.xs_c;
-                        const scalar_t v = dcn_blend(sp.w, xc[sp.o[0]], xc[sp.o[1]], xc[sp.o[2]], xc[sp.o[3]]);
+                        const scalar_t v = dcn_blend(sp.w, corner(xc, sp.o[0]), corner(xc, sp.o[1]), corner(xc, sp.o[2]),
+                                                     corner(xc, sp.o[3]));
                         col[row * TP + pl] = v * sp.m;
                     }
                 }

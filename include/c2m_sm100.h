@@ -52,7 +52,8 @@ enum {
 
 int c2m_abi_version(void);      /* 6 since the fp32 c2m_dcn_v2_* twins of c2m_deform_conv_* are gone (5: c2m_dcn_tc_args
                                  * takes only x_il; 4: .x_il / c2m_psa_interleave; 3: .mask; 2: out_f32_octets /
-                                 * om_octets) */
+                                 * om_octets).  Later additions (c2m_dcn_tc_args.x_amax / .mask_amax,
+                                 * c2m_dcn_tc_operand_*) come with new symbols that an older library lacks. */
 const char *c2m_last_error(void);
 
 /* --- correlation / index_map --------------------------------------------------------------
@@ -186,8 +187,6 @@ int c2m_psa_from_f32(const float *x, int B, int C, int H, int W, long long xs_b,
 int c2m_psa_to_f32(const void *hi, const void *lo, int B, int C, int H, int W, int sa, const float *add, float *out,
                    long long os_b, long long os_c, long long os_y, long long os_x, c2m_stream_t stream);
 int c2m_conv3x3(const c2m_conv3x3_args *args, c2m_stream_t stream);
-/* hi / lo planes -> interleaved [B][ceil(C/8)][H][W][hi 8 | lo 8] (the input operand of c2m_dcn_v2_fused_tc). */
-int c2m_psa_interleave(const void *hi, const void *lo, int B, int C, int H, int W, void *out, c2m_stream_t stream);
 /* MaxPool2d(2, 2) on a PSA tensor (floor semantics: odd trailing row / column dropped), PSA result. */
 int c2m_psa_maxpool2(const void *hi, const void *lo, int B, int C, int H, int W, void *out_hi, void *out_lo,
                      c2m_stream_t stream);
@@ -196,10 +195,18 @@ int c2m_psa_maxpool2(const void *hi, const void *lo, int B, int C, int H, int W,
  * Same contract as c2m_dcn_v2_fused_forward_f32 (raw conv_offset_mask output `om`, pre-offsets from
  * `pre` or rebuilt from `idx`), but the contraction runs as a split-fp16 tensor-core GEMM fed by
  * gather warps; the input `x_il` is a PSA tensor (see c2m_psa_from_f32) with the two halves of a (pixel, octet)
- * adjacent, fp16 [B][C/8][H][W][hi 8 | lo 8] (c2m_psa_interleave), 32 B aligned: its octet-planar layout lets a
+ * adjacent, fp16 [B][C/8][H][W][hi 8 | lo 8] (c2m_dcn_tc_operand_psa), 32 B aligned: its octet-planar layout lets a
  * warp's corner fetches share cache lines, and a corner fetch is one 32 B sector.  Outputs: PSA (out_hi/out_lo) and / or
  * strided fp32; `lrelu` != 0 applies LeakyReLU(0.1).  Weights are packed once with
  * c2m_dcn_tc_pack_weights_f32 into c2m_dcn_tc_packed_weight_bytes(C, Cout, dg) bytes.
+ * An fp32 input of any magnitude goes through c2m_dcn_tc_operand_f32, which writes x_il as x * 2^sa with a
+ * per-image exponent sa (amax * 2^sa in [2^11, 2^12), from the exponent bits of the image's largest finite |x|) and
+ * stores the amax bits in amax[0, B) (and, given the final mask, the mask's in amax[B, 2B)); pass x_amax = amax (and
+ * mask_amax = amax + B) here: the epilogue divides 2^sa back out image by image, and the gather scales each image's
+ * mask to max |mask| in [1, 2).  Computed on the device (no host synchronisation); NULL means exponent 0.
+ * x_il holds c2m_dcn_tc_operand_bytes(B, C, H, W, dg) bytes: the operand, then a zero tail that both operand writers
+ * fill and that the gather reads for a sample outside the window and a corner outside the image, so those contribute
+ * exactly 0 and, as in the reference, the image is not read for them.
  */
 typedef struct {
     const void *x_il;
@@ -213,12 +220,24 @@ typedef struct {
     const float *mask;           /* != NULL: the `_ext.dcn_v2_forward` contract (DCNv2/src/dcn_v2.h:9-22) — `om` is the
                                   * FINAL offset tensor [B,2*dg*9,H,W], `mask` the FINAL modulation [B,dg*9,H,W]
                                   * (no sigmoid applied); pre, idx and om_octets must be unset */
+    const unsigned *x_amax;      /* [B] or NULL: written by c2m_dcn_tc_operand_f32 together with x_il */
+    const unsigned *mask_amax;   /* [B] or NULL (needs mask): written by c2m_dcn_tc_operand_f32 given the mask */
 } c2m_dcn_tc_args;
 
 int c2m_dcn_tc_supported(int C, int Cout, int dg);
 size_t c2m_dcn_tc_packed_weight_bytes(int C, int Cout, int dg);
 int c2m_dcn_tc_pack_weights_f32(const float *w, int C, int Cout, int dg, void *packed, c2m_stream_t stream);
 int c2m_dcn_v2_fused_tc(const c2m_dcn_tc_args *args, c2m_stream_t stream);
+/* Bytes of x_il for c2m_dcn_v2_fused_tc: B*C*H*W*2 fp16 of operand, then the zero tail (0 if unsupported). */
+size_t c2m_dcn_tc_operand_bytes(int B, int C, int H, int W, int dg);
+/* PSA hi / lo planes (scale exponent 0) -> x_il: interleaved [B][C/8][H][W][hi 8 | lo 8] and its zero tail. */
+int c2m_dcn_tc_operand_psa(const void *hi, const void *lo, int B, int C, int H, int W, int dg, void *x_il,
+                           c2m_stream_t stream);
+/* fp32 x [B,C,H,W] (element strides; dense NCHW or channels-last) -> x_il (operand * 2^sa and zero tail) and amax[B]
+ * (bits of each image's largest finite |x|); with mask != NULL (the final mask [B,dg*9,H,W], contiguous) also
+ * amax[B + b] for the mask.  NaN and Inf do not count towards a maximum. */
+int c2m_dcn_tc_operand_f32(const float *x, int B, int C, int H, int W, long long xs_b, long long xs_c, long long xs_y,
+                           long long xs_x, int dg, const float *mask, void *x_il, unsigned *amax, c2m_stream_t stream);
 
 /* --- ordered input gradients (used when torch's deterministic algorithms are enabled) -----------------------------
  * Same results as the col2im / PS-ROI grad_input scatters above, except that every element of grad_input is a sum in
