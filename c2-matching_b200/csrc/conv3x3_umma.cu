@@ -211,13 +211,20 @@ conv3x3_wgmma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
             asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");          // previous tile's epilogue is done
             acc_store(acc_s, wg * 64, v);
             asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+            // The residual pointer is a constant in each call: a selected `has1 ? &ra : nullptr` would put `ra` in
+            // local memory, and its store there would wait for the prefetch in front of the MMAs.
             if (c0 < N) {
-                if (full_blk)
+                if (full_blk && has1)
                     epilogue_fast_dispatch(q, p, acc_s + e, c0, b, y, x, ok, o_base, sbias + UC_NMAX, out_scale * so,
-                                           res_scale * so, has1 ? &ra : nullptr);
+                                           res_scale * so, &ra);
+                else if (full_blk)
+                    epilogue_fast_dispatch(q, p, acc_s + e, c0, b, y, x, ok, o_base, sbias + UC_NMAX, out_scale * so,
+                                           res_scale * so, nullptr);
+                else if (has1)
+                    epilogue_store_block(q, p, acc_s + e, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, so, &ra);
                 else
                     epilogue_store_block(q, p, acc_s + e, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, so,
-                                         has1 ? &ra : nullptr);
+                                         nullptr);
             }
         }
     }
