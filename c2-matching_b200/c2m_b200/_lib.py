@@ -79,6 +79,12 @@ SYMBOLS = {
     'c2m_psa_to_f32': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 5 + [c_f32p, c_f32p] +
                        [ctypes.c_longlong] * 4 + [ctypes.c_void_p]),
     'c2m_conv3x3': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
+    'c2m_grad_psa_from_f32': (ctypes.c_int, [c_f32p] + [ctypes.c_int] * 4 + [ctypes.c_longlong] * 4 +
+                              [ctypes.c_void_p] * 4),
+    'c2m_grad_unscale_f32': (ctypes.c_int, [c_f32p, ctypes.c_longlong, ctypes.c_void_p, ctypes.c_void_p]),
+    'c2m_conv3x3_wgrad_workspace_bytes': (ctypes.c_size_t, [ctypes.c_int] * 5),
+    'c2m_conv3x3_wgrad': (ctypes.c_int, [ctypes.c_void_p] * 5 + [ctypes.c_int] * 5 +
+                          [c_f32p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
     'c2m_psa_maxpool2': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 4 + [ctypes.c_void_p] * 3),
     'c2m_dcn_tc_supported': (ctypes.c_int, [ctypes.c_int] * 3),
     'c2m_dcn_tc_packed_weight_bytes': (ctypes.c_size_t, [ctypes.c_int] * 3),

@@ -382,33 +382,41 @@ def invalidate_packs(obj):
         d = getattr(t, '__dict__', None)
         if d is not None:
             d.pop('_c2m_pack', None)
+            d.pop('_c2m_pack_dgrad', None)
             d.pop('_c2m_dcn_pack', None)
         _fallback_packs.pop(id(t), None)
 
 
-def conv3x3_pack_weights(weight):
-    """Pack a [Cout,Cin,3,3] fp32 weight for c2m_conv3x3_psa (cached, see _pack_cached)."""
+def conv3x3_pack_weights(weight, dgrad=False):
+    """Pack a [Cout,Cin,3,3] fp32 weight for c2m_conv3x3_psa (cached, see _pack_cached).  dgrad: pack the weights of the
+    input gradient instead, W'[ci][co][ky][kx] = W[co][ci][2-ky][2-kx] (a Cout -> Cin convolution)."""
     _require_cuda('weight', weight)
     cout, cin = weight.shape[:2]
+    if dgrad:
+        cout, cin = cin, cout
 
     def make():
+        w = weight.detach()
+        w = (w.transpose(0, 1).flip(2, 3) if dgrad else w).contiguous()
         n = _lib.lib().c2m_conv3x3_packed_weight_bytes(cin, cout)
         blob = torch.empty(n, dtype=torch.uint8, device=weight.device)
         with torch.cuda.device(weight.device):
-            rc = _lib.lib().c2m_conv3x3_pack_weights_f32(weight.detach().contiguous().data_ptr(), cin, cout,
-                                                         blob.data_ptr(), _stream())
+            rc = _lib.lib().c2m_conv3x3_pack_weights_f32(w.data_ptr(), cin, cout, blob.data_ptr(), _stream())
             _lib.check(rc, 'c2m_conv3x3_pack_weights_f32')
         return blob
-    return _pack_cached(weight, '_c2m_pack', None, make)
+    return _pack_cached(weight, '_c2m_pack_dgrad' if dgrad else '_c2m_pack', None, make)
 
 
 _ACT = {None: 0, 'none': 0, 'relu': 1, 'lrelu': 2}
 
 
 def conv3x3_psa(x, weight, bias, act=None, residual=None, residual2=None, x2=None, out=None, sa_out=0,
-                pixel_shuffle=0, out_f32=False, add_f32=None, psa_out=True, channels_last=False, f32_octets=False):
+                pixel_shuffle=0, out_f32=False, add_f32=None, psa_out=True, channels_last=False, f32_octets=False,
+                packed=None):
     """y = act(conv3x3(cat[x, x2], weight) + bias), fp32-grade on tensor cores.
     f32_octets: the fp32 result is an OctF32 (octet-planar) instead of a strided tensor.
+    packed: a packed blob of `weight` made elsewhere (the input gradient's rotated weights); `weight` then only gives
+    the shape.
 
     Returns the PSA tensor `y + residual + residual2` (or PixelShuffle(2)(y)), and/or — with
     out_f32=True — the fp32 tensor `y + add_f32`.  With both, returns (psa, f32)."""
@@ -416,7 +424,7 @@ def conv3x3_psa(x, weight, bias, act=None, residual=None, residual2=None, x2=Non
     c_in = x.C + (x2.C if x2 is not None else 0)
     if cin != c_in:
         raise RuntimeError(f'conv3x3_psa: weight expects {cin} input channels, got {c_in}')
-    blob = conv3x3_pack_weights(weight)
+    blob = conv3x3_pack_weights(weight) if packed is None else packed
     dev = x.hi.device
     a = _lib.ConvArgs()
     a.in_hi, a.in_lo, a.Cin = x.hi.data_ptr(), x.lo.data_ptr(), x.C
@@ -466,6 +474,77 @@ def conv3x3_psa(x, weight, bias, act=None, residual=None, residual2=None, x2=Non
     if ret_psa is not None and ret_f32 is not None:
         return ret_psa, ret_f32
     return ret_psa if ret_psa is not None else ret_f32
+
+
+class _Conv3x3(torch.autograd.Function):
+    """Forward on conv3x3_wgmma_kernel; backward: the activation's backward, dX on the same kernel with the rotated
+    weights, dW on conv3x3_wgrad_kernel, db as a torch sum.  grad_output enters the kernels as PSA at a power-of-two
+    scale chosen on the device (c2m_grad_psa_from_f32), which the results divide back out on the device."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, act):
+        xp = psa_from_f32(x)
+        y = conv3x3_psa(xp, weight, bias, act=act, psa_out=False, out_f32=True)
+        ctx.act = act
+        ctx.save_for_backward(xp.hi, xp.lo, weight, y if act else None)
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        x_hi, x_lo, weight, y = ctx.saved_tensors
+        need_x, need_w, need_b = ctx.needs_input_grad[:3]
+        B, c8, H, W, _ = x_hi.shape
+        cout, cin = weight.shape[:2]
+        if ctx.act == 'relu':
+            gy = torch.where(y > 0, gy, 0.)
+        elif ctx.act == 'lrelu':
+            gy = torch.where(y > 0, gy, gy * 0.1)
+        L = _lib.lib()
+        dev = gy.device
+        dx = dw = db = None
+        with torch.cuda.device(dev):
+            gp = PSA.empty(B, cout, H, W, dev)
+            amax = torch.empty(1, dtype=torch.int32, device=dev)
+            _lib.check(L.c2m_grad_psa_from_f32(gy.data_ptr(), B, cout, H, W, *gy.stride(), gp.hi.data_ptr(),
+                                               gp.lo.data_ptr(), amax.data_ptr(), _stream()), 'c2m_grad_psa_from_f32')
+            if need_x:
+                dx = conv3x3_psa(gp, weight.transpose(0, 1), None, psa_out=False, out_f32=True,
+                                 packed=conv3x3_pack_weights(weight, dgrad=True))
+                _lib.check(L.c2m_grad_unscale_f32(dx.data_ptr(), dx.numel(), amax.data_ptr(), _stream()),
+                           'c2m_grad_unscale_f32')
+            if need_w:
+                dw = torch.empty(cout, cin, 3, 3, dtype=torch.float32, device=dev)
+                nbytes = L.c2m_conv3x3_wgrad_workspace_bytes(B, cin, cout, H, W)
+                if nbytes == 0:
+                    raise C2MError('c2m_conv3x3_wgrad_workspace_bytes: ' + L.c2m_last_error().decode(errors='replace'))
+                ws = _workspace(nbytes, dev)
+                _lib.check(L.c2m_conv3x3_wgrad(gp.hi.data_ptr(), gp.lo.data_ptr(), amax.data_ptr(), x_hi.data_ptr(),
+                                               x_lo.data_ptr(), B, cin, cout, H, W, dw.data_ptr(), ws.data_ptr(),
+                                               nbytes, _stream()), 'c2m_conv3x3_wgrad')
+            if need_b:
+                db = gy.sum((0, 2, 3))
+        return dx, dw, db, None
+
+
+def conv3x3(x, weight, bias=None, act=None):
+    """Differentiable act(conv2d(x, weight, bias, stride 1, padding 1)) on the tensor cores, fp32-grade forward and
+    backward (fp32 in, fp32 out).  x [B,Cin,H,W] with H >= 18 and W >= 10, weight [Cout,Cin,3,3], bias [Cout] or None,
+    act None / 'relu' / 'lrelu' (LeakyReLU(0.1)).  The forward converts x to PSA at scale exponent 0, so |x| must stay
+    within fp16's range (the inference path's contract for activations); the backward scales grad_output itself."""
+    _require_cuda('x', x)
+    _require_cuda('weight', weight)
+    if bias is not None:
+        _require_cuda('bias', bias)
+    if act not in (None, 'relu', 'lrelu'):
+        raise ValueError(f'conv3x3: act must be None, relu or lrelu, got {act!r}')
+    if x.dim() != 4 or weight.dim() != 4 or tuple(weight.shape[1:]) != (x.shape[1], 3, 3):
+        raise RuntimeError(f'conv3x3: weight {tuple(weight.shape)} does not fit input {tuple(x.shape)} '
+                           '(expected [Cout, Cin, 3, 3])')
+    if bias is not None and tuple(bias.shape) != (weight.shape[0],):
+        raise RuntimeError(f'conv3x3: bias {tuple(bias.shape)} does not fit {weight.shape[0]} output channels')
+    if not conv3x3_supported(x.shape[1], weight.shape[0], x.shape[2], x.shape[3]):
+        raise RuntimeError(f'conv3x3: map {x.shape[2]}x{x.shape[3]} smaller than one halo tile (18x10)')
+    return _Conv3x3.apply(x, weight, bias, act)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -234,13 +234,14 @@ conv3x3_wgmma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
 // PSA <-> strided fp32 converters and the weight pre-pack
 // ------------------------------------------------------------------------------------------
 __global__ void psa_from_f32_kernel(const float *__restrict__ x, int C, int C8, int H, int W, long long xs_b,
-                                    long long xs_c, long long xs_y, long long xs_x, int sa, __half *__restrict__ hi,
+                                    long long xs_c, long long xs_y, long long xs_x, int sa,
+                                    const unsigned *__restrict__ amax, __half *__restrict__ hi,
                                     __half *__restrict__ lo) {
     // one thread = one (octet, pixel); pixel fastest -> coalesced NCHW reads and 16 B stores
     const long long HW = (long long)H * W;
     const long long n = (long long)C8 * HW;
     const int b = blockIdx.y;
-    const float S = ldexpf(1.f, sa);
+    const float S = ldexpf(1.f, amax ? grad_scale_exp(amax) : sa);
     for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x) {
         const int oct = (int)(e / HW);
         const long long pix = e % HW;
@@ -397,7 +398,7 @@ extern "C" int c2m_psa_from_f32(const float *x, int B, int C, int H, int W, long
     int bx = (int)((n + 255) / 256);
     if (bx > 4096) bx = 4096;
     psa_from_f32_kernel<<<dim3(bx, B), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-        x, C, C8, H, W, xs_b, xs_c, xs_y, xs_x, sa, reinterpret_cast<__half *>(hi), reinterpret_cast<__half *>(lo));
+        x, C, C8, H, W, xs_b, xs_c, xs_y, xs_x, sa, nullptr, reinterpret_cast<__half *>(hi), reinterpret_cast<__half *>(lo));
     C2M_LAUNCH_CHECK("psa_from_f32_kernel");
     return C2M_OK;
 }

@@ -31,6 +31,21 @@ __device__ __forceinline__ float wpack_scale(uint8_t *blob) {
     return ldexpf(1.f, s_sw);
 }
 
+// Gradient scale exponent: sg = 14 - floor(log2 amax) (amax * 2^sg in [2^14, 2^15)), from the bits of the largest finite
+// |grad_output|; 0 for an all-zero gradient, clamped to +-120 so that 2^sg and 2^-sg are normal floats.
+__host__ __device__ __forceinline__ int grad_scale_exp(const unsigned *amax) {
+    const unsigned bits = *amax;
+    if (bits == 0u) return 0;
+    const int s = 14 - ((int)(bits >> 23) - 127);
+    return s < -120 ? -120 : s > 120 ? 120 : s;
+}
+
+// fp32 [B,C,H,W] (element strides) -> PSA x * 2^sa, or x * 2^grad_scale_exp(amax) when amax is not null
+// (conv3x3_umma.cu; grid (blocks, B))
+__global__ void psa_from_f32_kernel(const float *__restrict__ x, int C, int C8, int H, int W, long long xs_b,
+                                    long long xs_c, long long xs_y, long long xs_x, int sa,
+                                    const unsigned *__restrict__ amax, __half *__restrict__ hi, __half *__restrict__ lo);
+
 struct ConvParams {
     int B, H, W;
     int nkc_a, nkc;           // K chunks taken from input 1 / in total (input 2 supplies the rest)

@@ -17,6 +17,7 @@ from torch import nn
 from torch.nn.modules.utils import _pair
 
 from c2m_b200 import ops as _ops
+from ..arch_util import Conv2d
 
 logger = logging.getLogger('base')
 
@@ -82,8 +83,8 @@ class _WithOffsetConv(DCNv2):
         super().__init__(*args, **kwargs)
         if extra_offset_mask is not None:
             self.extra_offset_mask = extra_offset_mask
-        self.conv_offset_mask = nn.Conv2d(self.in_channels, 3 * self.deformable_groups * self.kernel_size[0] *
-                                          self.kernel_size[1], self.kernel_size, self.stride, self.padding, bias=True)
+        self.conv_offset_mask = Conv2d(self.in_channels, 3 * self.deformable_groups * self.kernel_size[0] *
+                                       self.kernel_size[1], self.kernel_size, self.stride, self.padding, bias=True)
         self.init_offset()
 
     def init_offset(self):

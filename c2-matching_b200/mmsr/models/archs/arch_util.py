@@ -36,8 +36,8 @@ class ResidualBlockNoBN(nn.Module):
     def __init__(self, nf=64, res_scale=1, pytorch_init=False):
         super().__init__()
         self.res_scale = res_scale
-        self.conv1 = nn.Conv2d(nf, nf, 3, 1, 1, bias=True)
-        self.conv2 = nn.Conv2d(nf, nf, 3, 1, 1, bias=True)
+        self.conv1 = Conv2d(nf, nf, 3, 1, 1, bias=True)
+        self.conv2 = Conv2d(nf, nf, 3, 1, 1, bias=True)
         if not pytorch_init:
             default_init_weights([self.conv1, self.conv2], 0.1)
 
@@ -70,8 +70,26 @@ def psa_path_ok(x, *convs, cat_first=32):
                 f'c2m: feature map {x.shape[2]}x{x.shape[3]} is smaller than one halo tile (18x10): the plain 3x3 convolutions '
                 'of this call run on nn.Conv2d (cuDNN, TF32 off), not on the tensor-core kernel')
         return False
-    return all(isinstance(c, nn.Conv2d) and c.kernel_size == (3, 3) and c.stride == (1, 1) and c.padding == (1, 1) and
-               c.dilation == (1, 1) and c.groups == 1 and c.weight.is_cuda for c in convs) and cat_first % 32 == 0
+    return all(_tc_conv(c) for c in convs) and cat_first % 32 == 0
+
+
+def _tc_conv(c):
+    """A convolution the tensor-core 3x3 kernel computes: 3x3 / stride 1 / pad 1 / dilation 1 / one group, on the GPU."""
+    return (isinstance(c, nn.Conv2d) and c.kernel_size == (3, 3) and c.stride == (1, 1) and c.padding == (1, 1) and
+            c.dilation == (1, 1) and c.groups == 1 and c.weight.is_cuda)
+
+
+class Conv2d(nn.Conv2d):
+    """nn.Conv2d (same parameters and state-dict keys) whose 3x3 / stride 1 / pad 1 instances run forward and backward
+    on the tensor cores (c2m_b200.ops.conv3x3) under autograd, on the maps the inference path takes there: fp32 CUDA,
+    at least 18x10, C2M_FAST_CONV not 0.  Everything else, inference under no_grad included, is nn.Conv2d."""
+
+    def forward(self, x):
+        if (torch.is_grad_enabled() and fast_conv_enabled() and _tc_conv(self) and self.padding_mode == 'zeros' and
+                x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and x.shape[2] >= 18 and x.shape[3] >= 10):
+            from c2m_b200 import ops
+            return ops.conv3x3(x, self.weight, self.bias)
+        return super().forward(x)
 
 
 def conv_psa(conv, xp, act=None, **kw):

@@ -21,7 +21,7 @@ class ContentExtractor(nn.Module):
 
     def __init__(self, in_nc=3, out_nc=3, nf=64, n_blocks=16):
         super().__init__()
-        self.conv_first = nn.Conv2d(in_nc, nf, 3, 1, 1)
+        self.conv_first = arch_util.Conv2d(in_nc, nf, 3, 1, 1)
         self.body = arch_util.make_layer(arch_util.ResidualBlockNoBN, n_blocks, nf=nf)
         arch_util.default_init_weights([self.conv_first], 0.1)
 
@@ -42,16 +42,16 @@ class DynamicAggregationRestoration(nn.Module):
     def __init__(self, ngf=64, n_blocks=16, groups=8):
         super().__init__()
         for size, _, c in _LEVELS:
-            setattr(self, f'{size}_offset_conv1', nn.Conv2d(ngf + c, c, 3, 1, 1, bias=True))
-            setattr(self, f'{size}_offset_conv2', nn.Conv2d(c, c, 3, 1, 1, bias=True))
+            setattr(self, f'{size}_offset_conv1', arch_util.Conv2d(ngf + c, c, 3, 1, 1, bias=True))
+            setattr(self, f'{size}_offset_conv2', arch_util.Conv2d(c, c, 3, 1, 1, bias=True))
             setattr(self, f'{size}_dyn_agg', DynAgg(c, c, 3, stride=1, padding=1, dilation=1,
                                                     deformable_groups=groups, extra_offset_mask=True))
-            setattr(self, f'head_{size}', nn.Sequential(nn.Conv2d(ngf + c, ngf, 3, 1, 1), nn.LeakyReLU(0.1, True)))
+            setattr(self, f'head_{size}', nn.Sequential(arch_util.Conv2d(ngf + c, ngf, 3, 1, 1), nn.LeakyReLU(0.1, True)))
             setattr(self, f'body_{size}', arch_util.make_layer(arch_util.ResidualBlockNoBN, n_blocks, nf=ngf))
-        self.tail_small = nn.Sequential(nn.Conv2d(ngf, ngf * 4, 3, 1, 1), nn.PixelShuffle(2), nn.LeakyReLU(0.1, True))
-        self.tail_medium = nn.Sequential(nn.Conv2d(ngf, ngf * 4, 3, 1, 1), nn.PixelShuffle(2), nn.LeakyReLU(0.1, True))
-        self.tail_large = nn.Sequential(nn.Conv2d(ngf, ngf // 2, 3, 1, 1), nn.LeakyReLU(0.1, True),
-                                        nn.Conv2d(ngf // 2, 3, 3, 1, 1))
+        self.tail_small = nn.Sequential(arch_util.Conv2d(ngf, ngf * 4, 3, 1, 1), nn.PixelShuffle(2), nn.LeakyReLU(0.1, True))
+        self.tail_medium = nn.Sequential(arch_util.Conv2d(ngf, ngf * 4, 3, 1, 1), nn.PixelShuffle(2), nn.LeakyReLU(0.1, True))
+        self.tail_large = nn.Sequential(arch_util.Conv2d(ngf, ngf // 2, 3, 1, 1), nn.LeakyReLU(0.1, True),
+                                        arch_util.Conv2d(ngf // 2, 3, 3, 1, 1))
 
     @staticmethod
     def _pre(pre_offset, key):

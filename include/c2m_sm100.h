@@ -187,6 +187,27 @@ int c2m_psa_from_f32(const float *x, int B, int C, int H, int W, long long xs_b,
 int c2m_psa_to_f32(const void *hi, const void *lo, int B, int C, int H, int W, int sa, const float *add, float *out,
                    long long os_b, long long os_c, long long os_y, long long os_x, c2m_stream_t stream);
 int c2m_conv3x3(const c2m_conv3x3_args *args, c2m_stream_t stream);
+/* Backward of the convolution above (3x3 / stride 1 / pad 1, one input), fp32-grade, no host synchronisation.
+ * c2m_grad_psa_from_f32: grad_output g [B,C,H,W] fp32 (element strides) -> PSA hi / lo holding g * 2^sg, where
+ *   sg = 14 - floor(log2 amax) and amax, the largest finite |g| (NaN and Inf do not count; 0 gives sg = 0; sg is
+ *   clamped to +-120), is computed on the device and its fp32 bits stored in *amax (device memory, 4 bytes).  Scaling
+ *   g by 2^k leaves the PSA planes bit for bit the same, so the gradients below scale by exactly 2^k while in range.
+ * Input gradient: c2m_conv3x3 of that PSA tensor (sa_in = 0, Cin = the forward's Cout, Cout = the forward's Cin) with
+ *   the weights W'[ci][co][ky][kx] = W[co][ci][2-ky][2-kx] packed by c2m_conv3x3_pack_weights_f32, fp32 output, then
+ *   c2m_grad_unscale_f32 on that output: x[i] *= 2^-sg for n elements.
+ * c2m_conv3x3_wgrad: dW[co][ci][ky][kx] = sum over b, y, x of g[b,co,y,x] * x[b,ci,y+ky-1,x+kx-1] (zero outside the
+ *   map), written to dw [Cout,Cin,3,3] fp32.  gy_* / gy_amax: the output of c2m_grad_psa_from_f32; x_*: the forward's
+ *   input as PSA at scale exponent 0.  Split-K over CTAs with per-CTA partials in `ws` (at least
+ *   c2m_conv3x3_wgrad_workspace_bytes(B, Cin, Cout, H, W) bytes, which depends on the device's SM count), summed in one
+ *   fixed order: the same bits on every run on a given device.  Needs H >= 18 and W >= 10, like c2m_conv3x3.
+ */
+int c2m_grad_psa_from_f32(const float *g, int B, int C, int H, int W, long long gs_b, long long gs_c, long long gs_y,
+                          long long gs_x, void *hi, void *lo, unsigned *amax, c2m_stream_t stream);
+int c2m_grad_unscale_f32(float *x, long long n, const unsigned *amax, c2m_stream_t stream);
+size_t c2m_conv3x3_wgrad_workspace_bytes(int B, int Cin, int Cout, int H, int W);   /* 0 on a bad shape */
+int c2m_conv3x3_wgrad(const void *gy_hi, const void *gy_lo, const unsigned *gy_amax, const void *x_hi, const void *x_lo,
+                      int B, int Cin, int Cout, int H, int W, float *dw, void *ws, size_t ws_bytes,
+                      c2m_stream_t stream);
 /* MaxPool2d(2, 2) on a PSA tensor (floor semantics: odd trailing row / column dropped), PSA result. */
 int c2m_psa_maxpool2(const void *hi, const void *lo, int B, int C, int H, int W, void *out_hi, void *out_lo,
                      c2m_stream_t stream);
