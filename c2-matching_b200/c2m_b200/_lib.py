@@ -48,6 +48,17 @@ class DcnTcArgs(ctypes.Structure):
                 ('mask', ctypes.c_void_p), ('x_amax', ctypes.c_void_p), ('mask_amax', ctypes.c_void_p)]
 
 
+class DcnTcGradArgs(ctypes.Structure):
+    """c2m_dcn_tc_grad_args (include/c2m_sm100.h)."""
+    _fields_ = [('gy_hi', ctypes.c_void_p), ('gy_lo', ctypes.c_void_p), ('gy_amax', ctypes.c_void_p),
+                ('x_il', ctypes.c_void_p), ('x_amax', ctypes.c_void_p), ('mask_amax', ctypes.c_void_p),
+                ('offset', ctypes.c_void_p), ('mask', ctypes.c_void_p)] + \
+               [(n, ctypes.c_int) for n in ('B', 'C', 'H', 'W', 'Cout', 'dg')] + \
+               [('packed_w', ctypes.c_void_p), ('grad_offset', ctypes.c_void_p), ('grad_mask', ctypes.c_void_p),
+                ('grad_input', ctypes.c_void_p), ('grad_weight', ctypes.c_void_p), ('ws', ctypes.c_void_p),
+                ('ws_bytes', ctypes.c_size_t)]
+
+
 class PsroiShape(ctypes.Structure):
     """c2m_psroi_shape (include/c2m_sm100.h)."""
     _fields_ = [(n, ctypes.c_int) for n in ('B', 'C', 'H', 'W', 'R', 'no_trans', 'num_classes')] + \
@@ -95,6 +106,12 @@ SYMBOLS = {
                                [ctypes.c_void_p] * 2),
     'c2m_dcn_tc_operand_f32': (ctypes.c_int, [c_f32p] + [ctypes.c_int] * 4 + [ctypes.c_longlong] * 4 +
                                [ctypes.c_int, c_f32p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    'c2m_dcn_tc_dgrad_packed_weight_bytes': (ctypes.c_size_t, [ctypes.c_int] * 3),
+    'c2m_dcn_tc_pack_dgrad_weights_f32': (ctypes.c_int, [c_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                                         ctypes.c_void_p, ctypes.c_void_p]),
+    'c2m_dcn_tc_dgrad': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
+    'c2m_dcn_tc_wgrad_workspace_bytes': (ctypes.c_size_t, [ctypes.c_int] * 6),
+    'c2m_dcn_tc_wgrad': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
     'c2m_profile_enable': (ctypes.c_int, [ctypes.c_int]),
     'c2m_profile_collect': (ctypes.c_int, [ctypes.c_int, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_int),
                                            ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double)]),

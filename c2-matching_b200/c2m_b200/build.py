@@ -7,7 +7,7 @@ CSRC = os.path.join(PKG_ROOT, 'csrc')
 LIB_DIR = os.path.join(PKG_ROOT, 'lib')
 LIB_PATH = os.path.join(LIB_DIR, 'libc2m_sm100.so')
 SOURCES = ['c_abi.cu', 'corr_aux.cu', 'corr_umma.cu', 'dcn_v2.cu', 'offsets.cu', 'conv3x3_umma.cu', 'dcn_umma.cu', 'dcn_bwd.cu',
-           'psroi.cu', 'det_gather.cu', 'conv3x3_wgrad.cu']
+           'psroi.cu', 'det_gather.cu', 'conv3x3_wgrad.cu', 'dcn_tc_bwd.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-shared', '-Xcompiler', '-fPIC']
 

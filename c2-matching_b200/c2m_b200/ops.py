@@ -32,7 +32,7 @@ def profile_enable(on=True):
     _lib.check(_lib.lib().c2m_profile_enable(int(bool(on))), 'c2m_profile_enable')
 
 
-PROF_KERNELS = {'corr_search': 0, 'conv3x3': 1, 'dcn': 2}
+PROF_KERNELS = {'corr_search': 0, 'conv3x3': 1, 'dcn': 2, 'dcn_dgrad': 3, 'dcn_wgrad': 4}
 
 
 def profile_collect(kernel):
@@ -384,6 +384,7 @@ def invalidate_packs(obj):
             d.pop('_c2m_pack', None)
             d.pop('_c2m_pack_dgrad', None)
             d.pop('_c2m_dcn_pack', None)
+            d.pop('_c2m_dcn_pack_dgrad', None)
         _fallback_packs.pop(id(t), None)
 
 
@@ -652,6 +653,105 @@ def dcn_v2_fused_tc(x, om, weight, bias, deformable_group, pre_offset=None, idx=
     if ret_p is not None and ret_f is not None:
         return ret_p, ret_f
     return ret_p if ret_p is not None else ret_f
+
+
+def _dcn_tc_pack_dgrad(weight, dg):
+    cout, c = weight.shape[:2]
+
+    def make():
+        n = _lib.lib().c2m_dcn_tc_dgrad_packed_weight_bytes(c, cout, dg)
+        blob = torch.empty(n, dtype=torch.uint8, device=weight.device)
+        with torch.cuda.device(weight.device):
+            rc = _lib.lib().c2m_dcn_tc_pack_dgrad_weights_f32(weight.detach().contiguous().data_ptr(), c, cout, dg,
+                                                              blob.data_ptr(), _stream())
+            _lib.check(rc, 'c2m_dcn_tc_pack_dgrad_weights_f32')
+        return blob
+    return _pack_cached(weight, '_c2m_dcn_pack_dgrad', dg, make)
+
+
+class _DcnV2Tc(torch.autograd.Function):
+    """Forward: the tensor-core launch of `_ext.dcn_v2_forward` (dcn_v2_fused_tc with the final mask).  Backward:
+    grad_output as PSA at a power-of-two scale chosen on the device (c2m_grad_psa_from_f32), then
+    dcn_dgrad_kernel for grad_offset / grad_mask (and grad_input when x requires it) and dcn_wgrad_kernel for the
+    weight gradient; db is a torch sum."""
+
+    @staticmethod
+    def forward(ctx, x, offset, mask, weight, bias, dg):
+        offset, mask = offset.contiguous(), mask.contiguous()
+        ctx.dg = dg
+        ctx.save_for_backward(x, offset, mask, weight)
+        return dcn_v2_fused_tc(x, offset, weight, bias, dg, final_mask=mask)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, gy):
+        import ctypes
+        x, offset, mask, weight = ctx.saved_tensors
+        need_x, need_off, need_mask, need_w, need_b = ctx.needs_input_grad[:5]
+        dg = ctx.dg
+        x = _dense_nchw_or_nhwc(x)
+        B, C, H, W = x.shape
+        cout = weight.shape[0]
+        gy = gy.contiguous()
+        L = _lib.lib()
+        dev = gy.device
+        gx = goff = gmask = dw = db = None
+        with torch.cuda.device(dev):
+            gp = PSA.empty(B, cout, H, W, dev)
+            gamax = torch.empty(1, dtype=torch.int32, device=dev)
+            _lib.check(L.c2m_grad_psa_from_f32(gy.data_ptr(), B, cout, H, W, *gy.stride(), gp.hi.data_ptr(),
+                                               gp.lo.data_ptr(), gamax.data_ptr(), _stream()), 'c2m_grad_psa_from_f32')
+            # the forward's operand, made again: x * 2^sa and mask * 2^sm per image
+            x_il = torch.empty(L.c2m_dcn_tc_operand_bytes(B, C, H, W, dg) // 2, dtype=torch.float16, device=dev)
+            amax = torch.empty(2 * B, dtype=torch.int32, device=dev)
+            _lib.check(L.c2m_dcn_tc_operand_f32(x.data_ptr(), B, C, H, W, *x.stride(), dg, mask.data_ptr(),
+                                                x_il.data_ptr(), amax.data_ptr(), _stream()), 'c2m_dcn_tc_operand_f32')
+            a = _lib.DcnTcGradArgs()
+            a.gy_hi, a.gy_lo, a.gy_amax = gp.hi.data_ptr(), gp.lo.data_ptr(), gamax.data_ptr()
+            a.x_il, a.x_amax, a.mask_amax = x_il.data_ptr(), amax.data_ptr(), amax.data_ptr() + 4 * B
+            a.offset, a.mask = offset.data_ptr(), mask.data_ptr()
+            a.B, a.C, a.H, a.W, a.Cout, a.dg = B, C, H, W, cout, dg
+            if need_x or need_off or need_mask:
+                goff, gmask = torch.empty_like(offset), torch.empty_like(mask)
+                a.packed_w = _dcn_tc_pack_dgrad(weight, dg).data_ptr()
+                a.grad_offset, a.grad_mask = goff.data_ptr(), gmask.data_ptr()
+                if need_x:
+                    gx = torch.zeros(B, C, H, W, dtype=torch.float32, device=dev)
+                    a.grad_input = gx.data_ptr()
+                _lib.check(L.c2m_dcn_tc_dgrad(ctypes.addressof(a), _stream()), 'c2m_dcn_tc_dgrad')
+            if need_w:
+                dw = torch.empty(cout, C, 3, 3, dtype=torch.float32, device=dev)
+                nbytes = L.c2m_dcn_tc_wgrad_workspace_bytes(B, C, H, W, cout, dg)
+                if nbytes == 0:
+                    raise C2MError('c2m_dcn_tc_wgrad_workspace_bytes: ' + L.c2m_last_error().decode(errors='replace'))
+                ws = _workspace(nbytes, dev)
+                a.grad_weight, a.ws, a.ws_bytes = dw.data_ptr(), ws.data_ptr(), nbytes
+                _lib.check(L.c2m_dcn_tc_wgrad(ctypes.addressof(a), _stream()), 'c2m_dcn_tc_wgrad')
+            if need_b:
+                db = gy.sum((0, 2, 3))
+        return (gx, goff if need_off else None, gmask if need_mask else None, dw, db, None)
+
+
+def dcn_tc_backward_supported(C, Cout, dg, H, W):
+    """Shapes the tensor-core DCN backward takes: the forward's (dcn_tc_supported) on maps of at least 16 x 8."""
+    return dcn_tc_supported(C, Cout, dg) and H >= 16 and W >= 8
+
+
+def dcn_v2_tc(x, offset, mask, weight, bias, deformable_group):
+    """Differentiable modulated deformable convolution, 3x3 / stride 1 / pad 1 / dilation 1, on the tensor cores
+    forward and backward (fp32-grade).  The `_ext` contract: final offsets [B,2*dg*9,H,W] and final mask [B,dg*9,H,W];
+    the output equals `_ext.dcn_v2_forward`'s tensor-core route bit for bit.  Gradients flow to every input that
+    requires one; grad_input is summed with atomics, every other gradient in a fixed order."""
+    for n, t in (('x', x), ('offset', offset), ('mask', mask), ('weight', weight)):
+        _require_cuda(n, t)
+    if bias is not None:
+        _require_cuda('bias', bias)
+    B, C, H, W = x.shape
+    if tuple(weight.shape) != (weight.shape[0], C, 3, 3):
+        raise RuntimeError(f'dcn_v2_tc: weight {tuple(weight.shape)} does not fit input {tuple(x.shape)}')
+    if not dcn_tc_backward_supported(C, weight.shape[0], deformable_group, H, W):
+        raise RuntimeError(f'dcn_v2_tc: C={C} Cout={weight.shape[0]} dg={deformable_group} on {H}x{W} unsupported')
+    return _DcnV2Tc.apply(x, offset, mask, weight, bias, deformable_group)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -45,19 +45,6 @@ struct WgradGeom {
     int tiles_x, tiles_y;
     long long ntiles;
 };
-
-// wgmma m64n32k16, fp16 x fp16 -> fp32, both operands MN-major in shared memory (imm-trans-a = imm-trans-b = 1)
-__device__ __forceinline__ void wgmma_tt_n32(float (&d)[16], uint64_t da, uint64_t db) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-        "%16, %17, p, 1, 1, 1, 1;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
-          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-        : "l"(da), "l"(db), "r"(1)
-        : "memory");
-}
 }  // namespace
 
 // Largest finite |g| of a strided [B,C,H,W] tensor as fp32 bits (NaN and Inf do not set the scale); *amax starts at 0.

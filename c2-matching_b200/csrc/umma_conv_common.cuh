@@ -40,6 +40,24 @@ __host__ __device__ __forceinline__ int grad_scale_exp(const unsigned *amax) {
     return s < -120 ? -120 : s > 120 ? 120 : s;
 }
 
+// Per-image operand exponents of the tensor-core DCN kernels' fp32 boundary (dcn_umma.cu, dcn_tc_bwd.cu), from the bits of the image's largest finite magnitude (0 -> 0).
+// x: amax * 2^s in [2^11, 2^12), under fp16's 65504 with 16x headroom for the blend and well above its subnormals.
+// mask: max |mask| * 2^s in [1, 2), so the corner weights are at most 2.  Exponent arithmetic only: scaling an image
+// by 2^k shifts its exponent by -k and leaves the operand bit for bit the same.  Each exponent is clamped to +-120, so
+// 2^sa and 2^sm are normal floats.  Their sum with the weight exponent sw is not clamped: the epilogue's
+// 2^-(sa + sm + sw) leaves fp32's range (flushing the output to 0 or overflowing it) only when it exceeds 149 or
+// drops below -127.  Since amax(x) 2^sa is in [2^11, 2^12), amax(mask) 2^sm in [1, 2) and amax(w) 2^sw in
+// [2^13, 2^14), that happens only when amax(x) amax(mask) amax(w) is below 2^-121 or above 2^151: outputs at the
+// edge of fp32's range whatever computes them.
+__host__ __device__ __forceinline__ int amax_exp(unsigned bits, int top) {
+    if (bits == 0u) return 0;
+    const int e = (int)(bits >> 23) - 127;            // floor(log2 amax); a subnormal amax counts as 2^-127
+    const int s = top - e;
+    return s < -120 ? -120 : s > 120 ? 120 : s;
+}
+__device__ __forceinline__ int operand_exp(const unsigned *amax, int b) { return amax ? amax_exp(amax[b], 11) : 0; }
+__device__ __forceinline__ int mask_exp(const unsigned *amax, int b) { return amax ? amax_exp(amax[b], 0) : 0; }
+
 // fp32 [B,C,H,W] (element strides) -> PSA x * 2^sa, or x * 2^grad_scale_exp(amax) when amax is not null
 // (conv3x3_umma.cu; grid (blocks, B))
 __global__ void psa_from_f32_kernel(const float *__restrict__ x, int C, int C8, int H, int W, long long xs_b,

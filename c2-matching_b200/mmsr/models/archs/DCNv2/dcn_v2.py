@@ -161,8 +161,16 @@ class DCN_sep_pre_multi_offset(_WithOffsetConv):
             pre = pre_offset.materialize() if hasattr(pre_offset, 'materialize') else pre_offset
             n = om.shape[1] // 3
             reord = torch.stack((pre[..., 1], pre[..., 0]), dim=2).flatten(1, 2).repeat(1, self.deformable_groups, 1, 1)
-            out = dcn_v2_conv(x, om[:, :2 * n] + reord, torch.sigmoid(om[:, 2 * n:]), self.weight, self.bias,
-                              self.stride, self.padding, self.dilation, self.deformable_groups)
+            offset, mask = om[:, :2 * n] + reord, torch.sigmoid(om[:, 2 * n:])
+            # The tensor-core backward sums grad_input with atomics (every other gradient has a fixed order), and with
+            # grad_input it is slower than `_ext`'s on the 256-channel layer (DESIGN.md §4, K8): both cases keep `_ext`.
+            x_excluded = x.requires_grad and (_ops.deterministic() or self.in_channels >= 256)
+            if tc and not x_excluded and _ops.dcn_tc_backward_supported(self.in_channels, self.out_channels,
+                                                                        self.deformable_groups, *x.shape[2:]):
+                out = _ops.dcn_v2_tc(x, offset, mask, self.weight, self.bias, self.deformable_groups)
+            else:
+                out = dcn_v2_conv(x, offset, mask, self.weight, self.bias, self.stride, self.padding, self.dilation,
+                                  self.deformable_groups)
             out = out if lrelu_slope == 1.0 else torch.nn.functional.leaky_relu(out, lrelu_slope)
             return _ops.psa_from_f32(out) if want_psa else out
         idx = getattr(pre_offset, 'max_idx', None)

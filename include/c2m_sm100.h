@@ -260,6 +260,38 @@ int c2m_dcn_tc_operand_psa(const void *hi, const void *lo, int B, int C, int H, 
 int c2m_dcn_tc_operand_f32(const float *x, int B, int C, int H, int W, long long xs_b, long long xs_c, long long xs_y,
                            long long xs_x, int dg, const float *mask, void *x_il, unsigned *amax, c2m_stream_t stream);
 
+/* --- Backward of the tensor-core DCN (the `_ext` contract: final offsets and final mask) -------------------------
+ * Same shapes as c2m_dcn_v2_fused_tc (c2m_dcn_tc_supported), maps of at least 16 x 8.  Inputs:
+ *   gy_hi / gy_lo / gy_amax   grad_output [B,Cout,H,W] as PSA at the scale of c2m_grad_psa_from_f32
+ *   x_il, x_amax, mask_amax   the forward's operand: c2m_dcn_tc_operand_f32(x, ..., mask, x_il, amax) with
+ *                             x_amax = amax, mask_amax = amax + B
+ *   offset, mask              final offsets [B,2*dg*9,H,W] and final mask [B,dg*9,H,W], contiguous fp32
+ * c2m_dcn_tc_dgrad computes gcol = W^T gY on the tensor cores without storing it and writes grad_offset (shape of
+ * offset) and grad_mask (shape of mask), each element once in a fixed order.  With grad_input != NULL it also ADDS
+ * the input gradient into grad_input [B,C,H,W] (contiguous, caller zero-fills) with atomics.  packed_w: the weights
+ * packed by c2m_dcn_tc_pack_dgrad_weights_f32 into c2m_dcn_tc_dgrad_packed_weight_bytes(C, Cout, dg) bytes.
+ * c2m_dcn_tc_wgrad writes grad_weight [Cout,C,3,3], bitwise reproducible on a given device, using a workspace of
+ * c2m_dcn_tc_wgrad_workspace_bytes(B, C, H, W, Cout, dg) bytes (0 on bad arguments; it queries the current device). */
+typedef struct {
+    const void *gy_hi, *gy_lo;
+    const unsigned *gy_amax;
+    const void *x_il;
+    const unsigned *x_amax, *mask_amax;
+    const float *offset, *mask;
+    int B, C, H, W, Cout, dg;
+    const void *packed_w;        /* dgrad */
+    float *grad_offset, *grad_mask, *grad_input;   /* dgrad; grad_input may be NULL */
+    float *grad_weight;          /* wgrad */
+    void *ws;                    /* wgrad */
+    size_t ws_bytes;
+} c2m_dcn_tc_grad_args;
+
+size_t c2m_dcn_tc_dgrad_packed_weight_bytes(int C, int Cout, int dg);
+int c2m_dcn_tc_pack_dgrad_weights_f32(const float *w, int C, int Cout, int dg, void *packed, c2m_stream_t stream);
+int c2m_dcn_tc_dgrad(const c2m_dcn_tc_grad_args *args, c2m_stream_t stream);
+size_t c2m_dcn_tc_wgrad_workspace_bytes(int B, int C, int H, int W, int Cout, int dg);
+int c2m_dcn_tc_wgrad(const c2m_dcn_tc_grad_args *args, c2m_stream_t stream);
+
 /* --- ordered input gradients (used when torch's deterministic algorithms are enabled) -----------------------------
  * Same results as the col2im / PS-ROI grad_input scatters above, except that every element of grad_input is a sum in
  * one fixed order, so it is the same bit for bit on every run, and that grad_input is WRITTEN (every element, +0
@@ -337,8 +369,9 @@ int c2m_psroi_pooling_grad_input_det_f64(const double *out_grad, const double *b
 unsigned long long c2m_launch_count(void);
 
 /* Measurement hook (bench.py `roofline`): while enabled, the library brackets every launch of its
- * three heavy kernel classes with CUDA events on the caller's stream:
- *   0 = correlation candidate search (corr_umma / generic), 1 = conv3x3_umma, 2 = dcn_umma.
+ * heavy kernel classes with CUDA events on the caller's stream:
+ *   0 = correlation candidate search (corr_umma / generic), 1 = conv3x3_umma, 2 = dcn_umma,
+ *   3 = c2m_dcn_tc_dgrad, 4 = c2m_dcn_tc_wgrad (with its reduce).
  * c2m_profile_collect synchronises the recorded events of one class, returns their summed device
  * time, launch count and summed ALGORITHMIC flops / bytes (SURVEY.md §8d formulas), and clears them. */
 int c2m_profile_enable(int on);
