@@ -176,3 +176,10 @@ def check(rc, what):
     if rc != 0:
         msg = lib().c2m_last_error().decode(errors='replace')
         raise C2MError(f'{what} failed (status {rc}): {msg}')
+
+
+def check_size(nbytes, what):
+    """The byte count a size query returned; 0 means the query failed."""
+    if nbytes == 0:
+        raise C2MError(f'{what}: ' + lib().c2m_last_error().decode(errors='replace'))
+    return nbytes

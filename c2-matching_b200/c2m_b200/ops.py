@@ -5,7 +5,7 @@ are handed to the library."""
 import torch
 
 from . import _lib
-from ._lib import C2MError, DcnShape
+from ._lib import DcnShape
 
 _ws_cache = {}
 
@@ -71,14 +71,9 @@ def _det_workspace(query, shape, nplanes, device):
     """Workspace for an ordered gather: as many planes per pass as fit in DET_WORKSPACE_CAP, at least one.  Call with
     `device` current (the size query asks CUB, which reads the current device)."""
     global det_workspace_peak
-    L = _lib.lib()
-    one = query(shape, 1)
-    if one == 0:
-        raise C2MError('ordered input gradient: ' + L.c2m_last_error().decode(errors='replace'))
+    one = _lib.check_size(query(shape, 1), 'ordered input gradient')
     planes = max(1, min(nplanes, DET_WORKSPACE_CAP // one))
-    nbytes = query(shape, planes) if planes > 1 else one
-    if nbytes == 0:
-        raise C2MError('ordered input gradient: ' + L.c2m_last_error().decode(errors='replace'))
+    nbytes = _lib.check_size(query(shape, planes), 'ordered input gradient') if planes > 1 else one
     det_workspace_peak = max(det_workspace_peak, int(nbytes))
     return torch.empty(int(nbytes), dtype=torch.uint8, device=device)
 
@@ -116,9 +111,8 @@ def corr_argmax(feat_in, feat_ref, patch_size=3, input_stride=1, ref_stride=1, i
     hr, wr = feat_ref.shape[2:]
     L = _lib.lib()
     with torch.cuda.device(feat_in.device):
-        need = L.c2m_corr_workspace_bytes(B, C, h, w, hr, wr, patch_size, input_stride, ref_stride)
-        if need == 0:
-            raise C2MError('corr_argmax: ' + L.c2m_last_error().decode())
+        need = _lib.check_size(L.c2m_corr_workspace_bytes(B, C, h, w, hr, wr, patch_size, input_stride, ref_stride),
+                               'corr_argmax')
         ws = _workspace(need, feat_in.device)
         gh, gw = (h - patch_size) // input_stride + 1, (w - patch_size) // input_stride + 1
         idx = torch.empty(B, gh, gw, dtype=torch.int64, device=feat_in.device)
@@ -332,9 +326,9 @@ def psa_maxpool2(p):
     return out
 
 
-def conv3x3_supported(cin, cout, H=None, W=None):
+def conv3x3_supported(H, W):
     """The tensor-core kernel takes any channel counts; maps must hold one halo tile (18 x 10)."""
-    return H is None or (H >= 18 and W >= 10)
+    return H >= 18 and W >= 10
 
 
 # ---- packed-weight cache.  The blob lives ON the tensor object (so it dies with it — a global cache keyed
@@ -342,9 +336,13 @@ def conv3x3_supported(cin, cout, H=None, W=None):
 # version counter changes.  Writes through `.data` do NOT bump the version: call invalidate_packs() after
 # such an edit (load_state_dict / `with torch.no_grad(): p.copy_()` do bump it).
 _fallback_packs = {}          # id(tensor) -> (weakref, {attr: entry}) for tensors that refuse attributes
+_PACK_ATTRS = ('_c2m_pack', '_c2m_pack_dgrad', '_c2m_dcn_pack', '_c2m_dcn_pack_dgrad')
 
 
-def _pack_cached(weight, attr, extra, make):
+def _pack_cached(weight, attr, extra, size_fn, pack_fn, dims, source=None):
+    """The blob of `weight` cached under `attr` (one of _PACK_ATTRS), packed on a miss: size_fn(*dims) bytes filled by
+    pack_fn(w, *dims, blob, stream), where w is source(weight) (default: the weight itself) made contiguous.  `extra`
+    is part of the cache key."""
     import weakref
     tag = (weight.data_ptr(), weight._version, tuple(weight.shape), extra)
     store = getattr(weight, '__dict__', None)
@@ -364,7 +362,12 @@ def _pack_cached(weight, attr, extra, make):
             # an event recorded outside its capture; RestorationPipeline synchronises the device before it captures.)
             cur.wait_event(ev)
         return blob
-    blob = make()
+    L = _lib.lib()
+    w = weight.detach()
+    w = (source(w) if source else w).contiguous()
+    blob = torch.empty(getattr(L, size_fn)(*dims), dtype=torch.uint8, device=weight.device)
+    with torch.cuda.device(weight.device):
+        _lib.check(getattr(L, pack_fn)(w.data_ptr(), *dims, blob.data_ptr(), _stream()), pack_fn)
     ev = torch.cuda.Event()
     ev.record(cur)
     store[attr] = (tag, blob, ev, cur.cuda_stream)
@@ -381,10 +384,8 @@ def invalidate_packs(obj):
     for t in tensors:
         d = getattr(t, '__dict__', None)
         if d is not None:
-            d.pop('_c2m_pack', None)
-            d.pop('_c2m_pack_dgrad', None)
-            d.pop('_c2m_dcn_pack', None)
-            d.pop('_c2m_dcn_pack_dgrad', None)
+            for attr in _PACK_ATTRS:
+                d.pop(attr, None)
         _fallback_packs.pop(id(t), None)
 
 
@@ -394,18 +395,10 @@ def conv3x3_pack_weights(weight, dgrad=False):
     _require_cuda('weight', weight)
     cout, cin = weight.shape[:2]
     if dgrad:
-        cout, cin = cin, cout
-
-    def make():
-        w = weight.detach()
-        w = (w.transpose(0, 1).flip(2, 3) if dgrad else w).contiguous()
-        n = _lib.lib().c2m_conv3x3_packed_weight_bytes(cin, cout)
-        blob = torch.empty(n, dtype=torch.uint8, device=weight.device)
-        with torch.cuda.device(weight.device):
-            rc = _lib.lib().c2m_conv3x3_pack_weights_f32(w.data_ptr(), cin, cout, blob.data_ptr(), _stream())
-            _lib.check(rc, 'c2m_conv3x3_pack_weights_f32')
-        return blob
-    return _pack_cached(weight, '_c2m_pack_dgrad' if dgrad else '_c2m_pack', None, make)
+        return _pack_cached(weight, '_c2m_pack_dgrad', None, 'c2m_conv3x3_packed_weight_bytes',
+                            'c2m_conv3x3_pack_weights_f32', (cout, cin), lambda w: w.transpose(0, 1).flip(2, 3))
+    return _pack_cached(weight, '_c2m_pack', None, 'c2m_conv3x3_packed_weight_bytes', 'c2m_conv3x3_pack_weights_f32',
+                        (cin, cout))
 
 
 _ACT = {None: 0, 'none': 0, 'relu': 1, 'lrelu': 2}
@@ -477,6 +470,17 @@ def conv3x3_psa(x, weight, bias, act=None, residual=None, residual2=None, x2=Non
     return ret_psa if ret_psa is not None else ret_f32
 
 
+def _grad_psa(gy):
+    """grad_output [B,C,H,W] fp32 (any strides) as PSA at the power-of-two scale 2^sg chosen on the device, and the
+    one-element amax buffer the kernels read sg from (c2m_grad_psa_from_f32).  Call with gy's device current."""
+    B, C, H, W = gy.shape
+    gp = PSA.empty(B, C, H, W, gy.device)
+    amax = torch.empty(1, dtype=torch.int32, device=gy.device)
+    _lib.check(_lib.lib().c2m_grad_psa_from_f32(gy.data_ptr(), B, C, H, W, *gy.stride(), gp.hi.data_ptr(),
+                                                gp.lo.data_ptr(), amax.data_ptr(), _stream()), 'c2m_grad_psa_from_f32')
+    return gp, amax
+
+
 class _Conv3x3(torch.autograd.Function):
     """Forward on conv3x3_wgmma_kernel; backward: the activation's backward, dX on the same kernel with the rotated
     weights, dW on conv3x3_wgrad_kernel, db as a torch sum.  grad_output enters the kernels as PSA at a power-of-two
@@ -504,10 +508,7 @@ class _Conv3x3(torch.autograd.Function):
         dev = gy.device
         dx = dw = db = None
         with torch.cuda.device(dev):
-            gp = PSA.empty(B, cout, H, W, dev)
-            amax = torch.empty(1, dtype=torch.int32, device=dev)
-            _lib.check(L.c2m_grad_psa_from_f32(gy.data_ptr(), B, cout, H, W, *gy.stride(), gp.hi.data_ptr(),
-                                               gp.lo.data_ptr(), amax.data_ptr(), _stream()), 'c2m_grad_psa_from_f32')
+            gp, amax = _grad_psa(gy)
             if need_x:
                 dx = conv3x3_psa(gp, weight.transpose(0, 1), None, psa_out=False, out_f32=True,
                                  packed=conv3x3_pack_weights(weight, dgrad=True))
@@ -515,9 +516,8 @@ class _Conv3x3(torch.autograd.Function):
                            'c2m_grad_unscale_f32')
             if need_w:
                 dw = torch.empty(cout, cin, 3, 3, dtype=torch.float32, device=dev)
-                nbytes = L.c2m_conv3x3_wgrad_workspace_bytes(B, cin, cout, H, W)
-                if nbytes == 0:
-                    raise C2MError('c2m_conv3x3_wgrad_workspace_bytes: ' + L.c2m_last_error().decode(errors='replace'))
+                nbytes = _lib.check_size(L.c2m_conv3x3_wgrad_workspace_bytes(B, cin, cout, H, W),
+                                         'c2m_conv3x3_wgrad_workspace_bytes')
                 ws = _workspace(nbytes, dev)
                 _lib.check(L.c2m_conv3x3_wgrad(gp.hi.data_ptr(), gp.lo.data_ptr(), amax.data_ptr(), x_hi.data_ptr(),
                                                x_lo.data_ptr(), B, cin, cout, H, W, dw.data_ptr(), ws.data_ptr(),
@@ -543,7 +543,7 @@ def conv3x3(x, weight, bias=None, act=None):
                            '(expected [Cout, Cin, 3, 3])')
     if bias is not None and tuple(bias.shape) != (weight.shape[0],):
         raise RuntimeError(f'conv3x3: bias {tuple(bias.shape)} does not fit {weight.shape[0]} output channels')
-    if not conv3x3_supported(x.shape[1], weight.shape[0], x.shape[2], x.shape[3]):
+    if not conv3x3_supported(x.shape[2], x.shape[3]):
         raise RuntimeError(f'conv3x3: map {x.shape[2]}x{x.shape[3]} smaller than one halo tile (18x10)')
     return _Conv3x3.apply(x, weight, bias, act)
 
@@ -556,16 +556,8 @@ def dcn_tc_supported(C, Cout, dg, kh=3, kw=3):
 
 def _dcn_tc_pack(weight, dg):
     cout, c = weight.shape[:2]
-
-    def make():
-        n = _lib.lib().c2m_dcn_tc_packed_weight_bytes(c, cout, dg)
-        blob = torch.empty(n, dtype=torch.uint8, device=weight.device)
-        with torch.cuda.device(weight.device):
-            rc = _lib.lib().c2m_dcn_tc_pack_weights_f32(weight.detach().contiguous().data_ptr(), c, cout, dg,
-                                                        blob.data_ptr(), _stream())
-            _lib.check(rc, 'c2m_dcn_tc_pack_weights_f32')
-        return blob
-    return _pack_cached(weight, '_c2m_dcn_pack', dg, make)
+    return _pack_cached(weight, '_c2m_dcn_pack', dg, 'c2m_dcn_tc_packed_weight_bytes', 'c2m_dcn_tc_pack_weights_f32',
+                        (c, cout, dg))
 
 
 def dcn_v2_fused_tc(x, om, weight, bias, deformable_group, pre_offset=None, idx=None, pre_scale=1, ref_gw=None,
@@ -657,16 +649,8 @@ def dcn_v2_fused_tc(x, om, weight, bias, deformable_group, pre_offset=None, idx=
 
 def _dcn_tc_pack_dgrad(weight, dg):
     cout, c = weight.shape[:2]
-
-    def make():
-        n = _lib.lib().c2m_dcn_tc_dgrad_packed_weight_bytes(c, cout, dg)
-        blob = torch.empty(n, dtype=torch.uint8, device=weight.device)
-        with torch.cuda.device(weight.device):
-            rc = _lib.lib().c2m_dcn_tc_pack_dgrad_weights_f32(weight.detach().contiguous().data_ptr(), c, cout, dg,
-                                                              blob.data_ptr(), _stream())
-            _lib.check(rc, 'c2m_dcn_tc_pack_dgrad_weights_f32')
-        return blob
-    return _pack_cached(weight, '_c2m_dcn_pack_dgrad', dg, make)
+    return _pack_cached(weight, '_c2m_dcn_pack_dgrad', dg, 'c2m_dcn_tc_dgrad_packed_weight_bytes',
+                        'c2m_dcn_tc_pack_dgrad_weights_f32', (c, cout, dg))
 
 
 class _DcnV2Tc(torch.autograd.Function):
@@ -697,10 +681,7 @@ class _DcnV2Tc(torch.autograd.Function):
         dev = gy.device
         gx = goff = gmask = dw = db = None
         with torch.cuda.device(dev):
-            gp = PSA.empty(B, cout, H, W, dev)
-            gamax = torch.empty(1, dtype=torch.int32, device=dev)
-            _lib.check(L.c2m_grad_psa_from_f32(gy.data_ptr(), B, cout, H, W, *gy.stride(), gp.hi.data_ptr(),
-                                               gp.lo.data_ptr(), gamax.data_ptr(), _stream()), 'c2m_grad_psa_from_f32')
+            gp, gamax = _grad_psa(gy)
             # the forward's operand, made again: x * 2^sa and mask * 2^sm per image
             x_il = torch.empty(L.c2m_dcn_tc_operand_bytes(B, C, H, W, dg) // 2, dtype=torch.float16, device=dev)
             amax = torch.empty(2 * B, dtype=torch.int32, device=dev)
@@ -721,9 +702,8 @@ class _DcnV2Tc(torch.autograd.Function):
                 _lib.check(L.c2m_dcn_tc_dgrad(ctypes.addressof(a), _stream()), 'c2m_dcn_tc_dgrad')
             if need_w:
                 dw = torch.empty(cout, C, 3, 3, dtype=torch.float32, device=dev)
-                nbytes = L.c2m_dcn_tc_wgrad_workspace_bytes(B, C, H, W, cout, dg)
-                if nbytes == 0:
-                    raise C2MError('c2m_dcn_tc_wgrad_workspace_bytes: ' + L.c2m_last_error().decode(errors='replace'))
+                nbytes = _lib.check_size(L.c2m_dcn_tc_wgrad_workspace_bytes(B, C, H, W, cout, dg),
+                                         'c2m_dcn_tc_wgrad_workspace_bytes')
                 ws = _workspace(nbytes, dev)
                 a.grad_weight, a.ws, a.ws_bytes = dw.data_ptr(), ws.data_ptr(), nbytes
                 _lib.check(L.c2m_dcn_tc_wgrad(ctypes.addressof(a), _stream()), 'c2m_dcn_tc_wgrad')

@@ -70,10 +70,8 @@ __global__ void grad_unscale_kernel(float *__restrict__ x, long long n, const un
         x[i] = ldexpf(x[i], s);
 }
 
-__host__ __device__ inline size_t wgrad_slot(const WgradGeom &p) { return (size_t)p.nslice * WG_CO * p.nchunk * WG_CI * 9; }
-
 // Consumer warpgroup of conv3x3_wgrad_kernel: taps [T0, T0 + NT) of every K step of tiles [t0, t1), then the 64 x 32 x NT
-// partial into the CTA's workspace slot `dst` ([co_pad][ci_pad][9] fp32).
+// partial into the CTA's workspace slot `dst` ([co_pad][tap][ci_pad] fp32, see wgrad_flush).
 template <int T0, int NT>
 __device__ __forceinline__ void wgrad_consume(uint8_t *smem, uint64_t *full, uint64_t *empty, long long t0, long long t1,
                                               const WgradGeom &p, int slice, int chunk, float *dst) {
@@ -82,26 +80,9 @@ __device__ __forceinline__ void wgrad_consume(uint8_t *smem, uint64_t *full, uin
     for (int t = 0; t < NT; ++t)
 #pragma unroll
         for (int i = 0; i < 16; ++i) acc[t][i] = 0.f;
-    // accumulator register i of thread (warp w, lane l): row (cout) 16 w + l / 4 + 8 ((i / 2) % 2),
-    // column (cin) 8 (i / 4) + 2 (l % 4) + i % 2
-    const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
-    const int ci_pad = p.nchunk * WG_CI;
-    float *out = dst + ((size_t)(slice * WG_CO + 16 * w + (l >> 2)) * ci_pad + chunk * WG_CI + 2 * (l & 3)) * 9 + T0;
-    // The tensor cores' fp32 accumulation error grows with the number of MMAs into one accumulator (linearly, not as
-    // a random walk): every WG_FLUSH tiles the accumulator is added into the slot with fp32 adds and restarted.
+    const int ci_pad = p.nchunk * WG_CI, ncol = 9 * ci_pad;
+    float *blk = dst + (size_t)slice * WG_CO * ncol + T0 * ci_pad + chunk * WG_CI;
     bool first = true;
-    auto flush = [&]() {
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-            float *o = out + ((size_t)(8 * ((i >> 1) & 1)) * ci_pad + 8 * (i >> 2) + (i & 1)) * 9;
-#pragma unroll
-            for (int tt = 0; tt < NT; ++tt) {
-                o[tt] = first ? acc[tt][i] : o[tt] + acc[tt][i];
-                acc[tt][i] = 0.f;
-            }
-        }
-        first = false;
-    };
     int stage = 0, phase = 0, n = 0;
     for (long long t = t0; t < t1; ++t) {
         mbar_wait(&full[stage], phase);
@@ -128,9 +109,9 @@ __device__ __forceinline__ void wgrad_consume(uint8_t *smem, uint64_t *full, uin
         wgmma_wait_all();
         mbar_arrive(&empty[stage]);
         if (++stage == WG_NST) { stage = 0; phase ^= 1; }
-        if (++n == WG_FLUSH) { flush(); n = 0; }
+        if (++n == WG_FLUSH) { wgrad_flush<false>(acc, blk, ncol, ci_pad, first, 0); first = false; n = 0; }
     }
-    if (n || first) flush();
+    if (n || first) wgrad_flush<false>(acc, blk, ncol, ci_pad, first, 0);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -193,30 +174,28 @@ conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tg_hi, const __grid_con
         asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
         // warpgroup 1 takes taps 0..4, warpgroup 2 taps 5..8 (80 / 64 accumulator registers: the kernel's register
         // budget of 168 per thread does not hold all nine 64 x 32 tiles in one warpgroup)
-        if (warp < 8) wgrad_consume<0, 5>(smem, full, empty, t0, t1, p, slice, chunk, ws + (size_t)k * wgrad_slot(p));
-        else wgrad_consume<5, 4>(smem, full, empty, t0, t1, p, slice, chunk, ws + (size_t)k * wgrad_slot(p));
+        float *slot = ws + (size_t)k * p.nslice * WG_CO * 9 * p.nchunk * WG_CI;
+        if (warp < 8) wgrad_consume<0, 5>(smem, full, empty, t0, t1, p, slice, chunk, slot);
+        else wgrad_consume<5, 4>(smem, full, empty, t0, t1, p, slice, chunk, slot);
     }
 }
 
-// dW[co][ci][tap] = 2^-sg * (slot 0 + slot 1 + ... ), always in that order
-__global__ void wgrad_reduce_kernel(const float *__restrict__ ws, int nslots, int Cin, int Cout, int ci_pad, int co_pad,
-                                    const unsigned *__restrict__ amax, float *__restrict__ dw) {
-    const int s = -grad_scale_exp(amax);
-    const long long n = (long long)Cout * Cin * 9;
-    const size_t slot = (size_t)co_pad * ci_pad * 9;
+__global__ void wgrad_reduce_kernel(const float *__restrict__ ws, int nslots, int C, int Cout, int cpg, int co_pad,
+                                    int ncol, const unsigned *__restrict__ gy_amax, float *__restrict__ dw) {
+    const int s = -grad_scale_exp(gy_amax);
+    const long long n = (long long)Cout * ncol;
+    const size_t slot = (size_t)co_pad * ncol;
     for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x) {
-        const int tap = (int)(e % 9);
-        const int ci = (int)((e / 9) % Cin), co = (int)(e / (9LL * Cin));
-        const float *src = ws + ((size_t)co * ci_pad + ci) * 9 + tap;
+        const int co = (int)(e / ncol), col = (int)(e % ncol);
+        const int pair = col / cpg, c = (pair / 9) * cpg + col % cpg;     // pair = (group, tap)
+        if (c >= C) continue;                                             // padding column
         float v = 0.f;
-        for (int j = 0; j < nslots; ++j) v += src[j * slot];
-        dw[e] = ldexpf(v, s);
+        for (int j = 0; j < nslots; ++j) v += ws[e + j * slot];
+        dw[((size_t)co * C + c) * 9 + pair % 9] = ldexpf(v, s);
     }
 }
 
 static int wgrad_geom(int B, int Cin, int Cout, int H, int W, WgradGeom &g) {
-    int sms = 0;
-    C2M_CUDA(sm_count(sms));
     g.B = B; g.H = H; g.W = W; g.Cin = Cin; g.Cout = Cout;
     g.C8i = (Cin + 7) / 8; g.C8o = (Cout + 7) / 8;
     g.nslice = ceil_div(Cout, WG_CO);
@@ -224,15 +203,7 @@ static int wgrad_geom(int B, int Cin, int Cout, int H, int W, WgradGeom &g) {
     g.tiles_x = ceil_div(W, G_C);
     g.tiles_y = ceil_div(H, G_R);
     g.ntiles = (long long)B * g.tiles_x * g.tiles_y;
-    // one wave: the (slice, chunk) pairs share the SMs, each K range gets at least one tile
-    const int pairs = g.nslice * g.nchunk;
-    long long ks = sms / pairs > 0 ? sms / pairs : 1;
-    g.ksplit = (int)(ks < g.ntiles ? ks : g.ntiles);
-    return C2M_OK;
-}
-
-static size_t wgrad_ws_bytes(const WgradGeom &g) {
-    return (size_t)g.ksplit * wgrad_slot(g) * sizeof(float);
+    return wgrad_ksplit(g.nslice * g.nchunk, g.ntiles, g.ksplit);
 }
 
 }  // namespace c2m
@@ -272,7 +243,7 @@ extern "C" size_t c2m_conv3x3_wgrad_workspace_bytes(int B, int Cin, int Cout, in
     }
     WgradGeom g;
     if (wgrad_geom(B, Cin, Cout, H, W, g)) return 0;
-    return wgrad_ws_bytes(g);
+    return wgrad_ws_bytes(g.ksplit, g.nslice * WG_CO, 9 * g.nchunk * WG_CI);
 }
 
 extern "C" int c2m_conv3x3_wgrad(const void *gy_hi, const void *gy_lo, const unsigned *gy_amax, const void *x_hi,
@@ -283,7 +254,8 @@ extern "C" int c2m_conv3x3_wgrad(const void *gy_hi, const void *gy_lo, const uns
     C2M_CHECK_ARG(H >= X_R && W >= X_C, "conv3x3_wgrad: map %dx%d smaller than one halo tile (18x10)", H, W);
     WgradGeom g;
     if (const int rc = wgrad_geom(B, Cin, Cout, H, W, g)) return rc;
-    const size_t need = wgrad_ws_bytes(g);
+    const int co_pad = g.nslice * WG_CO, ci_pad = g.nchunk * WG_CI;
+    const size_t need = wgrad_ws_bytes(g.ksplit, co_pad, 9 * ci_pad);
     if (!ws || ws_bytes < need) {
         set_error("conv3x3_wgrad: workspace of %zu bytes, %zu needed", ws_bytes, need);
         return C2M_ERR_WORKSPACE;
@@ -300,9 +272,8 @@ extern "C" int c2m_conv3x3_wgrad(const void *gy_hi, const void *gy_lo, const uns
     float *part = reinterpret_cast<float *>(ws);
     conv3x3_wgrad_kernel<<<grid, 384, WG_SMEM, st>>>(mgh, mgl, mxh, mxl, g, part);
     C2M_LAUNCH_CHECK("conv3x3_wgrad_kernel");
-    const long long n = (long long)Cout * Cin * 9;
-    wgrad_reduce_kernel<<<grid_blocks(n), 256, 0, st>>>(part, g.ksplit, Cin, Cout, g.nchunk * WG_CI,
-                                                        g.nslice * WG_CO, gy_amax, dw);
+    wgrad_reduce_kernel<<<grid_blocks((long long)Cout * 9 * ci_pad), 256, 0, st>>>(part, g.ksplit, Cin, Cout, ci_pad,
+                                                                                co_pad, 9 * ci_pad, gy_amax, dw);
     C2M_LAUNCH_CHECK("wgrad_reduce_kernel");
     return C2M_OK;
 }

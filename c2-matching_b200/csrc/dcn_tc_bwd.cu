@@ -18,7 +18,8 @@
 // warps build mask * bilinear(x) for a tile in the forward's [octet][px][8] layout, which is an MN-major operand along
 // K = pixels; gY is the MN-major operand of the same tile by TMA (as in conv3x3_wgrad.cu).  The accumulator is added
 // into the CTA's fp32 workspace slot every WG_FLUSH tiles and whenever the image changes, divided by that image's
-// operand scale 2^(sa_b + sm_b); dcn_wgrad_reduce_kernel sums the slots in one fixed order and divides 2^sg out.
+// operand scale 2^(sa_b + sm_b); wgrad_reduce_kernel sums the slots in one fixed order and divides 2^sg out
+// (umma_conv_common.cuh).
 #include "dcn_sampling.cuh"
 #include "umma_conv_common.cuh"
 
@@ -335,23 +336,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) dcn_wgrad_kernel(const __grid_con
         for (int h = 0; h < NH; ++h)
 #pragma unroll
             for (int i = 0; i < 16; ++i) acc[h][i] = 0.f;
-        // accumulator register i of thread (warp w, lane l): row (cout) 16 w + l / 4 + 8 ((i / 2) % 2),
-        // column 8 (i / 4) + 2 (l % 4) + i % 2
-        const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
         const int ncol = d.nkc * 32;
-        float *out = d.ws + (size_t)kr * ((size_t)d.ncs * WG_NCO * ncol) +
-                     (size_t)(cs * WG_NCO + 16 * w + (l >> 2)) * ncol + kc * 32 + 2 * (l & 3);
+        float *blk = d.ws + ((size_t)kr * d.ncs * WG_NCO + cs * WG_NCO) * ncol + kc * 32;
         bool first = true;
         auto flush = [&](int b) {
-            const int sc = -(operand_exp(d.x_amax, b) + mask_exp(d.mask_amax, b));
-#pragma unroll
-            for (int h = 0; h < NH; ++h)
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    float *o = out + (size_t)(h * 64 + 8 * ((i >> 1) & 1)) * ncol + 8 * (i >> 2) + (i & 1);
-                    *o = first ? ldexpf(acc[h][i], sc) : *o + ldexpf(acc[h][i], sc);
-                    acc[h][i] = 0.f;
-                }
+            wgrad_flush<true>(acc, blk, ncol, 64 * ncol, first,
+                        -(operand_exp(d.x_amax, b) + mask_exp(d.mask_amax, b)));
             first = false;
         };
         int ys = 0, yph = 0, gs = 0, gph = 0, n = 0, cur_b = -1;
@@ -440,23 +430,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) dcn_wgrad_kernel(const __grid_con
     }
 }
 
-// dW[co][c][tap] = 2^-sg * (slot 0 + slot 1 + ...), always in that order; column of (c, tap) = K4's K index
-__global__ void dcn_wgrad_reduce_kernel(const float *__restrict__ ws, int nslots, int C, int Cout, int cpg, int co_pad,
-                                        int ncol, const unsigned *__restrict__ gy_amax, float *__restrict__ dw) {
-    const int s = -grad_scale_exp(gy_amax);
-    const long long n = (long long)Cout * C * 9;
-    const size_t slot = (size_t)co_pad * ncol;
-    for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x) {
-        const int tap = (int)(e % 9);
-        const int c = (int)((e / 9) % C), co = (int)(e / (9LL * C));
-        const int col = ((c / cpg) * 9 + tap) * cpg + c % cpg;
-        const float *src = ws + (size_t)co * ncol + col;
-        float v = 0.f;
-        for (int j = 0; j < nslots; ++j) v += src[j * slot];
-        dw[e] = ldexpf(v, s);
-    }
-}
-
 // ---- host side
 // columns per dgrad chunk: whole (g, tap) pairs when a pair has at most 64 columns (the last chunk is then partial
 // unless the pair count divides evenly), else the largest wgmma width dividing the pair, so that no chunk holds parts
@@ -488,17 +461,6 @@ static int grad_geom(int B, int C, int H, int W, int Cout, int dg, DcnGrad &d) {
     s.dh = s.dw = 1; s.dg = dg;
     return C2M_OK;
 }
-
-static int wgrad_split(DcnGrad &d) {
-    int sms = 0;
-    C2M_CUDA(sm_count(sms));
-    const int pairs = d.nkc * d.ncs;
-    const long long ks = sms / pairs > 0 ? sms / pairs : 1;
-    d.ksplit = (int)(ks < d.ntiles ? ks : d.ntiles);
-    return C2M_OK;
-}
-
-static size_t wgrad_ws(const DcnGrad &d) { return (size_t)d.ksplit * d.ncs * WG_NCO * d.nkc * 32 * sizeof(float); }
 
 // shape and operand checks shared by both entry points
 static int check_grad_args(const c2m_dcn_tc_grad_args *a, const char *who) {
@@ -596,8 +558,8 @@ extern "C" size_t c2m_dcn_tc_wgrad_workspace_bytes(int B, int C, int H, int W, i
     }
     DcnGrad d;
     grad_geom(B, C, H, W, Cout, dg, d);
-    if (wgrad_split(d)) return 0;
-    return wgrad_ws(d);
+    if (wgrad_ksplit(d.nkc * d.ncs, d.ntiles, d.ksplit)) return 0;
+    return wgrad_ws_bytes(d.ksplit, d.ncs * WG_NCO, d.nkc * 32);
 }
 
 extern "C" int c2m_dcn_tc_wgrad(const c2m_dcn_tc_grad_args *a, c2m_stream_t stream) {
@@ -605,8 +567,8 @@ extern "C" int c2m_dcn_tc_wgrad(const c2m_dcn_tc_grad_args *a, c2m_stream_t stre
     C2M_CHECK_ARG(a->grad_weight, "dcn_tc_wgrad: null pointer");
     DcnGrad d;
     grad_geom(a->B, a->C, a->H, a->W, a->Cout, a->dg, d);
-    if (const int rc = wgrad_split(d)) return rc;
-    const size_t need = wgrad_ws(d);
+    if (const int rc = wgrad_ksplit(d.nkc * d.ncs, d.ntiles, d.ksplit)) return rc;
+    const size_t need = wgrad_ws_bytes(d.ksplit, d.ncs * WG_NCO, d.nkc * 32);
     if (!a->ws || a->ws_bytes < need) {
         set_error("dcn_tc_wgrad: workspace of %zu bytes, %zu needed", a->ws_bytes, need);
         return C2M_ERR_WORKSPACE;
@@ -634,10 +596,9 @@ extern "C" int c2m_dcn_tc_wgrad(const c2m_dcn_tc_grad_args *a, c2m_stream_t stre
         dcn_wgrad_kernel<2><<<grid, NTHREADS, smem, st>>>(mh, ml, d);
     }
     C2M_LAUNCH_CHECK("dcn_wgrad_kernel");
-    const long long n = (long long)a->Cout * a->C * 9;
-    dcn_wgrad_reduce_kernel<<<grid_blocks(n), 256, 0, st>>>(d.ws, d.ksplit, a->C, a->Cout, d.cpg, d.ncs * WG_NCO,
-                                                            d.nkc * 32, a->gy_amax, a->grad_weight);
-    C2M_LAUNCH_CHECK("dcn_wgrad_reduce_kernel");
+    wgrad_reduce_kernel<<<grid_blocks((long long)a->Cout * d.nkc * 32), 256, 0, st>>>(
+        d.ws, d.ksplit, a->C, a->Cout, d.cpg, d.ncs * WG_NCO, d.nkc * 32, a->gy_amax, a->grad_weight);
+    C2M_LAUNCH_CHECK("wgrad_reduce_kernel");
     prof_end(ph, st);
     return C2M_OK;
 }

@@ -40,6 +40,52 @@ __host__ __device__ __forceinline__ int grad_scale_exp(const unsigned *amax) {
     return s < -120 ? -120 : s > 120 ? 120 : s;
 }
 
+// ---- Split-K weight gradients (conv3x3_wgrad.cu, dcn_tc_bwd.cu).  dW is a GEMM with M = Cout and K = every pixel of
+// the batch.  The pixel tiles are cut into ksplit contiguous K ranges; the CTAs of range k write their fp32 partials
+// to workspace slot k, [co_pad][ncol] with column ((c / cpg) * 9 + tap) * cpg + c % cpg holding (channel c, tap): the
+// tensor-core DCN's K order, cpg channels per deformable group.  The plain convolution is one group of cpg = ci_pad
+// channels, i.e. [co][tap][ci_pad].  wgrad_reduce_kernel sums the slots in one fixed order, so dW is the same bit for
+// bit on every run on a given device.
+
+// K ranges of a launch with `ctas` CTAs per range: one wave (the ranges share the SMs), at least one tile per range.
+inline int wgrad_ksplit(int ctas, long long ntiles, int &ksplit) {
+    int sms = 0;
+    C2M_CUDA(sm_count(sms));
+    const long long ks = sms / ctas > 0 ? sms / ctas : 1;
+    ksplit = (int)(ks < ntiles ? ks : ntiles);
+    return C2M_OK;
+}
+
+inline size_t wgrad_ws_bytes(int ksplit, int co_pad, int ncol) { return (size_t)ksplit * co_pad * ncol * sizeof(float); }
+
+// Adds the calling warpgroup's NA m64n32 fp32 wgmma accumulators into a slot and restarts them (`first` stores instead
+// of adding); SCALED multiplies them by 2^e first.  Accumulator a covers rows [0, 64) x columns [0, 32) from
+// blk + a * stride, row pitch ncol.  Register i of thread (warp w, lane l) holds row 16 w + l / 4 + 8 ((i / 2) % 2),
+// column 8 (i / 4) + 2 (l % 4) + i % 2.  The kernels flush every few tiles because the tensor cores' fp32 accumulation
+// error grows with the number of MMAs into one accumulator (linearly, not as a random walk); the slot adds are fp32.
+template <bool SCALED, int NA>
+__device__ __forceinline__ void wgrad_flush(float (&acc)[NA][16], float *blk, int ncol, int stride, bool first,
+                                            int e) {
+    const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+    float *out = blk + (16 * w + (l >> 2)) * ncol + 2 * (l & 3);
+#pragma unroll
+    for (int a = 0; a < NA; ++a) {
+        float *o0 = out + a * stride, *o1 = o0 + 8 * ncol;
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+            const float v = SCALED ? ldexpf(acc[a][i], e) : acc[a][i];
+            float &d = ((i >> 1) & 1 ? o1 : o0)[8 * (i >> 2) + (i & 1)];
+            d = first ? v : d + v;
+            acc[a][i] = 0.f;
+        }
+    }
+}
+
+// dW [Cout][C][3][3] = 2^-sg * (slot 0 + slot 1 + ...), always in that order; one thread per slot column, so the reads
+// are coalesced (conv3x3_wgrad.cu; grid-stride over Cout * ncol)
+__global__ void wgrad_reduce_kernel(const float *__restrict__ ws, int nslots, int C, int Cout, int cpg, int co_pad,
+                                    int ncol, const unsigned *__restrict__ gy_amax, float *__restrict__ dw);
+
 // Per-image operand exponents of the tensor-core DCN kernels' fp32 boundary (dcn_umma.cu, dcn_tc_bwd.cu), from the bits of the image's largest finite magnitude (0 -> 0).
 // x: amax * 2^s in [2^11, 2^12), under fp16's 65504 with 16x headroom for the blend and well above its subnormals.
 // mask: max |mask| * 2^s in [1, 2), so the corner weights are at most 2.  Exponent arithmetic only: scaling an image

@@ -60,7 +60,8 @@ def psa_path_ok(x, *convs, cat_first=32):
     the FIRST input of the two-input (concatenating) convolutions on the path — the kernel needs a multiple of 32 there."""
     if not (fast_conv_enabled() and x.is_cuda and x.dtype == torch.float32 and not torch.is_grad_enabled()):
         return False
-    if x.shape[2] < 18 or x.shape[3] < 10:
+    from c2m_b200 import ops
+    if not ops.conv3x3_supported(x.shape[2], x.shape[3]):
         # not silent: the tensor-core kernel needs one 18x10 halo tile; smaller maps run the plain modules (cuDNN, exact fp32)
         global _warned_small
         if not _warned_small:
@@ -86,9 +87,10 @@ class Conv2d(nn.Conv2d):
 
     def forward(self, x):
         if (torch.is_grad_enabled() and fast_conv_enabled() and _tc_conv(self) and self.padding_mode == 'zeros' and
-                x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and x.shape[2] >= 18 and x.shape[3] >= 10):
+                x.is_cuda and x.dtype == torch.float32 and x.dim() == 4):
             from c2m_b200 import ops
-            return ops.conv3x3(x, self.weight, self.bias)
+            if ops.conv3x3_supported(x.shape[2], x.shape[3]):
+                return ops.conv3x3(x, self.weight, self.bias)
         return super().forward(x)
 
 
