@@ -21,10 +21,11 @@
 //   Pre-offsets: per tile the index-map cells it can touch ((16/s + 2) x (8/s + 2)) are decoded once into a
 //   shared-memory flow table, so the per-(pixel, tap) pre-offset is one ld.shared instead of an 8-byte global
 //   load, two integer divisions and a modulo per (pixel, g, tap).
-//   Weights stream as 8 KB chunks (bulk copy ring).  One launch computes one 64-wide slice of the output channels
+//   Weights stream as 8 KB chunks (bulk copy ring).  A CTA computes one 64-wide slice of the output channels
 //   (the fp32 accumulator of a 128 x 64 tile is what one warpgroup holds in registers next to the gather warps);
-//   wider layers take one launch per slice.  The epilogue (bias, LeakyReLU, PSA and / or fp32 store) is shared
-//   with the plain convolution.
+//   wider layers run their S slices on the S CTAs of a thread-block cluster, which gather each stage once between
+//   them and hand it on through distributed shared memory.  The epilogue (bias, LeakyReLU, PSA and / or fp32 store)
+//   is shared with the plain convolution.
 // The im2col matrix never exists outside shared memory.
 #include "umma_conv_common.cuh"
 
@@ -60,7 +61,7 @@ struct DcnTc {
     int opp_shift;             // log2(opp) when opp is a power of two, else -1 (then L == 1)
     int nstage, nbst;          // ring depths (activation stages, weight chunks); powers of two
     int nstage_shift;          // log2(nstage)
-    int slice;                 // 64-wide output-channel slice this launch computes
+    int slice;                 // 64-wide output-channel slice this launch computes (0 under a cluster launch)
     int sc_shift;              // log2(pre_scale) when the flow table is used (idx given, scale in {1,2,4,8}), else -1
     int tab_h, tab_w;          // flow-table cells per tile: 16/s + 2, 8/s + 2
     float inv_ref_gw, inv_scale;   // reciprocals for the exact float-assisted integer divisions
@@ -111,7 +112,36 @@ __device__ __forceinline__ float ldg_stream_f1(const float *ptr, uint64_t pol) {
     return v;
 }
 
-template <int N>
+// ---- thread-block cluster helpers (CL = true kernels)
+__device__ __forceinline__ uint32_t cluster_reg(int which) {
+    uint32_t v;
+    if (which == 0) asm("mov.u32 %0, %%cluster_ctarank;" : "=r"(v));
+    else if (which == 1) asm("mov.u32 %0, %%cluster_nctarank;" : "=r"(v));
+    else if (which == 2) asm("mov.u32 %0, %%clusterid.x;" : "=r"(v));
+    else asm("mov.u32 %0, %%nclusterid.x;" : "=r"(v));
+    return v;
+}
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// shared::cluster address of the same shared-memory object in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t peer_addr(const void *p, int rank) {
+    uint32_t a;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(a) : "r"(smem_u32(p)), "r"(rank));
+    return a;
+}
+__device__ __forceinline__ void mbar_arrive_peer(uint32_t bar) {
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive_expect_tx_peer(uint32_t bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.release.cluster.shared::cluster.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes)
+                 : "memory");
+}
+
+// CL = false: one launch per 64-wide output-channel slice (d.slice).  CL = true: a cluster of S = nslice CTAs works on
+// the same tile sequence, CTA rank r computes slice r, and each gathered stage is built by one CTA and copied into the
+// other S - 1 (see the gather-distributor comment below).
+template <int N, bool CL>
 __global__ void __launch_bounds__(NTHREADS, 1)
 dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -133,14 +163,31 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
     // registers); item i runs on CTA i % grid, so at any moment the CTAs work on ~grid CONSECUTIVE tiles and the
     // gathered input map of ONE image is what has to stay in L2, not the whole batch.
     const int n_items = p.B * tiles_img;
-    const int nstage_mask = d.nstage - 1;                // ring depths are powers of two
+    const int nstage_mask = d.nstage - 1;                // ring depths are powers of two (CL: a multiple of S)
+    // Clusters: cluster k takes items k, k + nclusters, ... (all its CTAs the same ones), and ring slot i's stages are
+    // gathered by CTA i % S, which S | nstage keeps fixed for the whole kernel.
+    int rank = 0, S = 1;
+    if constexpr (CL) { rank = (int)cluster_reg(0); S = (int)cluster_reg(1); }
+    const auto item0 = [&] { return CL ? (int)cluster_reg(2) : (int)blockIdx.x; };
+    const auto istep = [&] { return CL ? (int)cluster_reg(3) : (int)gridDim.x; };
+    const auto slice = [&] { return CL ? rank : d.slice; };
 
     if (warp == 1 && lane == 0) {
-        for (int i = 0; i < d.nstage; ++i) { mbar_init(&full[i], NGATHER_WARPS >> d.lshift); mbar_init(&empty[i], 128); }
+        for (int i = 0; i < d.nstage; ++i) {
+            if (!CL || i % S == rank) {
+                mbar_init(&full[i], NGATHER_WARPS >> d.lshift);
+                // CL: + 1 elected arrive per MMA warp of each peer, + the distributor once its copies have been read
+                mbar_init(&empty[i], CL ? 128 + 4 * (S - 1) + 1 : 128);
+            } else {
+                mbar_init(&full[i], 1);              // the owner's remote arrive.expect_tx, completed by its bulk copy
+                mbar_init(&empty[i], 128);           // arrived on locally, never waited on: the owner's empty[i] gates
+            }
+        }
         for (int i = 0; i < d.nbst; ++i) { mbar_init(&bfull[i], 1); mbar_init(&bempty[i], 128); }
         fence_mbar_init();
     }
-    __syncthreads();
+    if constexpr (CL) cluster_sync();       // peers' barriers are initialised before any remote arrive or copy
+    else __syncthreads();
     const int sw = *reinterpret_cast<const int *>(q.wblob);
 
     // Register budget per warpgroup.  The CTA's pool is what it was launched with (80 x 768 = 61440):
@@ -152,16 +199,44 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
         // ================================ weight producer ===================================
         if (lane == 0) {
             int bst = 0, bphase = 0;
-            for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+            for (int item = item0(); item < n_items; item += istep()) {
                 for (int kc = 0; kc < p.nkc; ++kc) {
                     mbar_wait(&bempty[bst], bphase ^ 1);
                     mbar_arrive_expect_tx(&bfull[bst], w_chunk);
-                    const uint8_t *src = q.wblob + W_HDR + ((size_t)d.slice * p.nkc + kc) * w_chunk;
+                    const uint8_t *src = q.wblob + W_HDR + ((size_t)slice() * p.nkc + kc) * w_chunk;
                     asm volatile(
                         "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                         ::"r"(smem_u32(sW + bst * w_chunk)), "l"(src), "r"(w_chunk), "r"(smem_u32(&bfull[bst]))
                         : "memory");
                     if (++bst == d.nbst) { bst = 0; bphase ^= 1; }
+                }
+            }
+        }
+    } else if (CL && warp == 1) {
+        // ================================ gather distributor (CL) ===========================
+        // For each stage this CTA gathered: once its gather warps have completed full[rs], arm every peer's full[rs]
+        // for A_STAGE bytes and bulk-copy the slot into the same slot of that peer.  The local empty[rs] gets this
+        // thread's arrive only when the copies have finished reading the slot; the peers' MMA warps arrive on it
+        // when they have consumed their copy, so the gather warps overwrite the slot only when no CTA still needs it.
+        if (lane == 0) {
+            int ring = 0;
+            for (int item = item0(); item < n_items; item += istep(), ring += p.nkc) {
+                for (int kc = (rank - ring % S + S) % S; kc < p.nkc; kc += S) {
+                    const int stage_idx = ring + kc;
+                    const int rs = stage_idx % d.nstage;
+                    mbar_wait(&full[rs], (uint32_t)(stage_idx / d.nstage) & 1u);
+                    const uint32_t src = smem_u32(sA + rs * A_STAGE);
+                    for (int j = 1; j < S; ++j) {
+                        const int peer = (rank + j) % S;
+                        const uint32_t pbar = peer_addr(&full[rs], peer);
+                        mbar_arrive_expect_tx_peer(pbar, A_STAGE);
+                        asm volatile(
+                            "cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                            ::"r"(peer_addr(sA + rs * A_STAGE, peer)), "r"(src), "r"(A_STAGE), "r"(pbar)
+                            : "memory");
+                    }
+                    asm volatile("cp.async.bulk.commit_group;\n\tcp.async.bulk.wait_group.read 0;" ::: "memory");
+                    mbar_arrive(&empty[rs]);
                 }
             }
         }
@@ -175,12 +250,12 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
         const float res_scale = 1.f;
         const float so = ldexpf(1.f, p.sa_out);
         const bool fast = epilogue_fast_ok(q, p) && p.sa_out == 0;     // (this kernel does not pre-scale bias / factors)
-        const int o_base = d.slice * N;
+        const int o_base = slice() * N;
         for (int i = e; i < N; i += 128) sbias[i] = (q.bias && o_base + i < p.Cout) ? q.bias[o_base + i] : 0.f;
         asm volatile("bar.sync 1, 128;" ::: "memory");
         constexpr uint32_t b_lbo = N * 16;
         int stage = 0, phase = 0, bst = 0, bphase = 0;
-        for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+        for (int item = item0(); item < n_items; item += istep()) {
             const int b = item / tiles_img, tt = item - b * tiles_img;
             const int y = (tt / p.tiles_x) * T_R + e / T_C, x = (tt % p.tiles_x) * T_C + e % T_C;
             const bool ok = y < p.H && x < p.W;
@@ -209,6 +284,9 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
                 wgmma_commit();
                 wgmma_wait_all();
                 mbar_arrive(&empty[stage]);
+                // CL: a stage another CTA gathered is released on that CTA's empty barrier, once per warp (the
+                // warp's wgmma reads of it are complete after its wait above)
+                if (CL && lane == 0 && stage % S != rank) mbar_arrive_peer(peer_addr(&empty[stage], stage % S));
                 mbar_arrive(&bempty[bst]);
                 if (++stage == d.nstage) { stage = 0; phase ^= 1; }
                 if (++bst == d.nbst) { bst = 0; bphase ^= 1; }
@@ -250,7 +328,7 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
         struct Meta { float off_h, off_w, mr; };
         int ring = 0;                                       // stages issued by this CTA so far (all groups agree)
         int gi = 0;                                         // item counter (double buffer of tile info and table)
-        for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++gi) {
+        for (int item = item0(); item < n_items; item += istep(), ++gi) {
             int4 *tinfo = tile_info + (gi & 1);
             float2 *tab = flow_tab + (gi & 1) * tab_n;
 
@@ -349,12 +427,15 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
                 }
             };
 
-            // my K chunks of this item: sg, sg + NG, ...
+            // my K chunks of this item: sg, sg + NG, ...  CL: the chunks whose ring slot this CTA owns, the j-th of
+            // them for j = sg, sg + NG, ...
+            const int kfirst = CL ? (rank - ring % S + S) % S + sg * S : sg;
+            const int kstep = CL ? NG * S : NG;
             Meta mt, nx;
             int y, ny, xx, nxx, b, nb;
             bool lv, nlv;
-            fetch(sg, sg < p.nkc, mt, y, xx, b, lv);
-            for (int kc = sg; kc < p.nkc; kc += NG) {
+            fetch(kfirst, kfirst < p.nkc, mt, y, xx, b, lv);
+            for (int kc = kfirst; kc < p.nkc; kc += kstep) {
                 // ---- sampling point of the unit's (pixel, g, tap): dcn_v2_im2col_cuda.cu:25-54,172-190
                 const int xoff = lv ? c_xoff : 0;           // belongs to kc (set_kc(kc) ran in this unit's fetch)
                 // A corner the sample does not read (outside the image, or the sample outside the window) points at
@@ -387,11 +468,11 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
                 const __half2 wh0 = __float2half2_rn(w0), wh1 = __float2half2_rn(w1), wh2 = __float2half2_rn(w2),
                               wh3 = __float2half2_rn(w3);
                 const int stage_idx = ring + kc;
-                const int rs = stage_idx & nstage_mask;
-                const uint32_t rphase = (uint32_t)(stage_idx >> d.nstage_shift) & 1u;
+                const int rs = CL ? stage_idx % d.nstage : stage_idx & nstage_mask;
+                const uint32_t rphase = (uint32_t)(CL ? stage_idx / d.nstage : stage_idx >> d.nstage_shift) & 1u;
                 uint8_t *sdst = sA + rs * A_STAGE + (slot * L) * A_OCT_B + m * 16;
                 // next unit's metadata goes out before this unit's corner fetches come back
-                fetch(kc + NG, kc + NG < p.nkc, nx, ny, nxx, nb, nlv);
+                fetch(kc + kstep, kc + kstep < p.nkc, nx, ny, nxx, nb, nlv);
 #pragma unroll 1
                 for (int u = 0; u < L; ++u) {
                     // octet-planar operand: the 32 lanes of a warp (4 rows x 8 pixels) read 16 B each from runs of
@@ -440,7 +521,8 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
             ring += p.nkc;
         }
     }
-
+    // CL: no CTA exits while a peer can still copy into its shared memory or arrive on its barriers
+    if constexpr (CL) cluster_sync();
 }
 
 // blob: header | [slice][kc][hi|lo][octet 4][N][8], K ordered (g, tap, channel-in-group)
@@ -684,19 +766,29 @@ extern "C" int c2m_dcn_v2_fused_tc(const c2m_dcn_tc_args *a, c2m_stream_t stream
                   "dcn_v2_fused_tc: map too large for 32-bit in-kernel indexing");
     C2M_CHECK_ARG(a->idx == nullptr || (long long)a->gh * a->gw < (1 << 23), "dcn_v2_fused_tc: index map too large");
     C2M_CHECK_ARG((long long)a->B * a->H * a->W * a->C < (1ll << 31), "dcn_v2_fused_tc: batch too large for 32-bit in-kernel indexing");
-    // ring depths (powers of two): with L octets per thread, L stage groups fill consecutive stages concurrently
+    // ring depths (powers of two): with L octets per thread, L stage groups fill consecutive stages concurrently.
+    // Clusters of S = nslice CTAs: ring slot i belongs to CTA i % S, so the ring is a multiple of S deep (8, or 6 for
+    // S = 3), and each CTA gathers into nstage / S of its slots at a time.
+    const int S = p.nslice;
     const size_t w_chunk = (size_t)2 * KOCT * p.N * 16;
-    d.nstage = d.L == 1 ? 4 : 8;
-    d.nstage_shift = d.L == 1 ? 2 : 3;
+    d.nstage = S > 1 ? (S == 3 ? 6 : 8) : d.L == 1 ? 4 : 8;
+    d.nstage_shift = d.nstage == 4 ? 2 : 3;      // (the cluster kernel indexes the ring with / and %)
+    // A stage group's stages are NG * S apart (NG = L).  Its parity wait on empty[] is exact only if the previous
+    // stage of the same slot was its own, i.e. NG * S divides nstage: clusters of 3 and 4 use runs of at most 2.
+    if (S > 1 && d.L * S > d.nstage) {
+        d.L = d.nstage / S;
+        d.lshift = d.L == 2 ? 1 : 0;
+    }
     const size_t fixed = (size_t)d.nstage * A_STAGE + acc_stage_bytes(p.N) + (2 * MAX_NSTAGE + 2 * MAX_NBST) * 8 + 64 * 4 +
                          2 * 16 + (size_t)2 * d.tab_h * d.tab_w * 8 + 1024 + 128;
     d.nbst = fixed + 4 * w_chunk <= 227 * 1024 ? 4 : 2;
     const size_t smem = fixed + d.nbst * w_chunk;
     C2M_CHECK_ARG(smem <= 227 * 1024, "dcn_v2_fused_tc: %zu bytes of shared memory needed", smem);
-    C2M_CUDA(cudaFuncSetAttribute(dcn_wgmma_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    C2M_CUDA(cudaFuncSetAttribute(dcn_wgmma_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    C2M_CUDA(cudaFuncSetAttribute(dcn_wgmma_kernel<48>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    C2M_CUDA(cudaFuncSetAttribute(dcn_wgmma_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    C2M_CUDA(cudaFuncSetAttribute(dcn_wgmma_kernel<16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    C2M_CUDA(cudaFuncSetAttribute(dcn_wgmma_kernel<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    C2M_CUDA(cudaFuncSetAttribute(dcn_wgmma_kernel<48, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    C2M_CUDA(cudaFuncSetAttribute(dcn_wgmma_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    C2M_CUDA(cudaFuncSetAttribute(dcn_wgmma_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int sms = 0;
     C2M_CUDA(sm_count(sms));
     const long long n_items = (long long)a->B * p.tiles_x * p.tiles_y;
@@ -705,17 +797,40 @@ extern "C" int c2m_dcn_v2_fused_tc(const c2m_dcn_tc_args *a, c2m_stream_t stream
     const double px = (double)a->B * a->H * a->W;
     const double flops = 2.0 * a->Cout * a->C * 9.0 * px;
     const double bytes = 4.0 * px * (a->C + 27.0 * a->dg + a->Cout) + 4.0 * a->Cout * (a->C * 9.0 + 1.0);
-    void *ph = prof_begin(PROF_DCN, flops, bytes, st);
-    const int grid = n_items < sms ? (int)n_items : sms;
-    for (d.slice = 0; d.slice < p.nslice; ++d.slice) {
+    d.slice = 0;
+    if (S == 1) {
+        void *ph = prof_begin(PROF_DCN, flops, bytes, st);
+        const int grid = n_items < sms ? (int)n_items : sms;
         switch (p.N) {
-        case 16: dcn_wgmma_kernel<16><<<grid, NTHREADS, smem, st>>>(q, p, d); break;
-        case 32: dcn_wgmma_kernel<32><<<grid, NTHREADS, smem, st>>>(q, p, d); break;
-        case 48: dcn_wgmma_kernel<48><<<grid, NTHREADS, smem, st>>>(q, p, d); break;
-        default: dcn_wgmma_kernel<64><<<grid, NTHREADS, smem, st>>>(q, p, d); break;
+        case 16: dcn_wgmma_kernel<16, false><<<grid, NTHREADS, smem, st>>>(q, p, d); break;
+        case 32: dcn_wgmma_kernel<32, false><<<grid, NTHREADS, smem, st>>>(q, p, d); break;
+        case 48: dcn_wgmma_kernel<48, false><<<grid, NTHREADS, smem, st>>>(q, p, d); break;
+        default: dcn_wgmma_kernel<64, false><<<grid, NTHREADS, smem, st>>>(q, p, d); break;
         }
         C2M_LAUNCH_CHECK("dcn_wgmma_kernel");
+        prof_end(ph, st);
+        return C2M_OK;
     }
+    // Cout > 64: the S slices of a tile run at once on the CTAs of one cluster, which gather it once between them
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = (unsigned)S;
+    attr[0].val.clusterDim.y = attr[0].val.clusterDim.z = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)(S * (sms / S)));
+    cfg.blockDim = dim3(NTHREADS);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    int nclusters = 0;
+    C2M_CUDA(cudaOccupancyMaxActiveClusters(&nclusters, dcn_wgmma_kernel<64, true>, &cfg));
+    C2M_CHECK_ARG(nclusters > 0, "dcn_v2_fused_tc: no cluster of %d CTAs with %zu bytes of shared memory fits", S, smem);
+    if (nclusters > n_items) nclusters = (int)n_items;
+    cfg.gridDim = dim3((unsigned)(S * nclusters));
+    void *ph = prof_begin(PROF_DCN, flops, bytes, st);
+    C2M_CUDA(cudaLaunchKernelEx(&cfg, dcn_wgmma_kernel<64, true>, q, p, d));
+    C2M_LAUNCH_CHECK("dcn_wgmma_kernel");
     prof_end(ph, st);
     return C2M_OK;
 }
