@@ -77,6 +77,44 @@ int make_psa_tensor_map(CUtensorMap *map, const void *base, int B, int C8, int H
 // max |x[i]| over n floats, folded into *out_bits (float bits, start at 0); corr_aux.cu
 __global__ void amax_kernel(const float *__restrict__ x, size_t n, unsigned *__restrict__ out_bits);
 
+// ---- packed-split (PSA) format: every tensor-core operand and PSA activation.  A value v is the fp16 pair
+// hi = rn(v), lo = rn(v - hi) (|lo| <= 2^-11 |v|, so hi + lo carries ~22 bits of v), and a product of two such values
+// is the three MMAs hi*hi + hi*lo + lo*hi (the correlation search drops the Ref's lo, corr_umma.cu).  A tensor
+// [B][C][H][W] is stored as two fp16 planes (hi, lo), each laid out as channel octets [B][ceil(C/8)][H][W][8] with the
+// padding channels of the last octet zero; the tensor-core DCN's operand interleaves them per octet, [hi 8 | lo 8].
+// The split and the unsplit come in a per-element (__half) and a per-pair (__half2) form; each site keeps the form it
+// was tuned with (they round alike but compile differently).
+__device__ __forceinline__ void psa_split(float v, __half &hi, __half &lo) {
+    hi = __float2half_rn(v);
+    lo = __float2half_rn(v - __half2float(hi));
+}
+__device__ __forceinline__ void psa_split2(float a, float b, __half2 &hi, __half2 &lo) {
+    hi = __floats2half2_rn(a, b);
+    const float2 f = __half22float2(hi);
+    lo = __floats2half2_rn(a - f.x, b - f.y);
+}
+// hi + lo of one octet (16 B of each half): element j, or all 8 converted pairwise
+__device__ __forceinline__ float psa_unsplit(const uint4 &hi, const uint4 &lo, int j) {
+    return __half2float(reinterpret_cast<const __half *>(&hi)[j]) + __half2float(reinterpret_cast<const __half *>(&lo)[j]);
+}
+__device__ __forceinline__ void psa_unsplit2(const uint4 &hi, const uint4 &lo, float (&v)[8]) {
+    const __half2 *h = reinterpret_cast<const __half2 *>(&hi), *l = reinterpret_cast<const __half2 *>(&lo);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const float2 a = __half22float2(h[j]), b = __half22float2(l[j]);
+        v[2 * j] = a.x + b.x;
+        v[2 * j + 1] = a.y + b.y;
+    }
+}
+// element offset of octet `oct` of pixel (y, x) of image b in one half-plane; the second form takes the pixel index
+// pix = y * W + x of an HW = H * W plane
+__device__ __forceinline__ size_t psa_offset(int b, int oct, int y, int x, int C8, int H, int W) {
+    return ((((size_t)b * C8 + oct) * H + y) * W + x) * 8;
+}
+__device__ __forceinline__ size_t psa_offset(int b, int oct, long long pix, int C8, long long HW) {
+    return (((size_t)b * C8 + oct) * HW + pix) * 8;
+}
+
 __device__ __forceinline__ uint32_t smem_u32(const void *p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }

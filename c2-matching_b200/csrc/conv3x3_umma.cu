@@ -251,12 +251,9 @@ __global__ void psa_from_f32_kernel(const float *__restrict__ x, int C, int C8, 
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             const int c = oct * 8 + j;
-            const float v = c < C ? x[b * xs_b + c * xs_c + y * xs_y + xx * xs_x] * S : 0.f;
-            const __half hh = __float2half_rn(v);
-            h8[j] = hh;
-            l8[j] = __float2half_rn(v - __half2float(hh));
+            psa_split(c < C ? x[b * xs_b + c * xs_c + y * xs_y + xx * xs_x] * S : 0.f, h8[j], l8[j]);
         }
-        const size_t o = (((size_t)b * C8 + oct) * HW + pix) * 8;
+        const size_t o = psa_offset(b, oct, pix, C8, HW);
         *reinterpret_cast<uint4 *>(hi + o) = *reinterpret_cast<const uint4 *>(h8);
         *reinterpret_cast<uint4 *>(lo + o) = *reinterpret_cast<const uint4 *>(l8);
     }
@@ -273,17 +270,15 @@ __global__ void psa_to_f32_kernel(const __half *__restrict__ hi, const __half *_
         const int oct = (int)(e / HW);
         const long long pix = e % HW;
         const int y = (int)(pix / W), xx = (int)(pix % W);
-        const size_t o = (((size_t)b * C8 + oct) * HW + pix) * 8;
+        const size_t o = psa_offset(b, oct, pix, C8, HW);
         const uint4 rh = *reinterpret_cast<const uint4 *>(hi + o);
         const uint4 rl = *reinterpret_cast<const uint4 *>(lo + o);
-        const __half *hh = reinterpret_cast<const __half *>(&rh);
-        const __half *ll = reinterpret_cast<const __half *>(&rl);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             const int c = oct * 8 + j;
             if (c < C) {
                 const long long oi = b * os_b + c * os_c + y * os_y + xx * os_x;
-                float v = (__half2float(hh[j]) + __half2float(ll[j])) * S;
+                float v = psa_unsplit(rh, rl, j) * S;
                 if (add) v += add[oi];
                 out[oi] = v;
             }
@@ -311,20 +306,14 @@ __global__ void psa_maxpool2_kernel(const __half *__restrict__ hi, const __half 
                 const size_t o = ((((size_t)b * C8 + oct) * H + 2 * yo + dy) * W + 2 * xo + dx) * 8;
                 const uint4 rh = *reinterpret_cast<const uint4 *>(hi + o);
                 const uint4 rl = *reinterpret_cast<const uint4 *>(lo + o);
-                const __half *hh = reinterpret_cast<const __half *>(&rh);
-                const __half *ll = reinterpret_cast<const __half *>(&rl);
 #pragma unroll
-                for (int j = 0; j < 8; ++j) m[j] = fmaxf(m[j], __half2float(hh[j]) + __half2float(ll[j]));
+                for (int j = 0; j < 8; ++j) m[j] = fmaxf(m[j], psa_unsplit(rh, rl, j));
             }
         __align__(16) __half h8[8];
         __align__(16) __half l8[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const __half hq = __float2half_rn(m[j]);
-            h8[j] = hq;
-            l8[j] = __float2half_rn(m[j] - __half2float(hq));
-        }
-        const size_t oo = ((((size_t)b * C8 + oct) * Ho + yo) * Wo + xo) * 8;
+        for (int j = 0; j < 8; ++j) psa_split(m[j], h8[j], l8[j]);
+        const size_t oo = psa_offset(b, oct, yo, xo, C8, Ho, Wo);
         *reinterpret_cast<uint4 *>(ohi + oo) = *reinterpret_cast<const uint4 *>(h8);
         *reinterpret_cast<uint4 *>(olo + oo) = *reinterpret_cast<const uint4 *>(l8);
     }
@@ -334,24 +323,18 @@ __global__ void psa_maxpool2_kernel(const __half *__restrict__ hi, const __half 
 // (hi and lo rows of one octet are adjacent: together they are the 2N-row stacked B operand)
 __global__ void wpack_kernel(const float *__restrict__ w, int Cin, int Cout, int N, int nkc, int nslice,
                              uint8_t *__restrict__ blob) {
-    const float S = wpack_scale(blob);
-    const long long total = (long long)nslice * nkc * 2 * 9 * KOCT * N * 8;
-    __half *dst = reinterpret_cast<__half *>(blob + W_HDR);
-    for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+    wpack_loop(w, blob, (long long)nslice * nkc * 2 * 9 * KOCT * N * 8, [=](long long e, int &half) -> long long {
         const int j = (int)(e & 7);
         long long rest = e >> 3;
         const int ol = (int)(rest % N); rest /= N;
-        const int half = (int)(rest % 2); rest /= 2;
+        half = (int)(rest % 2); rest /= 2;
         const int oct = (int)(rest % KOCT); rest /= KOCT;
         const int tap = (int)(rest % 9); rest /= 9;
         const int kc = (int)(rest % nkc);
         const int slice = (int)(rest / nkc);
         const int c = (kc * KOCT + oct) * 8 + j, o = slice * NMAX + ol;
-        float v = 0.f;
-        if (c < Cin && o < Cout) v = w[((size_t)o * Cin + c) * 9 + tap] * S;
-        const __half hh = __float2half_rn(v);
-        dst[e] = half ? __float2half_rn(v - __half2float(hh)) : hh;
-    }
+        return c < Cin && o < Cout ? ((long long)o * Cin + c) * 9 + tap : -1;
+    });
 }
 
 int wpack_header(const float *w, int n, void *packed, cudaStream_t st) {

@@ -100,9 +100,8 @@ __device__ __forceinline__ void wgrad_consume(uint8_t *smem, uint64_t *full, uin
             for (int tt = 0; tt < NT; ++tt) {
                 const int tap = T0 + tt;
                 const uint32_t xb = (2 * j + tap / 3) * X_ROW_B + (tap % 3) * 16;
-                wgmma_tt_n32(acc[tt], wg_desc_advance(dgh, ga), wg_desc_advance(dxh, xb));
-                wgmma_tt_n32(acc[tt], wg_desc_advance(dgh, ga), wg_desc_advance(dxl, xb));
-                wgmma_tt_n32(acc[tt], wg_desc_advance(dgl, ga), wg_desc_advance(dxh, xb));
+                wgmma_tt_split(acc[tt], wg_desc_advance(dgh, ga), wg_desc_advance(dgl, ga), wg_desc_advance(dxh, xb),
+                               wg_desc_advance(dxl, xb));
             }
         }
         wgmma_commit();

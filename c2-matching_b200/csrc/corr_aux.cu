@@ -106,10 +106,7 @@ __global__ void __launch_bounds__(256) prep_kernel(const float *__restrict__ x, 
             for (int j = 0; j < 8; ++j) {
                 const float v = tile[wq * 8 + j][wp];
                 ssacc = fmaf(v, v, ssacc);
-                const float vs = v * S;
-                const __half hh = __float2half_rn(vs);
-                h8[j] = hh;
-                l8[j] = __float2half_rn(vs - __half2float(hh));
+                psa_split(v * S, h8[j], l8[j]);
             }
             const size_t o = (((size_t)b * (Cp / 8) + (c0 / 8 + wq)) * HW + pix0 + wp) * 8;
             *reinterpret_cast<uint4 *>(hi + o) = *reinterpret_cast<const uint4 *>(h8);

@@ -63,14 +63,7 @@ struct DcnGrad {
 // one corner octet of the interleaved operand (hi 8 | lo 8 = one 32 B sector) as 8 fp32 values
 __device__ __forceinline__ void ld_octet_f32(const __half *x_il, size_t pix, float (&v)[8]) {
     const uint4 *src = reinterpret_cast<const uint4 *>(x_il) + pix * 2;
-    const uint4 h = __ldg(src), l = __ldg(src + 1);
-    const __half2 *hh = reinterpret_cast<const __half2 *>(&h), *ll = reinterpret_cast<const __half2 *>(&l);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        const float2 a = __half22float2(hh[j]), b = __half22float2(ll[j]);
-        v[2 * j] = a.x + b.x;
-        v[2 * j + 1] = a.y + b.y;
-    }
+    psa_unsplit2(__ldg(src), __ldg(src + 1), v);
 }
 }  // namespace
 
@@ -141,20 +134,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) dcn_dgrad_kernel(const __grid_c
                     const uint32_t a_hi = smem_u32(smem + st * DG_STAGE), a_lo = a_hi + PIECE_HALF;
                     const uint32_t w_hi = a_hi + 2 * PIECE_HALF, w_lo = w_hi + w_half;
                     wgmma_fence();
-#pragma unroll
-                    for (int j = 0; j < KOCT / 2; ++j) {
-                        const uint32_t ao = j * 2 * OCT_B, bo = j * 2 * N * 16;
-                        const uint64_t dbh = wg_smem_desc(w_hi + bo, N * 16, 128);
-                        const uint64_t dbl = wg_smem_desc(w_lo + bo, N * 16, 128);
-                        const uint64_t dah = wg_smem_desc(a_hi + ao, OCT_B, 128);
-                        const uint64_t dal = wg_smem_desc(a_lo + ao, OCT_B, 128);
-                        Wgmma<N>::mma(acc0, dah, dbh, (kp | j) != 0);
-                        Wgmma<N>::mma(acc0, dah, dbl, 1);
-                        Wgmma<N>::mma(acc0, dal, dbh, 1);
-                        Wgmma<N>::mma(acc1, wg_desc_advance(dah, 1024), dbh, (kp | j) != 0);
-                        Wgmma<N>::mma(acc1, wg_desc_advance(dah, 1024), dbl, 1);
-                        Wgmma<N>::mma(acc1, wg_desc_advance(dal, 1024), dbh, 1);
-                    }
+                    wgmma_split_chunk128<N, KOCT>(acc0, acc1, a_hi, a_lo, OCT_B, w_hi, w_lo, kp);
                     wgmma_commit();
                     wgmma_wait_all();
                     mbar_arrive(&empty[st]);
@@ -253,24 +233,19 @@ __global__ void __launch_bounds__(DG_THREADS, 1) dcn_dgrad_kernel(const __grid_c
 // C * 9, in the last chunk), row (octet, j) of piece kp is output channel (kp * 4 + octet) * 8 + j
 __global__ void dcn_dgrad_wpack_kernel(const float *__restrict__ w, int C, int Cout, int dg, int N, int nch, int nkp,
                                        uint8_t *__restrict__ blob) {
-    const float S = wpack_scale(blob);
     const int cpg = C / dg;
-    const long long total = (long long)nch * nkp * 2 * KOCT * N * 8;
-    __half *dst = reinterpret_cast<__half *>(blob + W_HDR);
-    for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+    wpack_loop(w, blob, (long long)nch * nkp * 2 * KOCT * N * 8, [=](long long e, int &half) -> long long {
         const int j = (int)(e & 7);
         long long rest = e >> 3;
         const int n = (int)(rest % N); rest /= N;
         const int oct = (int)(rest % KOCT); rest /= KOCT;
-        const int half = (int)(rest % 2); rest /= 2;
+        half = (int)(rest % 2); rest /= 2;
         const int kp = (int)(rest % nkp);
         const int ch = (int)(rest / nkp);
         const int co = (kp * KOCT + oct) * 8 + j, col = ch * N + n;
         const int pair = col / cpg, g = pair / 9, tap = pair % 9, c = g * cpg + col % cpg;
-        const float v = co < Cout && col < C * 9 ? w[((size_t)co * C + c) * 9 + tap] * S : 0.f;
-        const __half hh = __float2half_rn(v);
-        dst[e] = half ? __float2half_rn(v - __half2float(hh)) : hh;
-    }
+        return co < Cout && col < C * 9 ? ((long long)co * C + c) * 9 + tap : -1;
+    });
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -360,11 +335,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) dcn_wgrad_kernel(const __grid_con
             for (int j = 0; j < 8; ++j) {                    // K step j: pixels [16 j, 16 j + 16)
 #pragma unroll
                 for (int h = 0; h < NH; ++h) {
-                    const uint64_t dyh = wg_smem_desc(yh + h * 8 * OCT_B + j * 256, 128, OCT_B);
-                    const uint64_t dyl = wg_smem_desc(yl + h * 8 * OCT_B + j * 256, 128, OCT_B);
-                    wgmma_tt_n32(acc[h], dyh, wg_desc_advance(dch, j * 256));
-                    wgmma_tt_n32(acc[h], dyh, wg_desc_advance(dcl, j * 256));
-                    wgmma_tt_n32(acc[h], dyl, wg_desc_advance(dch, j * 256));
+                    wgmma_tt_split(acc[h], wg_smem_desc(yh + h * 8 * OCT_B + j * 256, 128, OCT_B),
+                                   wg_smem_desc(yl + h * 8 * OCT_B + j * 256, 128, OCT_B), wg_desc_advance(dch, j * 256),
+                                   wg_desc_advance(dcl, j * 256));
                 }
             }
             wgmma_commit();
@@ -412,12 +385,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) dcn_wgrad_kernel(const __grid_con
             __align__(16) __half2 h4[4];
             __align__(16) __half2 l4[4];
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const __half2 hq = __floats2half2_rn(v[2 * j], v[2 * j + 1]);
-                const float2 hf = __half22float2(hq);
-                h4[j] = hq;
-                l4[j] = __floats2half2_rn(v[2 * j] - hf.x, v[2 * j + 1] - hf.y);
-            }
+            for (int j = 0; j < 4; ++j) psa_split2(v[2 * j], v[2 * j + 1], h4[j], l4[j]);
             mbar_wait(&gempty[gs], gph ^ 1);
             uint8_t *dst = sG + gs * WG_COL_STAGE + u * OCT_B + m * 16;
             *reinterpret_cast<uint4 *>(dst) = *reinterpret_cast<const uint4 *>(h4);

@@ -253,7 +253,6 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
         const int o_base = slice() * N;
         for (int i = e; i < N; i += 128) sbias[i] = (q.bias && o_base + i < p.Cout) ? q.bias[o_base + i] : 0.f;
         asm volatile("bar.sync 1, 128;" ::: "memory");
-        constexpr uint32_t b_lbo = N * 16;
         int stage = 0, phase = 0, bst = 0, bphase = 0;
         for (int item = item0(); item < n_items; item += istep()) {
             const int b = item / tiles_img, tt = item - b * tiles_img;
@@ -267,20 +266,7 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
                 const uint32_t w_hi = smem_u32(sW + bst * w_chunk), w_lo = w_hi + w_half;
                 const uint32_t a_hi = smem_u32(sA + stage * A_STAGE), a_lo = a_hi + A_HALF;
                 wgmma_fence();
-#pragma unroll
-                for (int j = 0; j < KOCT / 2; ++j) {
-                    const uint32_t ao = j * 2 * A_OCT_B, bo = j * 2 * b_lbo;
-                    const uint64_t dbh = wg_smem_desc(w_hi + bo, b_lbo, 128);
-                    const uint64_t dbl = wg_smem_desc(w_lo + bo, b_lbo, 128);
-                    const uint64_t dah = wg_smem_desc(a_hi + ao, A_OCT_B, 128);
-                    const uint64_t dal = wg_smem_desc(a_lo + ao, A_OCT_B, 128);
-                    Wgmma<N>::mma(acc0, dah, dbh, (kc | j) != 0);
-                    Wgmma<N>::mma(acc0, dah, dbl, 1);
-                    Wgmma<N>::mma(acc0, dal, dbh, 1);
-                    Wgmma<N>::mma(acc1, wg_desc_advance(dah, 1024), dbh, (kc | j) != 0);
-                    Wgmma<N>::mma(acc1, wg_desc_advance(dah, 1024), dbl, 1);
-                    Wgmma<N>::mma(acc1, wg_desc_advance(dal, 1024), dbh, 1);
-                }
+                wgmma_split_chunk128<N, KOCT>(acc0, acc1, a_hi, a_lo, A_OCT_B, w_hi, w_lo, kc);
                 wgmma_commit();
                 wgmma_wait_all();
                 mbar_arrive(&empty[stage]);
@@ -485,8 +471,8 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
                     ldg_keep_v8(xi + 2u * (unsigned)o1, pol_keep, ch1, cl1);
                     ldg_keep_v8(xi + 2u * (unsigned)o2, pol_keep, ch2, cl2);
                     ldg_keep_v8(xi + 2u * (unsigned)o3, pol_keep, ch3, cl3);
-                    // ---- blend, modulate, split.  value = hi + lo: the hi halves are blended in fp32, the lo halves
-                    // (|lo| <= 2^-11 |value|) in packed fp16 — their rounding lands at 2^-22 of the value
+                    // ---- blend, modulate, split: the hi halves are blended in fp32, the lo halves in packed fp16 —
+                    // their rounding lands at 2^-22 of the value
                     const __half2 *hp0 = reinterpret_cast<const __half2 *>(&ch0), *hp1 = reinterpret_cast<const __half2 *>(&ch1);
                     const __half2 *hp2 = reinterpret_cast<const __half2 *>(&ch2), *hp3 = reinterpret_cast<const __half2 *>(&ch3);
                     const __half2 *lp0 = reinterpret_cast<const __half2 *>(&cl0), *lp1 = reinterpret_cast<const __half2 *>(&cl1);
@@ -504,10 +490,7 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
                         const float2 cq = __half22float2(hp2[j]), dq = __half22float2(hp3[j]);
                         const float vx = fmaf(w0, a.x, fmaf(w1, bq.x, fmaf(w2, cq.x, fmaf(w3, dq.x, lf.x))));
                         const float vy = fmaf(w0, a.y, fmaf(w1, bq.y, fmaf(w2, cq.y, fmaf(w3, dq.y, lf.y))));
-                        const __half2 hq = __floats2half2_rn(vx, vy);
-                        const float2 hf2 = __half22float2(hq);
-                        h4[j] = hq;
-                        l4[j] = __floats2half2_rn(vx - hf2.x, vy - hf2.y);
+                        psa_split2(vx, vy, h4[j], l4[j]);
                     }
                     if (u == 0) mbar_wait(&empty[rs], rphase ^ 1u);
                     *reinterpret_cast<uint4 *>(sdst + u * A_OCT_B) = *reinterpret_cast<const uint4 *>(h4);
@@ -528,28 +511,20 @@ dcn_wgmma_kernel(const ConvPtrs q, const ConvParams p, const DcnTc d) {
 // blob: header | [slice][kc][hi|lo][octet 4][N][8], K ordered (g, tap, channel-in-group)
 __global__ void dcn_wpack_kernel(const float *__restrict__ w, int C, int Cout, int dg, int N, int nkc, int nslice,
                                  uint8_t *__restrict__ blob) {
-    const float S = wpack_scale(blob);
     const int cpg = C / dg, opp = cpg / 8, n_ko = (C / 8) * 9;
-    const long long total = (long long)nslice * nkc * 2 * KOCT * N * 8;
-    __half *dst = reinterpret_cast<__half *>(blob + W_HDR);
-    for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+    wpack_loop(w, blob, (long long)nslice * nkc * 2 * KOCT * N * 8, [=](long long e, int &half) -> long long {
         const int j = (int)(e & 7);
         long long rest = e >> 3;
         const int ol = (int)(rest % N); rest /= N;
         const int oct = (int)(rest % KOCT); rest /= KOCT;
-        const int half = (int)(rest % 2); rest /= 2;
+        half = (int)(rest % 2); rest /= 2;
         const int kc = (int)(rest % nkc);
         const int slice = (int)(rest / nkc);
         const int ko = kc * KOCT + oct, o = slice * N + ol;
-        float v = 0.f;
-        if (ko < n_ko && o < Cout) {
-            const int pair = ko / opp, oc = ko % opp, g = pair / 9, tap = pair % 9;
-            const int c = g * cpg + oc * 8 + j;
-            v = w[((size_t)o * C + c) * 9 + tap] * S;
-        }
-        const __half hh = __float2half_rn(v);
-        dst[e] = half ? __float2half_rn(v - __half2float(hh)) : hh;
-    }
+        if (ko >= n_ko || o >= Cout) return -1;
+        const int pair = ko / opp, oc = ko % opp, g = pair / 9, tap = pair % 9;
+        return ((long long)o * C + g * cpg + oc * 8 + j) * 9 + tap;
+    });
 }
 
 // Largest finite |v| of each image as fp32 bits, for x (blockIdx.z = 0: image b at x + b * nx) and the final mask
@@ -595,10 +570,7 @@ __global__ void dcn_operand_kernel(const float *__restrict__ x, int C, int C8, i
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             const int c = oct * 8 + j;
-            const float v = c < C ? x[b * xs_b + c * xs_c + y * xs_y + xx * xs_x] * S : 0.f;
-            const __half hh = __float2half_rn(v);
-            h8[j] = hh;
-            h8[8 + j] = __float2half_rn(v - __half2float(hh));
+            psa_split(c < C ? x[b * xs_b + c * xs_c + y * xs_y + xx * xs_x] * S : 0.f, h8[j], h8[8 + j]);
         }
         dst[0] = reinterpret_cast<const uint4 *>(h8)[0];
         dst[1] = reinterpret_cast<const uint4 *>(h8)[1];

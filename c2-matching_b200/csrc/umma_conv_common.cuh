@@ -31,6 +31,53 @@ __device__ __forceinline__ float wpack_scale(uint8_t *blob) {
     return ldexpf(1.f, s_sw);
 }
 
+// Pack loop of a weight blob, after wpack_header: packed element e (fp16, after the header) is the hi or lo half of
+// w[src(e, half)] * 2^sw, or 0 where src returns -1 (padding); `src` decodes e and sets `half` (0 hi, 1 lo).  The
+// three blob layouts (conv3x3_umma.cu, dcn_umma.cu, dcn_tc_bwd.cu) differ only in that decode.
+template <class Src>
+__device__ __forceinline__ void wpack_loop(const float *__restrict__ w, uint8_t *blob, long long total, Src src) {
+    const float S = wpack_scale(blob);
+    __half *dst = reinterpret_cast<__half *>(blob + W_HDR);
+    for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+        int half;
+        const long long i = src(e, half);
+        __half hi, lo;
+        psa_split(i >= 0 ? w[i] * S : 0.f, hi, lo);
+        dst[e] = half ? lo : hi;
+    }
+}
+
+// One K chunk (KOCT channel octets, KOCT / 2 K=16 steps) of a 128-row x N tile in split fp16, both operands K-major:
+// A = [octet][128 rows][8] per half, octets a_oct bytes apart, rows 64.. starting 1024 B in (acc1); B = [octet][N][8]
+// per half.  Three products per step, hi*hi + hi*lo + lo*hi; K chunk kc = 0 starts the accumulators.
+template <int N, int KOCT, int R>
+__device__ __forceinline__ void wgmma_split_chunk128(float (&acc0)[R], float (&acc1)[R], uint32_t a_hi, uint32_t a_lo,
+                                                     uint32_t a_oct, uint32_t w_hi, uint32_t w_lo, int kc) {
+    constexpr uint32_t b_lbo = N * 16;
+#pragma unroll
+    for (int j = 0; j < KOCT / 2; ++j) {
+        const uint32_t ao = j * 2 * a_oct, bo = j * 2 * b_lbo;
+        const uint64_t dbh = wg_smem_desc(w_hi + bo, b_lbo, 128);
+        const uint64_t dbl = wg_smem_desc(w_lo + bo, b_lbo, 128);
+        const uint64_t dah = wg_smem_desc(a_hi + ao, a_oct, 128);
+        const uint64_t dal = wg_smem_desc(a_lo + ao, a_oct, 128);
+        Wgmma<N>::mma(acc0, dah, dbh, (kc | j) != 0);
+        Wgmma<N>::mma(acc0, dah, dbl, 1);
+        Wgmma<N>::mma(acc0, dal, dbh, 1);
+        Wgmma<N>::mma(acc1, wg_desc_advance(dah, 1024), dbh, (kc | j) != 0);
+        Wgmma<N>::mma(acc1, wg_desc_advance(dah, 1024), dbl, 1);
+        Wgmma<N>::mma(acc1, wg_desc_advance(dal, 1024), dbh, 1);
+    }
+}
+
+// One K=16 step in split fp16 with both operands MN-major (wgmma_tt_n32): hi*hi + hi*lo + lo*hi into acc
+__device__ __forceinline__ void wgmma_tt_split(float (&acc)[16], uint64_t a_hi, uint64_t a_lo, uint64_t b_hi,
+                                               uint64_t b_lo) {
+    wgmma_tt_n32(acc, a_hi, b_hi);
+    wgmma_tt_n32(acc, a_hi, b_lo);
+    wgmma_tt_n32(acc, a_lo, b_hi);
+}
+
 // Gradient scale exponent: sg = 14 - floor(log2 amax) (amax * 2^sg in [2^14, 2^15)), from the bits of the largest finite
 // |grad_output|; 0 for an all-zero gradient, clamped to +-120 so that 2^sg and 2^-sg are normal floats.
 __host__ __device__ __forceinline__ int grad_scale_exp(const unsigned *amax) {
@@ -154,7 +201,7 @@ __device__ __forceinline__ void prefetch_residual(const __half *rh, const __half
     for (int o8 = 0; o8 < 4; ++o8) {
         const int oct = (o_base + c0) / 8 + o8;
         if (ok && c0 + o8 * 8 < p.N && oct < p.C8out) {
-            const size_t off = ((((size_t)b * p.C8out + oct) * p.H + y) * p.W + x) * 8;
+            const size_t off = psa_offset(b, oct, y, x, p.C8out, p.H, p.W);
             r.h[o8] = *reinterpret_cast<const uint4 *>(rh + off);
             r.l[o8] = *reinterpret_cast<const uint4 *>(rl + off);
         } else {
@@ -187,8 +234,7 @@ __device__ __forceinline__ void epilogue_store_block(const ConvPtrs &q, const Co
         for (int o8 = 0; o8 < 4; ++o8) {
             const int oct = (o_base + c0) / 8 + o8;
             if (o8 * 8 >= ncol || oct >= p.C8out) break;
-            float4 *dst = reinterpret_cast<float4 *>(
-                q.out_f32 + ((((size_t)b * p.C8out + oct) * p.H + y) * p.W + x) * 8);
+            float4 *dst = reinterpret_cast<float4 *>(q.out_f32 + psa_offset(b, oct, y, x, p.C8out, p.H, p.W));
             dst[0] = make_float4(v[o8 * 8], v[o8 * 8 + 1], v[o8 * 8 + 2], v[o8 * 8 + 3]);
             dst[1] = make_float4(v[o8 * 8 + 4], v[o8 * 8 + 5], v[o8 * 8 + 6], v[o8 * 8 + 7]);
         }
@@ -219,31 +265,24 @@ __device__ __forceinline__ void epilogue_store_block(const ConvPtrs &q, const Co
         for (int o8 = 0; o8 < 4; ++o8) {
             const int oct = (o_base + c0) / 8 + o8;
             if (o8 * 8 >= ncol || oct >= p.C8out) break;
-            const size_t off = ((((size_t)b * p.C8out + oct) * p.H + y) * p.W + x) * 8;
+            const size_t off = psa_offset(b, oct, y, x, p.C8out, p.H, p.W);
             float r8[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
             if (r1) {
-                const __half *hh = reinterpret_cast<const __half *>(&r1->h[o8]);
-                const __half *ll = reinterpret_cast<const __half *>(&r1->l[o8]);
 #pragma unroll
-                for (int j = 0; j < 8; ++j) r8[j] = (__half2float(hh[j]) + __half2float(ll[j])) * res_scale;
+                for (int j = 0; j < 8; ++j) r8[j] = psa_unsplit(r1->h[o8], r1->l[o8], j) * res_scale;
             }
             if (q.res2_hi) {
                 const uint4 rh = *reinterpret_cast<const uint4 *>(q.res2_hi + off);
                 const uint4 rl = *reinterpret_cast<const uint4 *>(q.res2_lo + off);
-                const __half *hh = reinterpret_cast<const __half *>(&rh);
-                const __half *ll = reinterpret_cast<const __half *>(&rl);
 #pragma unroll
-                for (int j = 0; j < 8; ++j) r8[j] += (__half2float(hh[j]) + __half2float(ll[j])) * res_scale;
+                for (int j = 0; j < 8; ++j) r8[j] += psa_unsplit(rh, rl, j) * res_scale;
             }
             __align__(16) __half h8[8];
             __align__(16) __half l8[8];
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
                 const int o = o_base + c0 + o8 * 8 + j;
-                const float vs = (o < p.Cout ? v[o8 * 8 + j] + r8[j] : 0.f) * so;
-                const __half hh = __float2half_rn(vs);
-                h8[j] = hh;
-                l8[j] = __float2half_rn(vs - __half2float(hh));
+                psa_split((o < p.Cout ? v[o8 * 8 + j] + r8[j] : 0.f) * so, h8[j], l8[j]);
             }
             if (p.cs) {
                 __stcs(reinterpret_cast<uint4 *>(q.out_hi + off), *reinterpret_cast<const uint4 *>(h8));
@@ -266,12 +305,7 @@ __device__ __forceinline__ void epilogue_store_block(const ConvPtrs &q, const Co
                 __align__(16) __half h8[8];
                 __align__(16) __half l8[8];
 #pragma unroll
-                for (int c = 0; c < 8; ++c) {
-                    const float vs = v[c * 4 + ij] * so;
-                    const __half hh = __float2half_rn(vs);
-                    h8[c] = hh;
-                    l8[c] = __float2half_rn(vs - __half2float(hh));
-                }
+                for (int c = 0; c < 8; ++c) psa_split(v[c * 4 + ij] * so, h8[c], l8[c]);
                 *reinterpret_cast<uint4 *>(q.out_hi + off) = *reinterpret_cast<const uint4 *>(h8);
                 *reinterpret_cast<uint4 *>(q.out_lo + off) = *reinterpret_cast<const uint4 *>(l8);
             }
@@ -343,14 +377,10 @@ __device__ __forceinline__ void epilogue_fast_block(const ConvPtrs &q, const Con
             v[j] = a;
         }
         if (RES) {
-            const __half2 *hh = reinterpret_cast<const __half2 *>(&r1->h[o8]);
-            const __half2 *ll = reinterpret_cast<const __half2 *>(&r1->l[o8]);
+            float r[8];
+            psa_unsplit2(r1->h[o8], r1->l[o8], r);
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const float2 fh = __half22float2(hh[j]), fl = __half22float2(ll[j]);
-                v[2 * j] = fmaf(fh.x + fl.x, res_scale, v[2 * j]);
-                v[2 * j + 1] = fmaf(fh.y + fl.y, res_scale, v[2 * j + 1]);
-            }
+            for (int j = 0; j < 8; ++j) v[j] = fmaf(r[j], res_scale, v[j]);
         }
         const size_t off = off0 + o8 * plane;
         if (F32OCT) {
@@ -361,12 +391,7 @@ __device__ __forceinline__ void epilogue_fast_block(const ConvPtrs &q, const Con
             __align__(16) __half2 h4[4];
             __align__(16) __half2 l4[4];
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const __half2 hq = __floats2half2_rn(v[2 * j], v[2 * j + 1]);
-                const float2 hf = __half22float2(hq);
-                h4[j] = hq;
-                l4[j] = __floats2half2_rn(v[2 * j] - hf.x, v[2 * j + 1] - hf.y);
-            }
+            for (int j = 0; j < 4; ++j) psa_split2(v[2 * j], v[2 * j + 1], h4[j], l4[j]);
             if (p.cs) {
                 __stcs(reinterpret_cast<uint4 *>(q.out_hi + off), *reinterpret_cast<const uint4 *>(h4));
                 __stcs(reinterpret_cast<uint4 *>(q.out_lo + off), *reinterpret_cast<const uint4 *>(l4));
