@@ -31,7 +31,7 @@ class ConvArgs(ctypes.Structure):
                 ('pixel_shuffle', ctypes.c_int),
                 ('out_f32', ctypes.c_void_p), ('add_f32', ctypes.c_void_p),
                 ('os_b', ctypes.c_longlong), ('os_c', ctypes.c_longlong), ('os_y', ctypes.c_longlong),
-                ('os_x', ctypes.c_longlong), ('out_f32_octets', ctypes.c_int)]
+                ('os_x', ctypes.c_longlong), ('out_f32_octets', ctypes.c_int), ('x_amax', ctypes.c_void_p)]
 
 
 class DcnTcArgs(ctypes.Structure):
@@ -94,8 +94,12 @@ SYMBOLS = {
                               [ctypes.c_void_p] * 4),
     'c2m_grad_unscale_f32': (ctypes.c_int, [c_f32p, ctypes.c_longlong, ctypes.c_void_p, ctypes.c_void_p]),
     'c2m_conv3x3_wgrad_workspace_bytes': (ctypes.c_size_t, [ctypes.c_int] * 5),
+    'c2m_conv3x3_operand_f32': (ctypes.c_int, [c_f32p] + [ctypes.c_int] * 4 + [ctypes.c_longlong] * 4 +
+                                [ctypes.c_void_p] * 4),
     'c2m_conv3x3_wgrad': (ctypes.c_int, [ctypes.c_void_p] * 5 + [ctypes.c_int] * 5 +
                           [c_f32p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
+    'c2m_conv3x3_wgrad_scaled': (ctypes.c_int, [ctypes.c_void_p] * 6 + [ctypes.c_int] * 5 +
+                                 [c_f32p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
     'c2m_psa_maxpool2': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 4 + [ctypes.c_void_p] * 3),
     'c2m_dcn_tc_supported': (ctypes.c_int, [ctypes.c_int] * 3),
     'c2m_dcn_tc_packed_weight_bytes': (ctypes.c_size_t, [ctypes.c_int] * 3),

@@ -32,7 +32,7 @@ def profile_enable(on=True):
     _lib.check(_lib.lib().c2m_profile_enable(int(bool(on))), 'c2m_profile_enable')
 
 
-PROF_KERNELS = {'corr_search': 0, 'conv3x3': 1, 'dcn': 2, 'dcn_dgrad': 3, 'dcn_wgrad': 4}
+PROF_KERNELS = {'corr_search': 0, 'conv3x3': 1, 'dcn': 2, 'dcn_dgrad': 3, 'dcn_wgrad': 4, 'conv3x3_wgrad': 5}
 
 
 def profile_collect(kernel):
@@ -406,11 +406,12 @@ _ACT = {None: 0, 'none': 0, 'relu': 1, 'lrelu': 2}
 
 def conv3x3_psa(x, weight, bias, act=None, residual=None, residual2=None, x2=None, out=None, sa_out=0,
                 pixel_shuffle=0, out_f32=False, add_f32=None, psa_out=True, channels_last=False, f32_octets=False,
-                packed=None):
+                packed=None, x_amax=None):
     """y = act(conv3x3(cat[x, x2], weight) + bias), fp32-grade on tensor cores.
     f32_octets: the fp32 result is an OctF32 (octet-planar) instead of a strided tensor.
     packed: a packed blob of `weight` made elsewhere (the input gradient's rotated weights); `weight` then only gives
     the shape.
+    x_amax: the per-image amax of `x` from _conv3x3_operand (x.sa is then unused).
 
     Returns the PSA tensor `y + residual + residual2` (or PixelShuffle(2)(y)), and/or — with
     out_f32=True — the fp32 tensor `y + add_f32`.  With both, returns (psa, f32)."""
@@ -427,6 +428,8 @@ def conv3x3_psa(x, weight, bias, act=None, residual=None, residual2=None, x2=Non
             raise RuntimeError('conv3x3_psa: concatenated inputs must share batch / size / scale')
         a.in2_hi, a.in2_lo, a.Cin2 = x2.hi.data_ptr(), x2.lo.data_ptr(), x2.C
     a.B, a.H, a.W, a.sa_in = x.B, x.H, x.W, x.sa
+    if x_amax is not None:
+        a.x_amax = x_amax.data_ptr()
     a.packed_w, a.bias = blob.data_ptr(), (bias.data_ptr() if bias is not None else None)
     a.Cout, a.act = cout, _ACT[act]
     for r, (fh, fl) in ((residual, ('res_hi', 'res_lo')), (residual2, ('res2_hi', 'res2_lo'))):
@@ -481,22 +484,36 @@ def _grad_psa(gy):
     return gp, amax
 
 
+def _conv3x3_operand(x):
+    """x [B,C,H,W] fp32 (any strides, any magnitude) as PSA image b times 2^sa_b, and the [B] amax buffer the kernels
+    read sa_b from (c2m_conv3x3_operand_f32).  Call with x's device current."""
+    B, C, H, W = x.shape
+    xp = PSA.empty(B, C, H, W, x.device)
+    amax = torch.empty(B, dtype=torch.int32, device=x.device)
+    _lib.check(_lib.lib().c2m_conv3x3_operand_f32(x.data_ptr(), B, C, H, W, *x.stride(), xp.hi.data_ptr(),
+                                                  xp.lo.data_ptr(), amax.data_ptr(), _stream()),
+               'c2m_conv3x3_operand_f32')
+    return xp, amax
+
+
 class _Conv3x3(torch.autograd.Function):
-    """Forward on conv3x3_wgmma_kernel; backward: the activation's backward, dX on the same kernel with the rotated
-    weights, dW on conv3x3_wgrad_kernel, db as a torch sum.  grad_output enters the kernels as PSA at a power-of-two
-    scale chosen on the device (c2m_grad_psa_from_f32), which the results divide back out on the device."""
+    """Forward on conv3x3_wgmma_kernel from x at a power-of-two scale per image chosen on the device
+    (c2m_conv3x3_operand_f32); backward: the activation's backward, dX on the same kernel with the rotated weights, dW
+    on conv3x3_wgrad_kernel, db as a torch sum.  grad_output enters the kernels as PSA at a power-of-two scale chosen on
+    the device (c2m_grad_psa_from_f32).  The results divide every scale back out on the device."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, act):
-        xp = psa_from_f32(x)
-        y = conv3x3_psa(xp, weight, bias, act=act, psa_out=False, out_f32=True)
+        with torch.cuda.device(x.device):
+            xp, x_amax = _conv3x3_operand(x)
+        y = conv3x3_psa(xp, weight, bias, act=act, psa_out=False, out_f32=True, x_amax=x_amax)
         ctx.act = act
-        ctx.save_for_backward(xp.hi, xp.lo, weight, y if act else None)
+        ctx.save_for_backward(xp.hi, xp.lo, x_amax, weight, y if act else None)
         return y
 
     @staticmethod
     def backward(ctx, gy):
-        x_hi, x_lo, weight, y = ctx.saved_tensors
+        x_hi, x_lo, x_amax, weight, y = ctx.saved_tensors
         need_x, need_w, need_b = ctx.needs_input_grad[:3]
         B, c8, H, W, _ = x_hi.shape
         cout, cin = weight.shape[:2]
@@ -519,9 +536,9 @@ class _Conv3x3(torch.autograd.Function):
                 nbytes = _lib.check_size(L.c2m_conv3x3_wgrad_workspace_bytes(B, cin, cout, H, W),
                                          'c2m_conv3x3_wgrad_workspace_bytes')
                 ws = _workspace(nbytes, dev)
-                _lib.check(L.c2m_conv3x3_wgrad(gp.hi.data_ptr(), gp.lo.data_ptr(), amax.data_ptr(), x_hi.data_ptr(),
-                                               x_lo.data_ptr(), B, cin, cout, H, W, dw.data_ptr(), ws.data_ptr(),
-                                               nbytes, _stream()), 'c2m_conv3x3_wgrad')
+                _lib.check(L.c2m_conv3x3_wgrad_scaled(gp.hi.data_ptr(), gp.lo.data_ptr(), amax.data_ptr(), x_hi.data_ptr(),
+                                               x_lo.data_ptr(), x_amax.data_ptr(), B, cin, cout, H, W, dw.data_ptr(),
+                                               ws.data_ptr(), nbytes, _stream()), 'c2m_conv3x3_wgrad_scaled')
             if need_b:
                 db = gy.sum((0, 2, 3))
         return dx, dw, db, None
@@ -530,8 +547,10 @@ class _Conv3x3(torch.autograd.Function):
 def conv3x3(x, weight, bias=None, act=None):
     """Differentiable act(conv2d(x, weight, bias, stride 1, padding 1)) on the tensor cores, fp32-grade forward and
     backward (fp32 in, fp32 out).  x [B,Cin,H,W] with H >= 18 and W >= 10, weight [Cout,Cin,3,3], bias [Cout] or None,
-    act None / 'relu' / 'lrelu' (LeakyReLU(0.1)).  The forward converts x to PSA at scale exponent 0, so |x| must stay
-    within fp16's range (the inference path's contract for activations); the backward scales grad_output itself."""
+    act None / 'relu' / 'lrelu' (LeakyReLU(0.1)).  Any fp32 magnitude: each image of x and grad_output enters the
+    kernels at a power-of-two scale chosen on the device from its largest finite value, so x * 2^k gives exactly 2^k
+    times the output and dW.  NaN / Inf propagate to the entries that depend on them, as in an fp32 convolution (the
+    input gradient of a non-finite weight also reaches the map's border)."""
     _require_cuda('x', x)
     _require_cuda('weight', weight)
     if bias is not None:

@@ -19,7 +19,7 @@ void count_launch(unsigned n = 1);
 // Measurement hook (include/c2m_sm100.h c2m_profile_*): kernel classes timed with CUDA events on the
 // launching stream while profiling is enabled.
 enum ProfKernel { PROF_CORR_SEARCH = 0, PROF_CONV3X3 = 1, PROF_DCN = 2, PROF_DCN_DGRAD = 3, PROF_DCN_WGRAD = 4,
-                  PROF_NKERNELS = 5 };
+                  PROF_CONV3X3_WGRAD = 5, PROF_NKERNELS = 6 };
 bool prof_enabled();
 void *prof_begin(int kernel, double flops, double bytes, cudaStream_t st);   // null when disabled
 void prof_end(void *handle, cudaStream_t st);

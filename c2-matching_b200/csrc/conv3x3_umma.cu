@@ -171,6 +171,8 @@ conv3x3_wgmma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
             tile_at(g, b, y0, x0);
             const int y = y0 + e / T_C, x = x0 + e % T_C;
             const bool ok = y < p.H && x < p.W;
+            // per-image input exponents (ops.conv3x3): 2^-(sa_b + sw) for this tile's image
+            const float osc = q.x_amax ? ldexpf(1.f, -(grad_scale_exp(q.x_amax + b) + sw)) : out_scale;
             ResRegs ra;
             if (has1 && c0 < N) {
                 if (full_blk) prefetch_residual_full(q.res_hi, q.res_lo, p, b, y, x, ok, o_base, c0, ra);
@@ -215,15 +217,15 @@ conv3x3_wgmma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
             // local memory, and its store there would wait for the prefetch in front of the MMAs.
             if (c0 < N) {
                 if (full_blk && has1)
-                    epilogue_fast_dispatch(q, p, acc_s + e, c0, b, y, x, ok, o_base, sbias + UC_NMAX, out_scale * so,
+                    epilogue_fast_dispatch(q, p, acc_s + e, c0, b, y, x, ok, o_base, sbias + UC_NMAX, osc * so,
                                            res_scale * so, &ra);
                 else if (full_blk)
-                    epilogue_fast_dispatch(q, p, acc_s + e, c0, b, y, x, ok, o_base, sbias + UC_NMAX, out_scale * so,
+                    epilogue_fast_dispatch(q, p, acc_s + e, c0, b, y, x, ok, o_base, sbias + UC_NMAX, osc * so,
                                            res_scale * so, nullptr);
                 else if (has1)
-                    epilogue_store_block(q, p, acc_s + e, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, so, &ra);
+                    epilogue_store_block(q, p, acc_s + e, c0, b, y, x, ok, o_base, sbias, osc, res_scale, so, &ra);
                 else
-                    epilogue_store_block(q, p, acc_s + e, c0, b, y, x, ok, o_base, sbias, out_scale, res_scale, so,
+                    epilogue_store_block(q, p, acc_s + e, c0, b, y, x, ok, o_base, sbias, osc, res_scale, so,
                                          nullptr);
             }
         }
@@ -235,13 +237,13 @@ conv3x3_wgmma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
 // ------------------------------------------------------------------------------------------
 __global__ void psa_from_f32_kernel(const float *__restrict__ x, int C, int C8, int H, int W, long long xs_b,
                                     long long xs_c, long long xs_y, long long xs_x, int sa,
-                                    const unsigned *__restrict__ amax, __half *__restrict__ hi,
+                                    const unsigned *__restrict__ amax, int amax_step, __half *__restrict__ hi,
                                     __half *__restrict__ lo) {
     // one thread = one (octet, pixel); pixel fastest -> coalesced NCHW reads and 16 B stores
     const long long HW = (long long)H * W;
     const long long n = (long long)C8 * HW;
     const int b = blockIdx.y;
-    const float S = ldexpf(1.f, amax ? grad_scale_exp(amax) : sa);
+    const float S = ldexpf(1.f, amax ? grad_scale_exp(amax + b * amax_step) : sa);
     for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x) {
         const int oct = (int)(e / HW);
         const long long pix = e % HW;
@@ -339,9 +341,11 @@ __global__ void wpack_kernel(const float *__restrict__ w, int Cin, int Cout, int
 
 int wpack_header(const float *w, int n, void *packed, cudaStream_t st) {
     C2M_CUDA(cudaMemsetAsync(packed, 0, W_HDR, st));
-    amax_kernel<<<ceil_div(n, 1024) > 64 ? 64 : ceil_div(n, 1024), 256, 0, st>>>(
-        w, (size_t)n, reinterpret_cast<unsigned *>(packed) + 1);
-    C2M_LAUNCH_CHECK("amax_kernel");
+    // the largest FINITE |w|: one Inf weight must not set the scale of all the others (it stays Inf in its own
+    // output channel)
+    grad_amax_kernel<<<dim3(ceil_div(n, 1024) > 64 ? 64 : ceil_div(n, 1024), 1), 256, 0, st>>>(
+        w, 1, 1, n, 0, 0, 0, 1, reinterpret_cast<unsigned *>(packed) + 1, 0);
+    C2M_LAUNCH_CHECK("grad_amax_kernel");
     return C2M_OK;
 }
 
@@ -381,7 +385,8 @@ extern "C" int c2m_psa_from_f32(const float *x, int B, int C, int H, int W, long
     int bx = (int)((n + 255) / 256);
     if (bx > 4096) bx = 4096;
     psa_from_f32_kernel<<<dim3(bx, B), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-        x, C, C8, H, W, xs_b, xs_c, xs_y, xs_x, sa, nullptr, reinterpret_cast<__half *>(hi), reinterpret_cast<__half *>(lo));
+        x, C, C8, H, W, xs_b, xs_c, xs_y, xs_x, sa, nullptr, 0, reinterpret_cast<__half *>(hi),
+        reinterpret_cast<__half *>(lo));
     C2M_LAUNCH_CHECK("psa_from_f32_kernel");
     return C2M_OK;
 }
@@ -427,6 +432,7 @@ extern "C" int c2m_conv3x3(const c2m_conv3x3_args *a, c2m_stream_t stream) {
     C2M_CHECK_ARG((a->res_hi == nullptr) == (a->res_lo == nullptr) && (a->res2_hi == nullptr) == (a->res2_lo == nullptr),
                   "conv3x3: residual needs both halves");
     C2M_CHECK_ARG(a->act >= 0 && a->act <= 2, "conv3x3: unknown activation %d", a->act);
+    C2M_CHECK_ARG(!a->x_amax || !a->in2_hi, "conv3x3: per-image input exponents need a single input");
     C2M_CHECK_ARG((a->out_hi == nullptr) == (a->out_lo == nullptr), "conv3x3: PSA output needs both halves");
     C2M_CHECK_ARG(a->out_hi || a->out_f32, "conv3x3: no output requested");
     C2M_CHECK_ARG(a->pixel_shuffle == 0 || (a->pixel_shuffle == 2 && a->Cout % 32 == 0 && a->out_hi && !a->res_hi),
@@ -459,6 +465,7 @@ extern "C" int c2m_conv3x3(const c2m_conv3x3_args *a, c2m_stream_t stream) {
     q.res2_hi = reinterpret_cast<const __half *>(a->res2_hi); q.res2_lo = reinterpret_cast<const __half *>(a->res2_lo);
     q.out_hi = reinterpret_cast<__half *>(a->out_hi); q.out_lo = reinterpret_cast<__half *>(a->out_lo);
     q.out_f32 = a->out_f32; q.add_f32 = a->add_f32;
+    q.x_amax = a->x_amax;
     CUtensorMap mh, ml, m2h, m2l;
     int rc;
     if ((rc = make_psa_tensor_map(&mh, a->in_hi, a->B, (a->Cin + 7) / 8, a->H, a->W, A_C, A_R))) return rc;

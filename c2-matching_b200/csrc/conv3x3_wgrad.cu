@@ -44,12 +44,31 @@ struct WgradGeom {
     int nslice, nchunk, ksplit;
     int tiles_x, tiles_y;
     long long ntiles;
+    const unsigned *x_amax;     // [B] or null: image b of X is stored as x * 2^grad_scale_exp(x_amax + b)
 };
+
+// Tile t of the batch: image b and top-left pixel (y0, x0).  The last tile row and column are moved back inside the
+// map (y0 = H - 16, x0 = W - 8) when the map is not a multiple of the tile, so no tile holds a pixel outside the map:
+// a zero-filled grad_output there would meet X's last row or column at tap ky = 0 / kx = 0, and 0 * Inf is NaN.  The
+// first dy rows and dx columns of such a tile were already summed by its neighbour; the consumers zero them in gY.
+struct WgradTile { int b, y0, x0, dy, dx; };
+__device__ __forceinline__ WgradTile wgrad_tile(const WgradGeom &p, long long t) {
+    const int tiles_img = p.tiles_x * p.tiles_y;
+    WgradTile r;
+    r.b = (int)(t / tiles_img);
+    const int tt = (int)(t % tiles_img);
+    r.y0 = (tt / p.tiles_x) * G_R;
+    r.x0 = (tt % p.tiles_x) * G_C;
+    r.dy = max(0, r.y0 + G_R - p.H);
+    r.dx = max(0, r.x0 + G_C - p.W);
+    r.y0 -= r.dy;
+    r.x0 -= r.dx;
+    return r;
+}
 }  // namespace
 
-// Largest finite |g| of a strided [B,C,H,W] tensor as fp32 bits (NaN and Inf do not set the scale); *amax starts at 0.
 __global__ void grad_amax_kernel(const float *__restrict__ g, int C, int H, int W, long long s_b, long long s_c,
-                                 long long s_y, long long s_x, unsigned *__restrict__ amax) {
+                                 long long s_y, long long s_x, unsigned *__restrict__ amax, int amax_step) {
     const long long n = (long long)C * H * W;
     const int b = blockIdx.y;
     float m = 0.f;
@@ -61,7 +80,7 @@ __global__ void grad_amax_kernel(const float *__restrict__ g, int C, int H, int 
     }
 #pragma unroll
     for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(amax, __float_as_uint(m));
+    if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(amax + b * amax_step, __float_as_uint(m));
 }
 
 __global__ void grad_unscale_kernel(float *__restrict__ x, long long n, const unsigned *__restrict__ amax) {
@@ -83,10 +102,35 @@ __device__ __forceinline__ void wgrad_consume(uint8_t *smem, uint64_t *full, uin
     const int ci_pad = p.nchunk * WG_CI, ncol = 9 * ci_pad;
     float *blk = dst + (size_t)slice * WG_CO * ncol + T0 * ci_pad + chunk * WG_CI;
     bool first = true;
-    int stage = 0, phase = 0, n = 0;
+    // each accumulator run holds one image: the flush divides its input exponent back out.  |exponent| <= 120, so
+    // the scale is a normal float and the product rounds like ldexpf (one multiply instead of ldexpf per register).
+    auto flush = [&](int b) {
+        const float sc = ldexpf(1.f, p.x_amax && b >= 0 ? -grad_scale_exp(p.x_amax + b) : 0);
+#pragma unroll
+        for (int t = 0; t < NT; ++t)
+#pragma unroll
+            for (int i = 0; i < 16; ++i) acc[t][i] *= sc;
+        wgrad_flush<false>(acc, blk, ncol, ci_pad, first, 0);
+        first = false;
+    };
+    int stage = 0, phase = 0, n = 0, cur_b = -1;
     for (long long t = t0; t < t1; ++t) {
+        const WgradTile tl = wgrad_tile(p, t);
+        if (n > 0 && (tl.b != cur_b || n == WG_FLUSH)) { flush(cur_b); n = 0; }
+        cur_b = tl.b;
         mbar_wait(&full[stage], phase);
         const uint32_t s = smem_u32(smem + stage * WG_STAGE);
+        if (tl.dy | tl.dx) {
+            // a tile moved back inside the map: zero gY (both halves, every octet) at the rows / columns its
+            // neighbour already summed, then make the writes visible to the tensor cores of both warpgroups
+            uint4 *g = reinterpret_cast<uint4 *>(smem + stage * WG_STAGE);
+            for (int i = threadIdx.x - 128; i < 2 * G_OCT * G_R * G_C; i += 256) {
+                const int c = i % G_C, r = (i / G_C) % G_R;
+                if (r < tl.dy || c < tl.dx) g[i] = make_uint4(0, 0, 0, 0);
+            }
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+        }
         // MN-major descriptors: lbo = next core matrix along K (the next tile row), sbo = next octet along M / N.
         // A = gY (M = Cout, K = pixels), B = X (N = Cin, K = pixels).
         const uint64_t dgh = wg_smem_desc(s, G_ROW_B, G_OCT_B), dgl = wg_smem_desc(s + G_HALF, G_ROW_B, G_OCT_B);
@@ -108,9 +152,9 @@ __device__ __forceinline__ void wgrad_consume(uint8_t *smem, uint64_t *full, uin
         wgmma_wait_all();
         mbar_arrive(&empty[stage]);
         if (++stage == WG_NST) { stage = 0; phase ^= 1; }
-        if (++n == WG_FLUSH) { wgrad_flush<false>(acc, blk, ncol, ci_pad, first, 0); first = false; n = 0; }
+        ++n;
     }
-    if (n || first) wgrad_flush<false>(acc, blk, ncol, ci_pad, first, 0);
+    if (n || first) flush(cur_b);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -131,7 +175,6 @@ conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tg_hi, const __grid_con
     const int chunk = (blockIdx.x / p.nslice) % p.nchunk;
     const int k = blockIdx.x / (p.nslice * p.nchunk);
     const long long t0 = p.ntiles * k / p.ksplit, t1 = p.ntiles * (k + 1) / p.ksplit;
-    const int tiles_img = p.tiles_x * p.tiles_y;
     // the second gY box (octets 4..7 of the slice) holds only zero padding when the slice has <= 32 channels: skip it
     const bool g_second = slice * G_OCT + 4 < p.C8o;
 
@@ -153,8 +196,8 @@ conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tg_hi, const __grid_con
             const uint32_t bytes = 2 * (g_second ? G_HALF : G_HALF / 2) + 2 * X_HALF;
             int stage = 0, phase = 0;
             for (long long t = t0; t < t1; ++t) {
-                const int b = (int)(t / tiles_img), tt = (int)(t % tiles_img);
-                const int y0 = (tt / p.tiles_x) * G_R, x0 = (tt % p.tiles_x) * G_C;
+                const WgradTile tl = wgrad_tile(p, t);
+                const int b = tl.b, y0 = tl.y0, x0 = tl.x0;
                 mbar_wait(&empty[stage], phase ^ 1);
                 uint8_t *s = smem + stage * WG_STAGE;
                 mbar_arrive_expect_tx(&full[stage], bytes);
@@ -196,6 +239,7 @@ __global__ void wgrad_reduce_kernel(const float *__restrict__ ws, int nslots, in
 
 static int wgrad_geom(int B, int Cin, int Cout, int H, int W, WgradGeom &g) {
     g.B = B; g.H = H; g.W = W; g.Cin = Cin; g.Cout = Cout;
+    g.x_amax = nullptr;
     g.C8i = (Cin + 7) / 8; g.C8o = (Cout + 7) / 8;
     g.nslice = ceil_div(Cout, WG_CO);
     g.nchunk = ceil_div(Cin, WG_CI);
@@ -209,23 +253,41 @@ static int wgrad_geom(int B, int Cin, int Cout, int H, int W, WgradGeom &g) {
 
 using namespace c2m;
 
-extern "C" int c2m_grad_psa_from_f32(const float *g, int B, int C, int H, int W, long long gs_b, long long gs_c,
-                                     long long gs_y, long long gs_x, void *hi, void *lo, unsigned *amax,
-                                     c2m_stream_t stream) {
-    C2M_CHECK_ARG(g && hi && lo && amax && B > 0 && C > 0 && H > 0 && W > 0, "grad_psa_from_f32: bad argument");
+namespace c2m {
+// g [B,C,H,W] fp32 -> PSA g * 2^grad_scale_exp(amax), with the largest finite |g| of the batch in amax[0]
+// (per_image 0) or of each image in amax[b] (1)
+static int scaled_psa_from_f32(const float *g, int B, int C, int H, int W, long long gs_b, long long gs_c,
+                               long long gs_y, long long gs_x, void *hi, void *lo, unsigned *amax, int per_image,
+                               c2m_stream_t stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    C2M_CUDA(cudaMemsetAsync(amax, 0, sizeof(unsigned), st));
+    C2M_CUDA(cudaMemsetAsync(amax, 0, (per_image ? B : 1) * sizeof(unsigned), st));
     const long long n = (long long)C * H * W;
     const int ba = (int)((n + 255) / 256 < 1024 ? (n + 255) / 256 : 1024);
-    grad_amax_kernel<<<dim3(ba, B), 256, 0, st>>>(g, C, H, W, gs_b, gs_c, gs_y, gs_x, amax);
+    grad_amax_kernel<<<dim3(ba, B), 256, 0, st>>>(g, C, H, W, gs_b, gs_c, gs_y, gs_x, amax, per_image);
     C2M_LAUNCH_CHECK("grad_amax_kernel");
     const int C8 = (C + 7) / 8;
     const long long np = (long long)C8 * H * W;
     const int bx = (int)((np + 255) / 256 < 4096 ? (np + 255) / 256 : 4096);
-    psa_from_f32_kernel<<<dim3(bx, B), 256, 0, st>>>(g, C, C8, H, W, gs_b, gs_c, gs_y, gs_x, 0, amax,
+    psa_from_f32_kernel<<<dim3(bx, B), 256, 0, st>>>(g, C, C8, H, W, gs_b, gs_c, gs_y, gs_x, 0, amax, per_image,
                                                      reinterpret_cast<__half *>(hi), reinterpret_cast<__half *>(lo));
     C2M_LAUNCH_CHECK("psa_from_f32_kernel");
     return C2M_OK;
+}
+
+}  // namespace c2m
+
+extern "C" int c2m_grad_psa_from_f32(const float *g, int B, int C, int H, int W, long long gs_b, long long gs_c,
+                                     long long gs_y, long long gs_x, void *hi, void *lo, unsigned *amax,
+                                     c2m_stream_t stream) {
+    C2M_CHECK_ARG(g && hi && lo && amax && B > 0 && C > 0 && H > 0 && W > 0, "grad_psa_from_f32: bad argument");
+    return scaled_psa_from_f32(g, B, C, H, W, gs_b, gs_c, gs_y, gs_x, hi, lo, amax, 0, stream);
+}
+
+extern "C" int c2m_conv3x3_operand_f32(const float *x, int B, int C, int H, int W, long long xs_b, long long xs_c,
+                                       long long xs_y, long long xs_x, void *hi, void *lo, unsigned *amax,
+                                       c2m_stream_t stream) {
+    C2M_CHECK_ARG(x && hi && lo && amax && B > 0 && C > 0 && H > 0 && W > 0, "conv3x3_operand_f32: bad argument");
+    return scaled_psa_from_f32(x, B, C, H, W, xs_b, xs_c, xs_y, xs_x, hi, lo, amax, 1, stream);
 }
 
 extern "C" int c2m_grad_unscale_f32(float *x, long long n, const unsigned *amax, c2m_stream_t stream) {
@@ -245,14 +307,16 @@ extern "C" size_t c2m_conv3x3_wgrad_workspace_bytes(int B, int Cin, int Cout, in
     return wgrad_ws_bytes(g.ksplit, g.nslice * WG_CO, 9 * g.nchunk * WG_CI);
 }
 
-extern "C" int c2m_conv3x3_wgrad(const void *gy_hi, const void *gy_lo, const unsigned *gy_amax, const void *x_hi,
-                                 const void *x_lo, int B, int Cin, int Cout, int H, int W, float *dw, void *ws,
-                                 size_t ws_bytes, c2m_stream_t stream) {
+// x_amax null: X is PSA at scale exponent 0
+static int conv3x3_wgrad(const void *gy_hi, const void *gy_lo, const unsigned *gy_amax, const void *x_hi,
+                         const void *x_lo, const unsigned *x_amax, int B, int Cin, int Cout, int H, int W, float *dw,
+                         void *ws, size_t ws_bytes, c2m_stream_t stream) {
     C2M_CHECK_ARG(gy_hi && gy_lo && gy_amax && x_hi && x_lo && dw, "conv3x3_wgrad: null pointer");
     C2M_CHECK_ARG(B > 0 && Cin > 0 && Cout > 0, "conv3x3_wgrad: bad shape");
     C2M_CHECK_ARG(H >= X_R && W >= X_C, "conv3x3_wgrad: map %dx%d smaller than one halo tile (18x10)", H, W);
     WgradGeom g;
     if (const int rc = wgrad_geom(B, Cin, Cout, H, W, g)) return rc;
+    g.x_amax = x_amax;
     const int co_pad = g.nslice * WG_CO, ci_pad = g.nchunk * WG_CI;
     const size_t need = wgrad_ws_bytes(g.ksplit, co_pad, 9 * ci_pad);
     if (!ws || ws_bytes < need) {
@@ -269,10 +333,29 @@ extern "C" int c2m_conv3x3_wgrad(const void *gy_hi, const void *gy_lo, const uns
     C2M_CUDA(cudaFuncSetAttribute(conv3x3_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WG_SMEM));
     const int grid = g.nslice * g.nchunk * g.ksplit;
     float *part = reinterpret_cast<float *>(ws);
+    // algorithmic work: 2 * Cin * Cout * 9 flops per pixel; bytes = the two PSA operands (4 B / element) + dW
+    const double px = (double)B * H * W;
+    void *ph = prof_begin(PROF_CONV3X3_WGRAD, 2.0 * Cin * Cout * 9.0 * px, 4.0 * px * (Cin + Cout) + 36.0 * Cin * Cout,
+                          st);
     conv3x3_wgrad_kernel<<<grid, 384, WG_SMEM, st>>>(mgh, mgl, mxh, mxl, g, part);
     C2M_LAUNCH_CHECK("conv3x3_wgrad_kernel");
+    prof_end(ph, st);
     wgrad_reduce_kernel<<<grid_blocks((long long)Cout * 9 * ci_pad), 256, 0, st>>>(part, g.ksplit, Cin, Cout, ci_pad,
                                                                                 co_pad, 9 * ci_pad, gy_amax, dw);
     C2M_LAUNCH_CHECK("wgrad_reduce_kernel");
     return C2M_OK;
+}
+
+extern "C" int c2m_conv3x3_wgrad(const void *gy_hi, const void *gy_lo, const unsigned *gy_amax, const void *x_hi,
+                                 const void *x_lo, int B, int Cin, int Cout, int H, int W, float *dw, void *ws,
+                                 size_t ws_bytes, c2m_stream_t stream) {
+    return conv3x3_wgrad(gy_hi, gy_lo, gy_amax, x_hi, x_lo, nullptr, B, Cin, Cout, H, W, dw, ws, ws_bytes, stream);
+}
+
+extern "C" int c2m_conv3x3_wgrad_scaled(const void *gy_hi, const void *gy_lo, const unsigned *gy_amax,
+                                        const void *x_hi, const void *x_lo, const unsigned *x_amax, int B, int Cin,
+                                        int Cout, int H, int W, float *dw, void *ws, size_t ws_bytes,
+                                        c2m_stream_t stream) {
+    C2M_CHECK_ARG(x_amax, "conv3x3_wgrad_scaled: null x_amax");
+    return conv3x3_wgrad(gy_hi, gy_lo, gy_amax, x_hi, x_lo, x_amax, B, Cin, Cout, H, W, dw, ws, ws_bytes, stream);
 }

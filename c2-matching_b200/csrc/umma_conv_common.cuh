@@ -78,14 +78,25 @@ __device__ __forceinline__ void wgmma_tt_split(float (&acc)[16], uint64_t a_hi, 
     wgmma_tt_n32(acc, a_lo, b_hi);
 }
 
-// Gradient scale exponent: sg = 14 - floor(log2 amax) (amax * 2^sg in [2^14, 2^15)), from the bits of the largest finite
-// |grad_output|; 0 for an all-zero gradient, clamped to +-120 so that 2^sg and 2^-sg are normal floats.
-__host__ __device__ __forceinline__ int grad_scale_exp(const unsigned *amax) {
-    const unsigned bits = *amax;
+// Per-image operand exponents of the tensor-core DCN kernels' fp32 boundary (dcn_umma.cu, dcn_tc_bwd.cu), from the bits of the image's largest finite magnitude (0 -> 0).
+// x: amax * 2^s in [2^11, 2^12), under fp16's 65504 with 16x headroom for the blend and well above its subnormals.
+// mask: max |mask| * 2^s in [1, 2), so the corner weights are at most 2.  Exponent arithmetic only: scaling an image
+// by 2^k shifts its exponent by -k and leaves the operand bit for bit the same.  Each exponent is clamped to +-120, so
+// 2^sa and 2^sm are normal floats.  Their sum with the weight exponent sw is not clamped: the epilogue's
+// 2^-(sa + sm + sw) leaves fp32's range (flushing the output to 0 or overflowing it) only when it exceeds 149 or
+// drops below -127.  Since amax(x) 2^sa is in [2^11, 2^12), amax(mask) 2^sm in [1, 2) and amax(w) 2^sw in
+// [2^13, 2^14), that happens only when amax(x) amax(mask) amax(w) is below 2^-121 or above 2^151: outputs at the
+// edge of fp32's range whatever computes them.
+__host__ __device__ __forceinline__ int amax_exp(unsigned bits, int top) {
     if (bits == 0u) return 0;
-    const int s = 14 - ((int)(bits >> 23) - 127);
+    const int e = (int)(bits >> 23) - 127;            // floor(log2 amax); a subnormal amax counts as 2^-127
+    const int s = top - e;
     return s < -120 ? -120 : s > 120 ? 120 : s;
 }
+// Gradient scale exponent: sg = 14 - floor(log2 amax) (amax * 2^sg in [2^14, 2^15)), from the bits of the largest finite
+// |grad_output|; 0 for an all-zero gradient, clamped to +-120 so that 2^sg and 2^-sg are normal floats.  The plain
+// convolution's per-image input exponents (c2m_conv3x3_operand_f32) are the same function of each image's amax.
+__host__ __device__ __forceinline__ int grad_scale_exp(const unsigned *amax) { return amax_exp(*amax, 14); }
 
 // ---- Split-K weight gradients (conv3x3_wgrad.cu, dcn_tc_bwd.cu).  dW is a GEMM with M = Cout and K = every pixel of
 // the batch.  The pixel tiles are cut into ksplit contiguous K ranges; the CTAs of range k write their fp32 partials
@@ -133,29 +144,21 @@ __device__ __forceinline__ void wgrad_flush(float (&acc)[NA][16], float *blk, in
 __global__ void wgrad_reduce_kernel(const float *__restrict__ ws, int nslots, int C, int Cout, int cpg, int co_pad,
                                     int ncol, const unsigned *__restrict__ gy_amax, float *__restrict__ dw);
 
-// Per-image operand exponents of the tensor-core DCN kernels' fp32 boundary (dcn_umma.cu, dcn_tc_bwd.cu), from the bits of the image's largest finite magnitude (0 -> 0).
-// x: amax * 2^s in [2^11, 2^12), under fp16's 65504 with 16x headroom for the blend and well above its subnormals.
-// mask: max |mask| * 2^s in [1, 2), so the corner weights are at most 2.  Exponent arithmetic only: scaling an image
-// by 2^k shifts its exponent by -k and leaves the operand bit for bit the same.  Each exponent is clamped to +-120, so
-// 2^sa and 2^sm are normal floats.  Their sum with the weight exponent sw is not clamped: the epilogue's
-// 2^-(sa + sm + sw) leaves fp32's range (flushing the output to 0 or overflowing it) only when it exceeds 149 or
-// drops below -127.  Since amax(x) 2^sa is in [2^11, 2^12), amax(mask) 2^sm in [1, 2) and amax(w) 2^sw in
-// [2^13, 2^14), that happens only when amax(x) amax(mask) amax(w) is below 2^-121 or above 2^151: outputs at the
-// edge of fp32's range whatever computes them.
-__host__ __device__ __forceinline__ int amax_exp(unsigned bits, int top) {
-    if (bits == 0u) return 0;
-    const int e = (int)(bits >> 23) - 127;            // floor(log2 amax); a subnormal amax counts as 2^-127
-    const int s = top - e;
-    return s < -120 ? -120 : s > 120 ? 120 : s;
-}
 __device__ __forceinline__ int operand_exp(const unsigned *amax, int b) { return amax ? amax_exp(amax[b], 11) : 0; }
 __device__ __forceinline__ int mask_exp(const unsigned *amax, int b) { return amax ? amax_exp(amax[b], 0) : 0; }
 
-// fp32 [B,C,H,W] (element strides) -> PSA x * 2^sa, or x * 2^grad_scale_exp(amax) when amax is not null
+// fp32 [B,C,H,W] (element strides) -> PSA x * 2^sa, or, when amax is not null, image b times
+// 2^grad_scale_exp(amax + b * amax_step): one exponent for the batch (amax_step 0) or one per image (1)
 // (conv3x3_umma.cu; grid (blocks, B))
 __global__ void psa_from_f32_kernel(const float *__restrict__ x, int C, int C8, int H, int W, long long xs_b,
                                     long long xs_c, long long xs_y, long long xs_x, int sa,
-                                    const unsigned *__restrict__ amax, __half *__restrict__ hi, __half *__restrict__ lo);
+                                    const unsigned *__restrict__ amax, int amax_step, __half *__restrict__ hi,
+                                    __half *__restrict__ lo);
+// Largest finite |g| of a strided [B,C,H,W] tensor as fp32 bits (NaN and Inf do not set the scale), of the whole batch
+// into amax[0] (amax_step 0) or image by image into amax[b] (1); the outputs start at 0 (conv3x3_wgrad.cu; grid
+// (blocks, B))
+__global__ void grad_amax_kernel(const float *__restrict__ g, int C, int H, int W, long long s_b, long long s_c,
+                                 long long s_y, long long s_x, unsigned *__restrict__ amax, int amax_step);
 
 struct ConvParams {
     int B, H, W;
@@ -185,6 +188,7 @@ struct ConvPtrs {
     __half *out_hi, *out_lo;
     float *out_f32;
     const float *add_f32;
+    const unsigned *x_amax;   // [B] or null: image b's input is x * 2^grad_scale_exp(x_amax + b), not x * 2^sa_in
 };
 
 // One thread = one output pixel; `acc` points at that pixel's row of the staged accumulator.

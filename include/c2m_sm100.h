@@ -53,7 +53,8 @@ enum {
 int c2m_abi_version(void);      /* 6 since the fp32 c2m_dcn_v2_* twins of c2m_deform_conv_* are gone (5: c2m_dcn_tc_args
                                  * takes only x_il; 4: .x_il / c2m_psa_interleave; 3: .mask; 2: out_f32_octets /
                                  * om_octets).  Later additions (c2m_dcn_tc_args.x_amax / .mask_amax,
-                                 * c2m_dcn_tc_operand_*) come with new symbols that an older library lacks. */
+                                 * c2m_dcn_tc_operand_*, c2m_conv3x3_args.x_amax with c2m_conv3x3_operand_f32 and
+                                 * c2m_conv3x3_wgrad_scaled) come with new symbols that an older library lacks. */
 const char *c2m_last_error(void);
 
 /* --- correlation / index_map --------------------------------------------------------------
@@ -178,6 +179,9 @@ typedef struct {
     void *out_hi, *out_lo; int sa_out; int pixel_shuffle;
     float *out_f32; const float *add_f32; long long os_b, os_c, os_y, os_x;
     int out_f32_octets;
+    const unsigned *x_amax;     /* [B] or NULL (then sa_in applies): per-image input exponents, the amax written by
+                                 * c2m_conv3x3_operand_f32 together with in_hi / in_lo; the epilogue divides image b by
+                                 * 2^(14 - floor(log2 x_amax[b])) (0 for an all-zero image).  One input only. */
 } c2m_conv3x3_args;
 
 size_t c2m_conv3x3_packed_weight_bytes(int Cin, int Cout);
@@ -187,6 +191,13 @@ int c2m_psa_from_f32(const float *x, int B, int C, int H, int W, long long xs_b,
 int c2m_psa_to_f32(const void *hi, const void *lo, int B, int C, int H, int W, int sa, const float *add, float *out,
                    long long os_b, long long os_c, long long os_y, long long os_x, c2m_stream_t stream);
 int c2m_conv3x3(const c2m_conv3x3_args *args, c2m_stream_t stream);
+/* Operand of the differentiable convolution: x [B,C,H,W] fp32 (element strides) of any magnitude -> PSA hi / lo holding
+ * image b times 2^sa_b, sa_b = 14 - floor(log2 amax[b]), where amax[b], the largest finite |x| of image b (NaN and Inf
+ * do not count; 0 gives sa_b = 0; sa_b is clamped to +-120), is computed on the device and its fp32 bits stored in
+ * amax[0, B) (device memory).  Pass amax as c2m_conv3x3_args.x_amax and to c2m_conv3x3_wgrad_scaled.  Scaling an image by
+ * 2^k leaves its PSA planes bit for bit the same, so the output and dW scale by exactly 2^k while in range. */
+int c2m_conv3x3_operand_f32(const float *x, int B, int C, int H, int W, long long xs_b, long long xs_c, long long xs_y,
+                            long long xs_x, void *hi, void *lo, unsigned *amax, c2m_stream_t stream);
 /* Backward of the convolution above (3x3 / stride 1 / pad 1, one input), fp32-grade, no host synchronisation.
  * c2m_grad_psa_from_f32: grad_output g [B,C,H,W] fp32 (element strides) -> PSA hi / lo holding g * 2^sg, where
  *   sg = 14 - floor(log2 amax) and amax, the largest finite |g| (NaN and Inf do not count; 0 gives sg = 0; sg is
@@ -197,7 +208,8 @@ int c2m_conv3x3(const c2m_conv3x3_args *args, c2m_stream_t stream);
  *   c2m_grad_unscale_f32 on that output: x[i] *= 2^-sg for n elements.
  * c2m_conv3x3_wgrad: dW[co][ci][ky][kx] = sum over b, y, x of g[b,co,y,x] * x[b,ci,y+ky-1,x+kx-1] (zero outside the
  *   map), written to dw [Cout,Cin,3,3] fp32.  gy_* / gy_amax: the output of c2m_grad_psa_from_f32; x_*: the forward's
- *   input as PSA at scale exponent 0.  Split-K over CTAs with per-CTA partials in `ws` (at least
+ *   input as PSA at scale exponent 0 (c2m_conv3x3_wgrad) or, with x_amax, the output of c2m_conv3x3_operand_f32
+ *   (c2m_conv3x3_wgrad_scaled).  Only pixels inside the map contribute, also next to a non-finite x.  Split-K over CTAs with per-CTA partials in `ws` (at least
  *   c2m_conv3x3_wgrad_workspace_bytes(B, Cin, Cout, H, W) bytes, which depends on the device's SM count), summed in one
  *   fixed order: the same bits on every run on a given device.  Needs H >= 18 and W >= 10, like c2m_conv3x3.
  */
@@ -208,6 +220,9 @@ size_t c2m_conv3x3_wgrad_workspace_bytes(int B, int Cin, int Cout, int H, int W)
 int c2m_conv3x3_wgrad(const void *gy_hi, const void *gy_lo, const unsigned *gy_amax, const void *x_hi, const void *x_lo,
                       int B, int Cin, int Cout, int H, int W, float *dw, void *ws, size_t ws_bytes,
                       c2m_stream_t stream);
+int c2m_conv3x3_wgrad_scaled(const void *gy_hi, const void *gy_lo, const unsigned *gy_amax, const void *x_hi,
+                             const void *x_lo, const unsigned *x_amax, int B, int Cin, int Cout, int H, int W,
+                             float *dw, void *ws, size_t ws_bytes, c2m_stream_t stream);
 /* MaxPool2d(2, 2) on a PSA tensor (floor semantics: odd trailing row / column dropped), PSA result. */
 int c2m_psa_maxpool2(const void *hi, const void *lo, int B, int C, int H, int W, void *out_hi, void *out_lo,
                      c2m_stream_t stream);

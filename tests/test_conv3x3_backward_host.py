@@ -44,6 +44,33 @@ def test_backward_entry_points_validate_arguments(lib):
                 'c2m_grad_unscale_f32')) <= set(_lib.SYMBOLS)
 
 
+def test_per_image_entry_points_validate_arguments(lib):
+    """c2m_conv3x3_operand_f32 and c2m_conv3x3_wgrad_scaled reject null pointers and empty shapes with status 1 and a
+    message, and per-image input exponents are refused for a concatenated input."""
+    from c2m_b200 import _lib
+    p = ctypes.c_void_p(16)
+    for args in ((None, 1, 8, 18, 10, 0, 0, 0, 0, p, p, p), (p, 1, 8, 18, 10, 0, 0, 0, 0, None, p, p),
+                 (p, 1, 8, 18, 10, 0, 0, 0, 0, p, None, p), (p, 1, 8, 18, 10, 0, 0, 0, 0, p, p, None),
+                 (p, 0, 8, 18, 10, 0, 0, 0, 0, p, p, p), (p, 1, 0, 18, 10, 0, 0, 0, 0, p, p, p),
+                 (p, 1, 8, 0, 10, 0, 0, 0, 0, p, p, p), (p, 1, 8, 18, 0, 0, 0, 0, 0, p, p, p)):
+        assert lib.c2m_conv3x3_operand_f32(*args, None) == 1
+        assert b'conv3x3_operand_f32: bad argument' in lib.c2m_last_error()
+    assert lib.c2m_conv3x3_wgrad_scaled(p, p, p, p, p, None, 1, 8, 8, 18, 10, p, p, 1 << 20, None) == 1
+    assert b'null x_amax' in lib.c2m_last_error()
+    assert lib.c2m_conv3x3_wgrad_scaled(p, p, p, p, None, p, 1, 8, 8, 18, 10, p, p, 1 << 20, None) == 1
+    assert b'null pointer' in lib.c2m_last_error()
+    assert lib.c2m_conv3x3_wgrad_scaled(p, p, p, p, p, p, 0, 8, 8, 18, 10, p, p, 1 << 20, None) == 1
+    assert b'bad shape' in lib.c2m_last_error()
+    assert lib.c2m_conv3x3_wgrad_scaled(p, p, p, p, p, p, 1, 8, 8, 18, 9, p, p, 1 << 20, None) == 1
+    assert b'smaller than one halo tile' in lib.c2m_last_error()
+    a = _lib.ConvArgs()
+    a.in_hi = a.in_lo = a.in2_hi = a.in2_lo = a.packed_w = a.out_f32 = a.x_amax = 16
+    a.Cin, a.Cin2, a.B, a.H, a.W, a.Cout = 32, 8, 1, 18, 10, 8
+    assert lib.c2m_conv3x3(ctypes.addressof(a), None) == 1
+    assert b'single input' in lib.c2m_last_error()
+    assert {'c2m_conv3x3_operand_f32', 'c2m_conv3x3_wgrad_scaled'} <= set(_lib.SYMBOLS)
+
+
 def test_invalidate_packs_drops_the_dgrad_pack():
     from c2m_b200 import ops
     conv = torch.nn.Conv2d(8, 4, 3, 1, 1)

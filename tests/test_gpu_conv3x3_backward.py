@@ -147,9 +147,10 @@ def _guards_intact(buf, dtype):
 
 @pytest.mark.parametrize('case', [(2, 40, 72, 19, 11, None), (1, 64, 64, 130, 70, None), (3, 3, 3, 18, 10, None)],
                          ids=_ids)
-def test_backward_writes_stay_in_bounds(case):
-    """Every buffer the backward's entry points write (the PSA gradient, its amax, dW, the workspace, the unscaled dX)
-    sits between sentinel guards that must come back untouched; the results must equal the op's."""
+def test_backward_with_image_exponents_writes_stay_in_bounds(case):
+    """Every buffer the backward's entry points write (the PSA gradient, its amax, dW from the forward's per-image
+    operand through c2m_conv3x3_wgrad_scaled, the workspace, the unscaled dX) sits between sentinel guards that must
+    come back untouched; the results must equal the op's."""
     from c2m_b200 import _lib, ops
     B, cin, cout, H, W, _ = case
     x, w, b, gy = _inputs(case, 400)
@@ -163,15 +164,16 @@ def test_backward_writes_stay_in_bounds(case):
     rc = L.c2m_grad_psa_from_f32(gy.data_ptr(), B, cout, H, W, *gy.stride(), ghi[GUARD:].data_ptr(),
                                  glo[GUARD:].data_ptr(), amax[GUARD:].data_ptr(), st)
     _lib.check(rc, 'c2m_grad_psa_from_f32')
-    xp = ops.psa_from_f32(x)
+    xp, x_amax = ops._conv3x3_operand(x)
     assert xp.hi.numel() == B * c8i * H * W * 8
     nws = L.c2m_conv3x3_wgrad_workspace_bytes(B, cin, cout, H, W)
     ws = _guarded(nws // 4, torch.float32)
     dw = _guarded(cout * cin * 9, torch.float32)
-    rc = L.c2m_conv3x3_wgrad(ghi[GUARD:].data_ptr(), glo[GUARD:].data_ptr(), amax[GUARD:].data_ptr(),
-                             xp.hi.data_ptr(), xp.lo.data_ptr(), B, cin, cout, H, W, dw[GUARD:].data_ptr(),
+    rc = L.c2m_conv3x3_wgrad_scaled(ghi[GUARD:].data_ptr(), glo[GUARD:].data_ptr(), amax[GUARD:].data_ptr(),
+                             xp.hi.data_ptr(), xp.lo.data_ptr(), x_amax.data_ptr(), B, cin, cout, H, W,
+                             dw[GUARD:].data_ptr(),
                              ws[GUARD:].data_ptr(), nws, st)
-    _lib.check(rc, 'c2m_conv3x3_wgrad')
+    _lib.check(rc, 'c2m_conv3x3_wgrad_scaled')
     dxs = _guarded(x.numel(), torch.float32)
     gp = ops.PSA(ghi[GUARD:GUARD + npsa].view(B, c8o, H, W, 8), glo[GUARD:GUARD + npsa].view(B, c8o, H, W, 8),
                  B, cout, H, W)
@@ -190,17 +192,21 @@ def test_backward_writes_stay_in_bounds(case):
 
 
 @pytest.mark.parametrize('bad', ['nan', 'inf', '-inf'])
-def test_non_finite_grad_output_reaches_every_dependent_gradient(bad):
+@pytest.mark.parametrize('where', [(0, 12), (20, 6), (9, 12), (20, 12)], ids=['corner', 'last_row', 'last_col',
+                                                                             'last_corner'])
+def test_non_finite_grad_output_reaches_every_dependent_gradient(bad, where):
+    """NaN / +-Inf in grad_output at a corner, in the last row or column of a 21 x 13 map (neither a multiple of the
+    16 x 8 tile), plus an interior pixel: the finiteness patterns of dX, dW and db equal the fp64 reference's."""
+    import conv3x3_ref
     case = (2, 40, 24, 21, 13, None)
     x, w, b, gy = _inputs(case, 500)
-    gy[1, 5, 0, 12] = float(bad)                 # a corner: its taps reach outside the map
+    gy[1, 5, where[0], where[1]] = float(bad)
     gy[0, 17, 9, 6] = float(bad)
     _, dx, dw, db = _tc_grads(x, w, b, None, gy)
-    want = _grads_of(x.double(), w.double(), gy.double())
+    want = conv3x3_ref.conv3x3_grads(x, w, gy)
     for name, got, ref in zip(('dX', 'dW', 'db'), (dx, dw, db), want):
-        nonfinite = ~torch.isfinite(ref)
-        assert bool(nonfinite.any()), name
-        assert not bool(torch.isfinite(got[nonfinite]).any()), name
+        assert bool((~torch.isfinite(ref)).any()), name
+        assert torch.equal(torch.isfinite(got), torch.isfinite(ref)), name
 
 
 def test_restoration_net_training_step_matches_cudnn(monkeypatch):

@@ -165,6 +165,9 @@ def test_nonfinite_pattern_matches_oracle(where):
     t = {'x': x, 'offset': off, 'grad_output': gy}[where]
     t.view(-1)[5] = float('nan')
     t.view(-1)[t.numel() // 2 + 3] = float('inf')
+    H, W = case[3], case[4]
+    t[0, 7, H - 1, W - 1] = float('-inf')          # the last row and column of the map
+    t[1, 2, H - 1, W // 2] = float('nan')
     _, *mine = _tc(x, off, mask, w, b, gy)
     ref = c_oracle.dcn_v2_backward(x.cpu().double(), w.cpu().double(), b.cpu().double(), off.cpu().double(),
                                    mask.cpu().double(), gy.cpu().double(), dg=8)

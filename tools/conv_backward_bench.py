@@ -71,7 +71,7 @@ def shape_times(cin, cout, H, iters, warmup):
     w = torch.randn(cout, cin, 3, 3, device=dev, generator=g) / (3 * cin ** 0.5)
     gy = torch.randn(B, cout, H, H, device=dev, generator=g) * 2.0 ** -19
     st = torch.cuda.current_stream().cuda_stream
-    xp = ops.psa_from_f32(x)
+    xp, x_amax = ops._conv3x3_operand(x)
     gp = ops.PSA.empty(B, cout, H, H, dev)
     amax = torch.empty(1, dtype=torch.int32, device=dev)
     wt = w.transpose(0, 1)
@@ -90,8 +90,8 @@ def shape_times(cin, cout, H, iters, warmup):
         _lib.check(L.c2m_grad_unscale_f32(dx.data_ptr(), dx.numel(), amax.data_ptr(), st), 'unscale')
 
     def tc_dw():
-        _lib.check(L.c2m_conv3x3_wgrad(gp.hi.data_ptr(), gp.lo.data_ptr(), amax.data_ptr(), xp.hi.data_ptr(),
-                                       xp.lo.data_ptr(), B, cin, cout, H, H, dw.data_ptr(), ws.data_ptr(), nws, st),
+        _lib.check(L.c2m_conv3x3_wgrad_scaled(gp.hi.data_ptr(), gp.lo.data_ptr(), amax.data_ptr(), xp.hi.data_ptr(),
+                                       xp.lo.data_ptr(), x_amax.data_ptr(), B, cin, cout, H, H, dw.data_ptr(), ws.data_ptr(), nws, st),
                    'wgrad')
 
     def cudnn_dx():
