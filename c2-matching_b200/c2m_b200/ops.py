@@ -2,12 +2,18 @@
 grouped deformable convolution entries); outputs are
 allocated here with torch (caller-owned in ABI terms) and raw pointers + the current stream
 are handed to the library."""
+import ctypes
+import math
+import os
+import weakref
+
 import torch
 
 from . import _lib
 from ._lib import DcnShape
 
 _ws_cache = {}
+_DTYPE_SFX = {torch.float32: 'f32', torch.float64: 'f64'}      # entry-point suffix of each dtype
 
 
 def _require_cuda(name, t, dtype=torch.float32):
@@ -24,6 +30,42 @@ def _stream():
     return torch.cuda.current_stream().cuda_stream
 
 
+def _ptr(t):
+    return None if t is None else t.data_ptr()
+
+
+def _call(name, *args, device=None):
+    """Runs the entry point `name` with `device` current (None: as it is) on that device's current stream, which goes
+    in as the last argument: tensors go in as their data pointers, None, numbers and ctypes structs as given.  The
+    symbol is looked up on every call, so that a wrapper set on the library object sees it; a nonzero status raises
+    C2MError."""
+    if device is not None:
+        with torch.cuda.device(device):
+            return _call(name, *args)
+    fn = getattr(_lib.lib(), name)
+    _lib.check(fn(*[a.data_ptr() if isinstance(a, torch.Tensor) else a for a in args], _stream()), name)
+
+
+def _size(name, *args):
+    """The byte count the size query `name` returns; 0 (a bad shape) raises C2MError."""
+    return _lib.check_size(getattr(_lib.lib(), name)(*args), name)
+
+
+def _memory_format(channels_last):
+    return torch.channels_last if channels_last else torch.contiguous_format
+
+
+def _empty_f32(B, C, H, W, device, channels_last=False):
+    return torch.empty(B, C, H, W, dtype=torch.float32, device=device, memory_format=_memory_format(channels_last))
+
+
+def _one_or_both(psa, f32):
+    """(psa, f32) when both outputs were made, else the one that was."""
+    if psa is not None and f32 is not None:
+        return psa, f32
+    return psa if psa is not None else f32
+
+
 def launch_count():
     return int(_lib.lib().c2m_launch_count())
 
@@ -37,7 +79,6 @@ PROF_KERNELS = {'corr_search': 0, 'conv3x3': 1, 'dcn': 2, 'dcn_dgrad': 3, 'dcn_w
 
 def profile_collect(kernel):
     """{'ms', 'launches', 'flops', 'bytes'} of one kernel class since the last collect."""
-    import ctypes
     ms, n, fl, by = ctypes.c_float(0), ctypes.c_int(0), ctypes.c_double(0), ctypes.c_double(0)
     _lib.check(_lib.lib().c2m_profile_collect(PROF_KERNELS[kernel], ctypes.byref(ms), ctypes.byref(n),
                                               ctypes.byref(fl), ctypes.byref(by)), 'c2m_profile_collect')
@@ -71,27 +112,23 @@ def _det_workspace(query, shape, nplanes, device):
     """Workspace for an ordered gather: as many planes per pass as fit in DET_WORKSPACE_CAP, at least one.  Call with
     `device` current (the size query asks CUB, which reads the current device)."""
     global det_workspace_peak
-    one = _lib.check_size(query(shape, 1), 'ordered input gradient')
+    one = _size(query, shape, 1)
     planes = max(1, min(nplanes, DET_WORKSPACE_CAP // one))
-    nbytes = _lib.check_size(query(shape, planes), 'ordered input gradient') if planes > 1 else one
+    nbytes = _size(query, shape, planes) if planes > 1 else one
     det_workspace_peak = max(det_workspace_peak, int(nbytes))
     return torch.empty(int(nbytes), dtype=torch.uint8, device=device)
 
 
-def _col2im(sfx, gcol, offset, mask_ptr, s, x):
+def _col2im(sfx, gcol, offset, mask, s, x):
     """grad_input of the deformable convolution from gcol: the ordered gather when deterministic algorithms are on,
     else the atomic scatter into zeros."""
-    L = _lib.lib()
     if deterministic():
         grad_input = torch.empty_like(x)
-        ws = _det_workspace(L.c2m_dcn_col2im_det_workspace_bytes, s, s.B * s.dg, x.device)
-        fn = f'c2m_deform_conv_col2im_det_{sfx}'
-        _lib.check(getattr(L, fn)(gcol.data_ptr(), offset.data_ptr(), mask_ptr, s, grad_input.data_ptr(),
-                                  ws.data_ptr(), ws.numel(), _stream()), fn)
+        ws = _det_workspace('c2m_dcn_col2im_det_workspace_bytes', s, s.B * s.dg, x.device)
+        _call(f'c2m_deform_conv_col2im_det_{sfx}', gcol, offset, mask, s, grad_input, ws, ws.numel())
         return grad_input
     grad_input = torch.zeros_like(x)
-    fn = f'c2m_deform_conv_col2im_{sfx}'
-    _lib.check(getattr(L, fn)(gcol.data_ptr(), offset.data_ptr(), mask_ptr, s, grad_input.data_ptr(), _stream()), fn)
+    _call(f'c2m_deform_conv_col2im_{sfx}', gcol, offset, mask, s, grad_input)
     return grad_input
 
 
@@ -109,19 +146,14 @@ def corr_argmax(feat_in, feat_ref, patch_size=3, input_stride=1, ref_stride=1, i
     feat_ref = feat_ref.contiguous()
     B, C, h, w = feat_in.shape
     hr, wr = feat_ref.shape[2:]
-    L = _lib.lib()
     with torch.cuda.device(feat_in.device):
-        need = _lib.check_size(L.c2m_corr_workspace_bytes(B, C, h, w, hr, wr, patch_size, input_stride, ref_stride),
-                               'corr_argmax')
+        need = _size('c2m_corr_workspace_bytes', B, C, h, w, hr, wr, patch_size, input_stride, ref_stride)
         ws = _workspace(need, feat_in.device)
         gh, gw = (h - patch_size) // input_stride + 1, (w - patch_size) // input_stride + 1
         idx = torch.empty(B, gh, gw, dtype=torch.int64, device=feat_in.device)
         val = torch.empty(B, gh, gw, dtype=torch.float32, device=feat_in.device)
-        rc = L.c2m_corr_argmax_f32(feat_in.data_ptr(), feat_ref.data_ptr(), B, C, h, w, hr, wr, patch_size,
-                                   input_stride, ref_stride, int(is_norm), int(norm_input), int(l2norm),
-                                   1 if force_generic else 0, idx.data_ptr(), val.data_ptr(), ws.data_ptr(),
-                                   ws.numel(), _stream())
-        _lib.check(rc, 'c2m_corr_argmax_f32')
+        _call('c2m_corr_argmax_f32', feat_in, feat_ref, B, C, h, w, hr, wr, patch_size, input_stride, ref_stride,
+              int(is_norm), int(norm_input), int(l2norm), 1 if force_generic else 0, idx, val, ws, ws.numel())
     return idx, val
 
 
@@ -139,10 +171,7 @@ def offset_pyramid(idx, scale, ref_gw=None):
     idx = idx.contiguous()
     B, gh, gw = idx.shape
     out = torch.empty(B, 9, scale * (gh + 2), scale * (gw + 2), 2, dtype=torch.float32, device=idx.device)
-    with torch.cuda.device(idx.device):
-        rc = _lib.lib().c2m_offset_pyramid_f32(idx.data_ptr(), B, gh, gw, ref_gw or gw, scale, out.data_ptr(),
-                                               _stream())
-        _lib.check(rc, 'c2m_offset_pyramid_f32')
+    _call('c2m_offset_pyramid_f32', idx, B, gh, gw, ref_gw or gw, scale, out, device=idx.device)
     return out
 
 
@@ -165,6 +194,26 @@ def _shape(x, cout, kh, kw, sh, sw, ph, pw, dh, dw, dg, out):
 
 def _out_hw(H, W, kh, kw, sh, sw, ph, pw, dh, dw):
     return ((H + 2 * ph - (dh * (kh - 1) + 1)) // sh + 1, (W + 2 * pw - (dw * (kw - 1) + 1)) // sw + 1)
+
+
+def _deform_out(x, weight, offset, mask, geom, deformable_group, grad_output=None, nonempty=False):
+    """(Ho, Wo) of the deformable convolution of x [B, C, H, W] by weight [Cout, ...] with geom = (kh, kw, sh, sw, ph,
+    pw, dh, dw).  Refuses, in this order: an empty output (when nonempty), a grad_output (when given) that is not
+    [B, Cout, Ho, Wo], an offset that is not [B, 2*dg*kh*kw, Ho, Wo] or a mask (when given) that is not
+    [B, dg*kh*kw, Ho, Wo]."""
+    B, _, H, W = x.shape
+    Ho, Wo = _out_hw(H, W, *geom)
+    if nonempty and (Ho < 1 or Wo < 1):
+        raise RuntimeError(f'convolution input is too small (output would be {Ho} x {Wo})')
+    want = (B, weight.shape[0], Ho, Wo)
+    if grad_output is not None and tuple(grad_output.shape) != want:
+        raise RuntimeError(f'grad_output has shape {tuple(grad_output.shape)}, expected {want}')
+    T = geom[0] * geom[1]
+    if tuple(offset.shape) != (B, 2 * deformable_group * T, Ho, Wo) or (
+            mask is not None and tuple(mask.shape) != (B, deformable_group * T, Ho, Wo)):
+        raise RuntimeError(f'offset/mask shape mismatch: {tuple(offset.shape)}, '
+                           f'{None if mask is None else tuple(mask.shape)} for output {Ho}x{Wo}')
+    return Ho, Wo
 
 
 def _pre_offset_source(pre_offset, idx, B, taps, Ho, Wo):
@@ -191,22 +240,16 @@ def dcn_v2_forward(input, weight, bias, offset, mask, kernel_h, kernel_w, stride
                            f'{weight.shape[2]} x {weight.shape[3]}).')
     if input.shape[1] != weight.shape[1]:
         raise RuntimeError(f'Input shape and kernel channels wont match: ({input.shape[1]} vs {weight.shape[1]}).')
+    geom = (kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w)
     x = _dense_nchw_or_nhwc(input)
-    B, C, H, W = x.shape
-    Ho, Wo = _out_hw(H, W, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w)
-    T = kernel_h * kernel_w
-    if tuple(offset.shape) != (B, 2 * deformable_group * T, Ho, Wo) or tuple(mask.shape) != (B, deformable_group * T, Ho, Wo):
-        raise RuntimeError(f'offset/mask shape mismatch: {tuple(offset.shape)}, {tuple(mask.shape)} for output {Ho}x{Wo}')
-    import os
-    if ((kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w) == (3, 3, 1, 1, 1, 1, 1, 1) and
-            dcn_tc_supported(C, weight.shape[0], deformable_group) and os.environ.get('C2M_EXT_DCN_TC', '1') != '0'):
+    Ho, Wo = _deform_out(x, weight, offset, mask, geom, deformable_group)
+    if (geom == (3, 3, 1, 1, 1, 1, 1, 1) and dcn_tc_supported(x.shape[1], weight.shape[0], deformable_group) and
+            os.environ.get('C2M_EXT_DCN_TC', '1') != '0'):
         # eligible shapes (every DCN of C2-Matching) take the tensor-core kernel: fp32 NCHW -> packed-split operand
         # in one pass, final offsets / mask read as given, fp32 NCHW out.  The FFMA kernel below stays the general
         # path (any kernel size / stride / dilation / group width).
         return dcn_v2_fused_tc(x, offset.contiguous(), weight, bias, deformable_group, final_mask=mask.contiguous())
-    return _deform_forward(x, weight, offset, mask, bias, Ho, Wo,
-                           (kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w), 1,
-                           deformable_group)
+    return _deform_forward(x, weight, offset, mask, bias, Ho, Wo, geom, 1, deformable_group)
 
 
 def dcn_v2_fused_forward(x, om, weight, bias, deformable_group, pre_offset=None, idx=None, pre_scale=1,
@@ -222,18 +265,12 @@ def dcn_v2_fused_forward(x, om, weight, bias, deformable_group, pre_offset=None,
     Ho, Wo = _out_hw(H, W, kh, kw, 1, 1, kh // 2, kw // 2, 1, 1)
     if tuple(om.shape) != (B, 3 * deformable_group * kh * kw, Ho, Wo):
         raise RuntimeError(f'conv_offset_mask output has shape {tuple(om.shape)}')
-    mf = torch.channels_last if channels_last_out else torch.contiguous_format
-    out = torch.empty(B, weight.shape[0], Ho, Wo, dtype=torch.float32, device=x.device, memory_format=mf)
+    out = _empty_f32(B, weight.shape[0], Ho, Wo, x.device, channels_last_out)
     s = _shape(x, weight.shape[0], kh, kw, 1, 1, kh // 2, kw // 2, 1, 1, deformable_group, out)
     pre_offset, idx = _pre_offset_source(pre_offset, idx, B, kh * kw, Ho, Wo)
     gh, gw = idx.shape[1:] if idx is not None else (0, 0)
-    with torch.cuda.device(x.device):
-        rc = _lib.lib().c2m_dcn_v2_fused_forward_f32(
-            x.data_ptr(), om.data_ptr(), pre_offset.data_ptr() if pre_offset is not None else None,
-            idx.data_ptr() if idx is not None else None, gh, gw, ref_gw or gw, pre_scale,
-            weight.contiguous().data_ptr(), bias.contiguous().data_ptr() if bias is not None else None,
-            float(lrelu_slope), out.data_ptr(), s, _stream())
-        _lib.check(rc, 'c2m_dcn_v2_fused_forward_f32')
+    _call('c2m_dcn_v2_fused_forward_f32', x, om, pre_offset, idx, gh, gw, ref_gw or gw, pre_scale, weight.contiguous(),
+          bias.contiguous() if bias is not None else None, float(lrelu_slope), out, s, device=x.device)
     return out
 
 
@@ -279,7 +316,6 @@ class OctF32:
 def suggest_sa(amax, target_log2=12):
     """Scale exponent for a PSA tensor whose largest magnitude is `amax`: amax * 2^sa ~ 2^target_log2 (fp16 tops out
     at 65504 = 2^16, so 16x headroom; values below 2^-14 * 2^-sa lose their lo half to fp16 subnormals)."""
-    import math
     if not (amax > 0) or not math.isfinite(amax):
         return 0
     return max(-14, min(24, target_log2 - math.ceil(math.log2(amax))))
@@ -294,35 +330,30 @@ def psa_from_f32(x, sa=0):
     _require_cuda('x', x)
     B, C, H, W = x.shape
     out = PSA.empty(B, C, H, W, x.device, sa)
-    with torch.cuda.device(x.device):
-        rc = _lib.lib().c2m_psa_from_f32(x.data_ptr(), B, C, H, W, *x.stride(), sa, out.hi.data_ptr(),
-                                         out.lo.data_ptr(), _stream())
-        _lib.check(rc, 'c2m_psa_from_f32')
+    _call('c2m_psa_from_f32', x, B, C, H, W, *x.stride(), sa, out.hi, out.lo, device=x.device)
     return out
 
 
+def _strided_like(add, out, channels_last):
+    """`add` with the shape and strides of `out` (copied into the layout `channels_last` names when they differ)."""
+    if add.shape != out.shape or add.stride() != out.stride():
+        return add.contiguous(memory_format=_memory_format(channels_last))
+    return add
+
+
 def psa_to_f32(p, add=None, channels_last=False):
-    mf = torch.channels_last if channels_last else torch.contiguous_format
-    out = torch.empty(p.B, p.C, p.H, p.W, dtype=torch.float32, device=p.hi.device, memory_format=mf)
+    out = _empty_f32(p.B, p.C, p.H, p.W, p.hi.device, channels_last)
     if add is not None:
         _require_cuda('add', add)
-        if add.shape != out.shape or add.stride() != out.stride():
-            add = add.contiguous(memory_format=mf)
-    with torch.cuda.device(out.device):
-        rc = _lib.lib().c2m_psa_to_f32(p.hi.data_ptr(), p.lo.data_ptr(), p.B, p.C, p.H, p.W, p.sa,
-                                       add.data_ptr() if add is not None else None, out.data_ptr(), *out.stride(),
-                                       _stream())
-        _lib.check(rc, 'c2m_psa_to_f32')
+        add = _strided_like(add, out, channels_last)
+    _call('c2m_psa_to_f32', p.hi, p.lo, p.B, p.C, p.H, p.W, p.sa, add, out, *out.stride(), device=out.device)
     return out
 
 
 def psa_maxpool2(p):
     """nn.MaxPool2d(kernel_size=2, stride=2) on a PSA tensor."""
     out = PSA.empty(p.B, p.C, p.H // 2, p.W // 2, p.hi.device, p.sa)
-    with torch.cuda.device(p.hi.device):
-        rc = _lib.lib().c2m_psa_maxpool2(p.hi.data_ptr(), p.lo.data_ptr(), p.B, p.C, p.H, p.W, out.hi.data_ptr(),
-                                         out.lo.data_ptr(), _stream())
-        _lib.check(rc, 'c2m_psa_maxpool2')
+    _call('c2m_psa_maxpool2', p.hi, p.lo, p.B, p.C, p.H, p.W, out.hi, out.lo, device=p.hi.device)
     return out
 
 
@@ -343,7 +374,6 @@ def _pack_cached(weight, attr, extra, size_fn, pack_fn, dims, source=None):
     """The blob of `weight` cached under `attr` (one of _PACK_ATTRS), packed on a miss: size_fn(*dims) bytes filled by
     pack_fn(w, *dims, blob, stream), where w is source(weight) (default: the weight itself) made contiguous.  `extra`
     is part of the cache key."""
-    import weakref
     tag = (weight.data_ptr(), weight._version, tuple(weight.shape), extra)
     store = getattr(weight, '__dict__', None)
     if store is None:
@@ -362,12 +392,11 @@ def _pack_cached(weight, attr, extra, size_fn, pack_fn, dims, source=None):
             # an event recorded outside its capture; RestorationPipeline synchronises the device before it captures.)
             cur.wait_event(ev)
         return blob
-    L = _lib.lib()
     w = weight.detach()
     w = (source(w) if source else w).contiguous()
-    blob = torch.empty(getattr(L, size_fn)(*dims), dtype=torch.uint8, device=weight.device)
-    with torch.cuda.device(weight.device):
-        _lib.check(getattr(L, pack_fn)(w.data_ptr(), *dims, blob.data_ptr(), _stream()), pack_fn)
+    # unsupported dims size to 0 without an error message; the pack call then reports them
+    blob = torch.empty(getattr(_lib.lib(), size_fn)(*dims), dtype=torch.uint8, device=weight.device)
+    _call(pack_fn, w, *dims, blob, device=weight.device)
     ev = torch.cuda.Event()
     ev.record(cur)
     store[attr] = (tag, blob, ev, cur.cuda_stream)
@@ -428,9 +457,8 @@ def conv3x3_psa(x, weight, bias, act=None, residual=None, residual2=None, x2=Non
             raise RuntimeError('conv3x3_psa: concatenated inputs must share batch / size / scale')
         a.in2_hi, a.in2_lo, a.Cin2 = x2.hi.data_ptr(), x2.lo.data_ptr(), x2.C
     a.B, a.H, a.W, a.sa_in = x.B, x.H, x.W, x.sa
-    if x_amax is not None:
-        a.x_amax = x_amax.data_ptr()
-    a.packed_w, a.bias = blob.data_ptr(), (bias.data_ptr() if bias is not None else None)
+    a.x_amax = _ptr(x_amax)
+    a.packed_w, a.bias = blob.data_ptr(), _ptr(bias)
     a.Cout, a.act = cout, _ACT[act]
     for r, (fh, fl) in ((residual, ('res_hi', 'res_lo')), (residual2, ('res2_hi', 'res2_lo'))):
         if r is not None:
@@ -456,21 +484,14 @@ def conv3x3_psa(x, weight, bias, act=None, residual=None, residual2=None, x2=Non
         ret_f32 = OctF32(torch.empty(x.B, (cout + 7) // 8, x.H, x.W, 8, dtype=torch.float32, device=dev), cout)
         a.out_f32, a.out_f32_octets = ret_f32.data.data_ptr(), 1
     elif out_f32:
-        mf = torch.channels_last if channels_last else torch.contiguous_format
-        ret_f32 = torch.empty(x.B, cout, x.H, x.W, dtype=torch.float32, device=dev, memory_format=mf)
+        ret_f32 = _empty_f32(x.B, cout, x.H, x.W, dev, channels_last)
         a.out_f32 = ret_f32.data_ptr()
         a.os_b, a.os_c, a.os_y, a.os_x = ret_f32.stride()
         if add_f32 is not None:
-            if add_f32.shape != ret_f32.shape or add_f32.stride() != ret_f32.stride():
-                add_f32 = add_f32.contiguous(memory_format=mf)
+            add_f32 = _strided_like(add_f32, ret_f32, channels_last)
             a.add_f32 = add_f32.data_ptr()
-    import ctypes
-    with torch.cuda.device(dev):
-        rc = _lib.lib().c2m_conv3x3(ctypes.addressof(a), _stream())
-        _lib.check(rc, 'c2m_conv3x3')
-    if ret_psa is not None and ret_f32 is not None:
-        return ret_psa, ret_f32
-    return ret_psa if ret_psa is not None else ret_f32
+    _call('c2m_conv3x3', ctypes.addressof(a), device=dev)
+    return _one_or_both(ret_psa, ret_f32)
 
 
 def _grad_psa(gy):
@@ -479,8 +500,7 @@ def _grad_psa(gy):
     B, C, H, W = gy.shape
     gp = PSA.empty(B, C, H, W, gy.device)
     amax = torch.empty(1, dtype=torch.int32, device=gy.device)
-    _lib.check(_lib.lib().c2m_grad_psa_from_f32(gy.data_ptr(), B, C, H, W, *gy.stride(), gp.hi.data_ptr(),
-                                                gp.lo.data_ptr(), amax.data_ptr(), _stream()), 'c2m_grad_psa_from_f32')
+    _call('c2m_grad_psa_from_f32', gy, B, C, H, W, *gy.stride(), gp.hi, gp.lo, amax)
     return gp, amax
 
 
@@ -490,9 +510,7 @@ def _conv3x3_operand(x):
     B, C, H, W = x.shape
     xp = PSA.empty(B, C, H, W, x.device)
     amax = torch.empty(B, dtype=torch.int32, device=x.device)
-    _lib.check(_lib.lib().c2m_conv3x3_operand_f32(x.data_ptr(), B, C, H, W, *x.stride(), xp.hi.data_ptr(),
-                                                  xp.lo.data_ptr(), amax.data_ptr(), _stream()),
-               'c2m_conv3x3_operand_f32')
+    _call('c2m_conv3x3_operand_f32', x, B, C, H, W, *x.stride(), xp.hi, xp.lo, amax)
     return xp, amax
 
 
@@ -521,7 +539,6 @@ class _Conv3x3(torch.autograd.Function):
             gy = torch.where(y > 0, gy, 0.)
         elif ctx.act == 'lrelu':
             gy = torch.where(y > 0, gy, gy * 0.1)
-        L = _lib.lib()
         dev = gy.device
         dx = dw = db = None
         with torch.cuda.device(dev):
@@ -529,16 +546,13 @@ class _Conv3x3(torch.autograd.Function):
             if need_x:
                 dx = conv3x3_psa(gp, weight.transpose(0, 1), None, psa_out=False, out_f32=True,
                                  packed=conv3x3_pack_weights(weight, dgrad=True))
-                _lib.check(L.c2m_grad_unscale_f32(dx.data_ptr(), dx.numel(), amax.data_ptr(), _stream()),
-                           'c2m_grad_unscale_f32')
+                _call('c2m_grad_unscale_f32', dx, dx.numel(), amax)
             if need_w:
                 dw = torch.empty(cout, cin, 3, 3, dtype=torch.float32, device=dev)
-                nbytes = _lib.check_size(L.c2m_conv3x3_wgrad_workspace_bytes(B, cin, cout, H, W),
-                                         'c2m_conv3x3_wgrad_workspace_bytes')
+                nbytes = _size('c2m_conv3x3_wgrad_workspace_bytes', B, cin, cout, H, W)
                 ws = _workspace(nbytes, dev)
-                _lib.check(L.c2m_conv3x3_wgrad_scaled(gp.hi.data_ptr(), gp.lo.data_ptr(), amax.data_ptr(), x_hi.data_ptr(),
-                                               x_lo.data_ptr(), x_amax.data_ptr(), B, cin, cout, H, W, dw.data_ptr(),
-                                               ws.data_ptr(), nbytes, _stream()), 'c2m_conv3x3_wgrad_scaled')
+                _call('c2m_conv3x3_wgrad_scaled', gp.hi, gp.lo, amax, x_hi, x_lo, x_amax, B, cin, cout, H, W, dw, ws,
+                      nbytes)
             if need_b:
                 db = gy.sum((0, 2, 3))
         return dx, dw, db, None
@@ -579,12 +593,27 @@ def _dcn_tc_pack(weight, dg):
                         (c, cout, dg))
 
 
+def _dcn_tc_operand(x, dg, mask=None):
+    """The tensor-core DCN's interleaved operand x_il of x, with its x_amax and mask_amax buffers.  x is a PSA tensor at
+    scale exponent 0 (both buffers None) or fp32 [B,C,H,W], dense NCHW or channels-last, of any magnitude: x_il then
+    holds image b times 2^sa_b, x_amax its [B] exponents and, given the final mask [B,dg*9,H,W], mask_amax the mask's
+    (else None), all taken on the device.  Call with x's device current."""
+    B, C, H, W = x.shape
+    dev = x.hi.device if isinstance(x, PSA) else x.device
+    x_il = torch.empty(_lib.lib().c2m_dcn_tc_operand_bytes(B, C, H, W, dg) // 2, dtype=torch.float16, device=dev)
+    if isinstance(x, PSA):
+        _call('c2m_dcn_tc_operand_psa', x.hi, x.lo, B, C, H, W, dg, x_il)
+        return x_il, None, None
+    amax = torch.empty(2 * B, dtype=torch.int32, device=dev)
+    _call('c2m_dcn_tc_operand_f32', x, B, C, H, W, *x.stride(), dg, mask, x_il, amax)
+    return x_il, amax[:B], None if mask is None else amax[B:]
+
+
 def dcn_v2_fused_tc(x, om, weight, bias, deformable_group, pre_offset=None, idx=None, pre_scale=1, ref_gw=None,
                     lrelu=False, psa_out=False, out_f32=True, channels_last_out=False, final_mask=None):
     """Tensor-core version of dcn_v2_fused_forward (3x3/s1/p1/d1).  Returns fp32 and / or PSA.
     final_mask: `om` then holds the FINAL offsets [B,2*dg*9,H,W] and final_mask the FINAL modulation
     [B,dg*9,H,W] (the `_ext.dcn_v2_forward` contract: no pre-offsets, no sigmoid)."""
-    import ctypes
     om_oct = isinstance(om, OctF32)
     _require_cuda('om', om.data if om_oct else om)
     xp = x if isinstance(x, PSA) else getattr(x, '_c2m_psa', None)
@@ -593,13 +622,12 @@ def dcn_v2_fused_tc(x, om, weight, bias, deformable_group, pre_offset=None, idx=
     if xp is not None:
         if xp.sa != 0:
             raise RuntimeError('dcn_v2_fused_tc: PSA input must have scale exponent 0')
-        B, C, H, W = xp.shape
-        dev = xp.hi.device
+        x, dev = xp, xp.hi.device
     else:
         _require_cuda('x', x)
         x = _dense_nchw_or_nhwc(x)
-        B, C, H, W = x.shape
         dev = x.device
+    B, C, H, W = x.shape
     cout = weight.shape[0]
     if final_mask is not None:
         _require_cuda('final_mask', final_mask)
@@ -609,61 +637,41 @@ def dcn_v2_fused_tc(x, om, weight, bias, deformable_group, pre_offset=None, idx=
             raise RuntimeError(f'offset/mask shape mismatch: {tuple(om.shape)}, {tuple(final_mask.shape)}')
     elif tuple(om.shape) != (B, 27 * deformable_group, H, W):
         raise RuntimeError(f'conv_offset_mask output has shape {tuple(om.shape)}')
-    a = _lib.DcnTcArgs()
-    # x_il (the interleaved operand and its zero tail) and the amax buffer are kept alive until the launch below is
-    # enqueued (same stream)
-    x_il = torch.empty(_lib.lib().c2m_dcn_tc_operand_bytes(B, C, H, W, deformable_group) // 2, dtype=torch.float16,
-                       device=dev)
     if final_mask is not None:
         final_mask = final_mask.contiguous()
-        a.mask = final_mask.data_ptr()
+    a = _lib.DcnTcArgs()
+    # every tensor whose address `a` holds stays referenced here until the launch below is enqueued (same stream)
     with torch.cuda.device(dev):
-        if xp is not None:
-            rc = _lib.lib().c2m_dcn_tc_operand_psa(xp.hi.data_ptr(), xp.lo.data_ptr(), B, C, H, W, deformable_group,
-                                                   x_il.data_ptr(), _stream())
-            _lib.check(rc, 'c2m_dcn_tc_operand_psa')
+        x_il, x_amax, mask_amax = _dcn_tc_operand(x, deformable_group, final_mask)
+        a.x_il, a.x_amax, a.mask_amax, a.mask = x_il.data_ptr(), _ptr(x_amax), _ptr(mask_amax), _ptr(final_mask)
+        if om_oct:
+            a.om, a.om_octets = om.data.data_ptr(), 1
         else:
-            # an fp32 input of any magnitude: per-image operand (and final mask) exponents, taken on the device
-            amax = torch.empty(2 * B, dtype=torch.int32, device=dev)
-            rc = _lib.lib().c2m_dcn_tc_operand_f32(x.data_ptr(), B, C, H, W, *x.stride(), deformable_group,
-                                                   a.mask, x_il.data_ptr(), amax.data_ptr(), _stream())
-            _lib.check(rc, 'c2m_dcn_tc_operand_f32')
-            a.x_amax = amax.data_ptr()
-            if final_mask is not None:
-                a.mask_amax = amax.data_ptr() + 4 * B
-    a.x_il = x_il.data_ptr()
-    if om_oct:
-        a.om, a.om_octets = om.data.data_ptr(), 1
-    else:
-        om = om.contiguous()
-        a.om = om.data_ptr()
-    pre_offset, idx = _pre_offset_source(pre_offset, idx, B, 9, H, W)
-    if pre_offset is not None:
-        a.pre = pre_offset.data_ptr()
-    elif idx is not None:
-        a.idx = idx.data_ptr()
-        a.gh, a.gw = idx.shape[1:]
-        a.ref_gw, a.pre_scale = (ref_gw or idx.shape[2]), pre_scale
-    a.B, a.C, a.H, a.W, a.Cout, a.dg = B, C, H, W, cout, deformable_group
-    blob = _dcn_tc_pack(weight, deformable_group)
-    a.packed_w = blob.data_ptr()
-    a.bias = bias.contiguous().data_ptr() if bias is not None else None
-    a.lrelu = int(bool(lrelu))
-    ret_p = ret_f = None
-    if psa_out:
-        ret_p = PSA.empty(B, cout, H, W, dev)
-        a.out_hi, a.out_lo, a.sa_out = ret_p.hi.data_ptr(), ret_p.lo.data_ptr(), 0
-    if out_f32:
-        mf = torch.channels_last if channels_last_out else torch.contiguous_format
-        ret_f = torch.empty(B, cout, H, W, dtype=torch.float32, device=dev, memory_format=mf)
-        a.out_f32 = ret_f.data_ptr()
-        a.os_b, a.os_c, a.os_y, a.os_x = ret_f.stride()
-    with torch.cuda.device(dev):
-        rc = _lib.lib().c2m_dcn_v2_fused_tc(ctypes.addressof(a), _stream())
-        _lib.check(rc, 'c2m_dcn_v2_fused_tc')
-    if ret_p is not None and ret_f is not None:
-        return ret_p, ret_f
-    return ret_p if ret_p is not None else ret_f
+            om = om.contiguous()
+            a.om = om.data_ptr()
+        pre_offset, idx = _pre_offset_source(pre_offset, idx, B, 9, H, W)
+        if pre_offset is not None:
+            a.pre = pre_offset.data_ptr()
+        elif idx is not None:
+            a.idx = idx.data_ptr()
+            a.gh, a.gw = idx.shape[1:]
+            a.ref_gw, a.pre_scale = (ref_gw or idx.shape[2]), pre_scale
+        a.B, a.C, a.H, a.W, a.Cout, a.dg = B, C, H, W, cout, deformable_group
+        blob = _dcn_tc_pack(weight, deformable_group)
+        a.packed_w = blob.data_ptr()
+        bias = bias.contiguous() if bias is not None else None
+        a.bias = _ptr(bias)
+        a.lrelu = int(bool(lrelu))
+        ret_p = ret_f = None
+        if psa_out:
+            ret_p = PSA.empty(B, cout, H, W, dev)
+            a.out_hi, a.out_lo, a.sa_out = ret_p.hi.data_ptr(), ret_p.lo.data_ptr(), 0
+        if out_f32:
+            ret_f = _empty_f32(B, cout, H, W, dev, channels_last_out)
+            a.out_f32 = ret_f.data_ptr()
+            a.os_b, a.os_c, a.os_y, a.os_x = ret_f.stride()
+        _call('c2m_dcn_v2_fused_tc', ctypes.addressof(a))
+    return _one_or_both(ret_p, ret_f)
 
 
 def _dcn_tc_pack_dgrad(weight, dg):
@@ -688,7 +696,6 @@ class _DcnV2Tc(torch.autograd.Function):
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, gy):
-        import ctypes
         x, offset, mask, weight = ctx.saved_tensors
         need_x, need_off, need_mask, need_w, need_b = ctx.needs_input_grad[:5]
         dg = ctx.dg
@@ -696,19 +703,15 @@ class _DcnV2Tc(torch.autograd.Function):
         B, C, H, W = x.shape
         cout = weight.shape[0]
         gy = gy.contiguous()
-        L = _lib.lib()
         dev = gy.device
         gx = goff = gmask = dw = db = None
         with torch.cuda.device(dev):
             gp, gamax = _grad_psa(gy)
             # the forward's operand, made again: x * 2^sa and mask * 2^sm per image
-            x_il = torch.empty(L.c2m_dcn_tc_operand_bytes(B, C, H, W, dg) // 2, dtype=torch.float16, device=dev)
-            amax = torch.empty(2 * B, dtype=torch.int32, device=dev)
-            _lib.check(L.c2m_dcn_tc_operand_f32(x.data_ptr(), B, C, H, W, *x.stride(), dg, mask.data_ptr(),
-                                                x_il.data_ptr(), amax.data_ptr(), _stream()), 'c2m_dcn_tc_operand_f32')
+            x_il, x_amax, mask_amax = _dcn_tc_operand(x, dg, mask)
             a = _lib.DcnTcGradArgs()
             a.gy_hi, a.gy_lo, a.gy_amax = gp.hi.data_ptr(), gp.lo.data_ptr(), gamax.data_ptr()
-            a.x_il, a.x_amax, a.mask_amax = x_il.data_ptr(), amax.data_ptr(), amax.data_ptr() + 4 * B
+            a.x_il, a.x_amax, a.mask_amax = x_il.data_ptr(), x_amax.data_ptr(), mask_amax.data_ptr()
             a.offset, a.mask = offset.data_ptr(), mask.data_ptr()
             a.B, a.C, a.H, a.W, a.Cout, a.dg = B, C, H, W, cout, dg
             if need_x or need_off or need_mask:
@@ -718,14 +721,13 @@ class _DcnV2Tc(torch.autograd.Function):
                 if need_x:
                     gx = torch.zeros(B, C, H, W, dtype=torch.float32, device=dev)
                     a.grad_input = gx.data_ptr()
-                _lib.check(L.c2m_dcn_tc_dgrad(ctypes.addressof(a), _stream()), 'c2m_dcn_tc_dgrad')
+                _call('c2m_dcn_tc_dgrad', ctypes.addressof(a))
             if need_w:
                 dw = torch.empty(cout, C, 3, 3, dtype=torch.float32, device=dev)
-                nbytes = _lib.check_size(L.c2m_dcn_tc_wgrad_workspace_bytes(B, C, H, W, cout, dg),
-                                         'c2m_dcn_tc_wgrad_workspace_bytes')
+                nbytes = _size('c2m_dcn_tc_wgrad_workspace_bytes', B, C, H, W, cout, dg)
                 ws = _workspace(nbytes, dev)
                 a.grad_weight, a.ws, a.ws_bytes = dw.data_ptr(), ws.data_ptr(), nbytes
-                _lib.check(L.c2m_dcn_tc_wgrad(ctypes.addressof(a), _stream()), 'c2m_dcn_tc_wgrad')
+                _call('c2m_dcn_tc_wgrad', ctypes.addressof(a))
             if need_b:
                 db = gy.sum((0, 2, 3))
         return (gx, goff if need_off else None, gmask if need_mask else None, dw, db, None)
@@ -765,13 +767,9 @@ def dcn_v2_backward(input, weight, bias, offset, mask, grad_output, kernel_h, ke
         _require_cuda(n, t)
     x, w = input.contiguous(), weight.contiguous()
     offset, mask, gout = offset.contiguous(), mask.contiguous(), grad_output.contiguous()
-    B, C, H, W = x.shape
-    cout = w.shape[0]
-    Ho, Wo = _out_hw(H, W, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w)
-    if tuple(gout.shape) != (B, cout, Ho, Wo):
-        raise RuntimeError(f'grad_output has shape {tuple(gout.shape)}, expected {(B, cout, Ho, Wo)}')
-    s = _shape(x, cout, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w, deformable_group,
-               gout)
+    geom = (kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w)
+    _deform_out(x, w, offset, mask, geom, deformable_group, grad_output=gout)
+    s = _shape(x, w.shape[0], *geom, deformable_group, gout)
     return list(_deform_backward(x, w, offset, mask, gout, s, 1, True, True))
 
 
@@ -815,10 +813,6 @@ def _psroi_prepare(input, bbox, trans, no_trans, spatial_scale, output_dim, grou
     return s, input.contiguous(), bbox.contiguous(), None if no_trans else trans.contiguous()
 
 
-def _psroi_sfx(dtype):
-    return 'f32' if dtype == torch.float32 else 'f64'
-
-
 def dcn_v2_psroi_pooling_forward(input, bbox, trans, no_trans, spatial_scale, output_dim, group_size, pooled_size,
                                  part_size, sample_per_part, trans_std):
     """`_ext.dcn_v2_psroi_pooling_forward` (DCNv2/src/dcn_v2.h:75-108; call site dcn_v2.py:280-283) ->
@@ -827,10 +821,7 @@ def dcn_v2_psroi_pooling_forward(input, bbox, trans, no_trans, spatial_scale, ou
                                        pooled_size, part_size, sample_per_part, trans_std)
     out = torch.empty(s.R, output_dim, pooled_size, pooled_size, dtype=x.dtype, device=x.device)
     count = torch.empty_like(out)
-    fn = f'c2m_psroi_pooling_forward_{_psroi_sfx(x.dtype)}'
-    with torch.cuda.device(x.device):
-        _lib.check(getattr(_lib.lib(), fn)(x.data_ptr(), bbox.data_ptr(), None if trans is None else trans.data_ptr(),
-                                           s, out.data_ptr(), count.data_ptr(), _stream()), fn)
+    _call(f'c2m_psroi_pooling_forward_{_DTYPE_SFX[x.dtype]}', x, bbox, trans, s, out, count, device=x.device)
     return out, count
 
 
@@ -850,8 +841,7 @@ def dcn_v2_psroi_pooling_backward(out_grad, input, bbox, trans, top_count, no_tr
         raise RuntimeError(f'out_grad and top_count must be {want}, got {tuple(out_grad.shape)} and '
                            f'{tuple(top_count.shape)}')
     gout, cnt = out_grad.contiguous(), top_count.contiguous()
-    L = _lib.lib()
-    fn = f'c2m_psroi_pooling_backward_{_psroi_sfx(x.dtype)}'
+    sfx = _DTYPE_SFX[x.dtype]
     det = deterministic()
     with torch.cuda.device(x.device):
         grad_trans = torch.zeros_like(trans) if tr is None else torch.zeros_like(tr)
@@ -859,42 +849,35 @@ def dcn_v2_psroi_pooling_backward(out_grad, input, bbox, trans, top_count, no_tr
             # grad_trans (and, unless deterministic, grad_input) from the backward kernel; in deterministic mode its
             # scattered grad_input goes to a scratch buffer and is discarded
             grad_input = torch.zeros_like(x)
-            nbytes = L.c2m_psroi_pooling_workspace_bytes(s, x.element_size())
+            # 0 bytes is a valid answer here (no_trans needs no workspace), so the query is not checked
+            nbytes = _lib.lib().c2m_psroi_pooling_workspace_bytes(s, x.element_size())
             ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device) if nbytes else None
-            _lib.check(getattr(L, fn)(gout.data_ptr(), x.data_ptr(), bbox.data_ptr(),
-                                      None if tr is None else tr.data_ptr(), cnt.data_ptr(), s, grad_input.data_ptr(),
-                                      None if tr is None else grad_trans.data_ptr(),
-                                      None if ws is None else ws.data_ptr(), nbytes, _stream()), fn)
+            _call(f'c2m_psroi_pooling_backward_{sfx}', gout, x, bbox, tr, cnt, s, grad_input,
+                  None if tr is None else grad_trans, ws, nbytes)
         if det:
             grad_input = torch.empty_like(x)
-            fn = f'c2m_psroi_pooling_grad_input_det_{_psroi_sfx(x.dtype)}'
-            ws = _det_workspace(L.c2m_psroi_grad_input_det_workspace_bytes, s, s.B * (1 if no_trans else s.num_classes),
+            ws = _det_workspace('c2m_psroi_grad_input_det_workspace_bytes', s, s.B * (1 if no_trans else s.num_classes),
                                 x.device) if s.R and grad_input.numel() else None
-            _lib.check(getattr(L, fn)(gout.data_ptr(), bbox.data_ptr(), None if tr is None else tr.data_ptr(),
-                                      cnt.data_ptr(), s, grad_input.data_ptr(), None if ws is None else ws.data_ptr(),
-                                      0 if ws is None else ws.numel(), _stream()), fn)
+            _call(f'c2m_psroi_pooling_grad_input_det_{sfx}', gout, bbox, tr, cnt, s, grad_input, ws,
+                  0 if ws is None else ws.numel())
     return grad_input, grad_trans
 
 
 # ------------------------------------------------------------------------------------------------
 # Grouped deformable convolution, v1 and modulated (`deform_conv_cuda`, mmsr/models/archs/dcn/src)
-_DEFORM_DTYPES = {torch.float32: 'f32', torch.float64: 'f64'}
-
-
 def _deform_check(input, weight, offset, mask, kernel_h, kernel_w, groups, deformable_group, **more):
-    """Validates dtype, channel / kernel shapes, then devices; returns (B, C, H, W, Cout, dtype suffix)."""
+    """Validates dtype, channel / kernel shapes, then devices; returns the dtype suffix."""
     if not isinstance(input, torch.Tensor):
         raise TypeError('input must be a Tensor')
     dtype = input.dtype
-    if dtype not in _DEFORM_DTYPES:
+    if dtype not in _DTYPE_SFX:
         raise RuntimeError(f'deformable convolution supports torch.float32 and torch.float64, got {dtype}')
     if input.dim() != 4:
         raise RuntimeError(f'input must be [B, C, H, W], got shape {tuple(input.shape)}')
     if weight.dim() != 4 or weight.shape[2] != kernel_h or weight.shape[3] != kernel_w:
         raise RuntimeError(f'Input shape and kernel shape wont match: ({kernel_h} x {kernel_w} vs '
                            f'{tuple(weight.shape[2:])}).')
-    B, C, H, W = input.shape
-    cout = weight.shape[0]
+    C, cout = input.shape[1], weight.shape[0]
     if groups < 1 or C != weight.shape[1] * groups:
         raise RuntimeError(f'Input shape and kernel channels wont match: ({C} vs {weight.shape[1]} x {groups} groups).')
     if cout % groups:
@@ -907,7 +890,7 @@ def _deform_check(input, weight, offset, mask, kernel_h, kernel_w, groups, defor
             _require_cuda(n, t, dtype)
             if t.device != input.device:
                 raise RuntimeError(f'{n} is on {t.device}, input on {input.device}')
-    return B, C, H, W, cout, _DEFORM_DTYPES[dtype]
+    return _DTYPE_SFX[dtype]
 
 
 def deform_conv_forward(input, weight, offset, mask, bias, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w,
@@ -917,25 +900,17 @@ def deform_conv_forward(input, weight, offset, mask, bias, kernel_h, kernel_w, s
 
     A modulated fp32 call with groups == 1 is exactly `_ext.dcn_v2_forward` (dcn_v2_forward above, zero bias when
     bias is None), so eligible 3x3 shapes run on the tensor cores there."""
-    B, C, H, W, cout, sfx = _deform_check(input, weight, offset, mask, kernel_h, kernel_w, groups, deformable_group,
-                                          bias=bias)
-    Ho, Wo = _out_hw(H, W, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w)
-    if Ho < 1 or Wo < 1:
-        raise RuntimeError(f'convolution input is too small (output would be {Ho} x {Wo})')
-    T = kernel_h * kernel_w
-    if tuple(offset.shape) != (B, 2 * deformable_group * T, Ho, Wo) or (
-            mask is not None and tuple(mask.shape) != (B, deformable_group * T, Ho, Wo)):
-        raise RuntimeError(f'offset/mask shape mismatch: {tuple(offset.shape)}, '
-                           f'{None if mask is None else tuple(mask.shape)} for output {Ho}x{Wo}')
+    sfx = _deform_check(input, weight, offset, mask, kernel_h, kernel_w, groups, deformable_group, bias=bias)
+    geom = (kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w)
+    Ho, Wo = _deform_out(input, weight, offset, mask, geom, deformable_group, nonempty=True)
+    cout = weight.shape[0]
     if bias is not None and tuple(bias.shape) != (cout,):
         raise RuntimeError(f'bias must be [{cout}], got shape {tuple(bias.shape)}')
     if mask is not None and sfx == 'f32' and groups == 1:
         if bias is None:
             bias = torch.zeros(cout, dtype=input.dtype, device=input.device)
-        return dcn_v2_forward(input, weight, bias, offset, mask, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w,
-                              dilation_h, dilation_w, deformable_group)
-    return _deform_forward(_dense_nchw_or_nhwc(input), weight, offset, mask, bias, Ho, Wo,
-                           (kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w), groups,
+        return dcn_v2_forward(input, weight, bias, offset, mask, *geom, deformable_group)
+    return _deform_forward(_dense_nchw_or_nhwc(input), weight, offset, mask, bias, Ho, Wo, geom, groups,
                            deformable_group)
 
 
@@ -948,11 +923,8 @@ def _deform_forward(x, weight, offset, mask, bias, Ho, Wo, geom, groups, deforma
     offset, weight = offset.contiguous(), weight.contiguous()
     mask = mask.contiguous() if mask is not None else None
     bias = bias.contiguous() if bias is not None else None
-    fn = f'c2m_deform_conv_forward_{_DEFORM_DTYPES[x.dtype]}'
-    with torch.cuda.device(x.device):
-        _lib.check(getattr(_lib.lib(), fn)(x.data_ptr(), offset.data_ptr(), mask.data_ptr() if mask is not None else None,
-                                           weight.data_ptr(), bias.data_ptr() if bias is not None else None, groups,
-                                           out.data_ptr(), s, _stream()), fn)
+    _call(f'c2m_deform_conv_forward_{_DTYPE_SFX[x.dtype]}', x, offset, mask, weight, bias, groups, out, s,
+          device=x.device)
     return out
 
 
@@ -965,21 +937,13 @@ def deform_conv_backward(input, weight, offset, mask, grad_output, kernel_h, ker
         gcol_g = W_g^T gout_g,   grad_W_g = sum_b gout_g col_g^T.
     grad_mask is None when mask is None.  need_input=False skips grad_input / grad_offset / grad_mask (None),
     need_weight=False skips grad_weight / grad_bias (None)."""
-    B, C, H, W, cout, _ = _deform_check(input, weight, offset, mask, kernel_h, kernel_w, groups, deformable_group,
-                                        grad_output=grad_output)
+    _deform_check(input, weight, offset, mask, kernel_h, kernel_w, groups, deformable_group, grad_output=grad_output)
     x, w = input.contiguous(), weight.contiguous()
     offset, gout = offset.contiguous(), grad_output.contiguous()
     mask = mask.contiguous() if mask is not None else None
-    Ho, Wo = _out_hw(H, W, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w)
-    T = kernel_h * kernel_w
-    if tuple(gout.shape) != (B, cout, Ho, Wo):
-        raise RuntimeError(f'grad_output has shape {tuple(gout.shape)}, expected {(B, cout, Ho, Wo)}')
-    if tuple(offset.shape) != (B, 2 * deformable_group * T, Ho, Wo) or (
-            mask is not None and tuple(mask.shape) != (B, deformable_group * T, Ho, Wo)):
-        raise RuntimeError(f'offset/mask shape mismatch: {tuple(offset.shape)}, '
-                           f'{None if mask is None else tuple(mask.shape)} for output {Ho}x{Wo}')
-    s = _shape(x, cout, kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w, deformable_group,
-               gout)
+    geom = (kernel_h, kernel_w, stride_h, stride_w, pad_h, pad_w, dilation_h, dilation_w)
+    _deform_out(x, w, offset, mask, geom, deformable_group, grad_output=gout)
+    s = _shape(x, w.shape[0], *geom, deformable_group, gout)
     return _deform_backward(x, w, offset, mask, gout, s, groups, need_input, need_weight)
 
 
@@ -988,9 +952,7 @@ def _deform_backward(x, w, offset, mask, gout, s, groups, need_input, need_weigh
     B, C = x.shape[:2]
     cout = w.shape[0]
     T, P = s.kh * s.kw, gout.shape[2] * gout.shape[3]
-    sfx = _DEFORM_DTYPES[x.dtype]
-    L = _lib.lib()
-    mp = mask.data_ptr() if mask is not None else None
+    sfx = _DTYPE_SFX[x.dtype]
     G, cin_g, cout_g = groups, C // groups, cout // groups
     grad_input = grad_offset = grad_mask = grad_weight = grad_bias = None
     prev = torch.backends.cuda.matmul.allow_tf32
@@ -1004,17 +966,13 @@ def _deform_backward(x, w, offset, mask, gout, s, groups, need_input, need_weigh
                 gcol = torch.matmul(wg.transpose(1, 2), gg).contiguous()            # [B, G, Cin_g*T, P] = [B, C*T, P]
                 grad_offset = torch.empty_like(offset)
                 grad_mask = torch.empty_like(mask) if mask is not None else None
-                fn = f'c2m_deform_conv_col2im_coord_{sfx}'
-                _lib.check(getattr(L, fn)(gcol.data_ptr(), x.data_ptr(), offset.data_ptr(), mp, s,
-                                          grad_offset.data_ptr(),
-                                          grad_mask.data_ptr() if grad_mask is not None else None, _stream()), fn)
-                grad_input = _col2im(sfx, gcol, offset, mp, s, x)
+                _call(f'c2m_deform_conv_col2im_coord_{sfx}', gcol, x, offset, mask, s, grad_offset, grad_mask)
+                grad_input = _col2im(sfx, gcol, offset, mask, s, x)
                 columns = gcol                                                      # reuse the buffer
             if need_weight:
                 if columns is None:
                     columns = torch.empty(B, C * T, P, dtype=x.dtype, device=x.device)
-                fn = f'c2m_deform_conv_im2col_{sfx}'
-                _lib.check(getattr(L, fn)(x.data_ptr(), offset.data_ptr(), mp, s, columns.data_ptr(), _stream()), fn)
+                _call(f'c2m_deform_conv_im2col_{sfx}', x, offset, mask, s, columns)
                 cg = columns.view(B, G, cin_g * T, P)
                 grad_weight = torch.matmul(gg, cg.transpose(2, 3)).sum(0).view_as(w)
                 grad_bias = gout.sum(dim=(0, 2, 3))

@@ -26,13 +26,14 @@ c = ops.conv3x3_psa(a, w, b, residual=xp, residual2=a)
 wbig = seeding.randn(7, (256, 128, 3, 3), 0.05).to(dev)
 d = ops.conv3x3_psa(xp, wbig, None, x2=a, act='lrelu', pixel_shuffle=2)
 e = ops.conv3x3_psa(xp, wbig[:216, :64].contiguous(), None, psa_out=False, out_f32=True)
-# the literal `_ext` boundary on the tensor-core route, the max-pool, the PSA round trip and the interleaved DCN operand
+# the literal `_ext` boundary on the tensor-core route, the max-pool, the PSA round trip and the tensor-core DCN on a PSA
+# input (its operand from c2m_dcn_tc_operand_psa)
 import _ext
 off = seeding.randn(8, (1, 144, 24, 24), 2.0).to(dev)
 msk = torch.sigmoid(seeding.randn(9, (1, 72, 24, 24)).to(dev))
 y3 = _ext.dcn_v2_forward(x, w, b, off, msk, 3, 3, 1, 1, 1, 1, 1, 1, 8)
 mp = ops.psa_maxpool2(xp)
-xi = ops.psa_interleave(xp)
+yi = ops.dcn_v2_fused_tc(xp, om, w, b, 8)
 back = ops.psa_to_f32(a)
 # grouped deformable convolution, v1 and modulated, fp32 and fp64, forward and backward (3 conv groups of 4 input
 # channels against 2 deformable groups of 6, Cout_g = 7: a partial NO block)

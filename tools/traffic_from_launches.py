@@ -34,11 +34,13 @@ print('| kernel | launches | ms | share | DRAM read MB | DRAM write MB | MB per 
 for k, a in sorted(acc.items(), key=lambda kv: -kv[1][1]):
     print(f'| `{k[:70]}` | {a[0]} | {a[1]:.3f} | {a[1] / tot * 100:.1f}% | {a[2] / 1e6:.0f} | {a[3] / 1e6:.0f} | {(a[2] + a[3]) / a[0] / 1e6:.1f} |')
 if len(sys.argv) > 2:
-    out = {}
+    per = {}                                  # kernel -> [launches, bytes] over all its template instances
     for k, a in acc.items():
-        short = k.split('::')[-1]
-        if short in ('conv3x3_umma_kernel', 'corr_umma_kernel', 'dcn_umma_kernel', 'conv3x3_umma2_kernel'):
-            out[short] = (a[2] + a[3]) / a[0]
+        short = k.split('<')[0].split('::')[-1]
+        if short in ('conv3x3_wgmma_kernel', 'corr_umma_kernel', 'dcn_wgmma_kernel'):
+            p = per.setdefault(short, [0, 0.0])
+            p[0] += a[0]; p[1] += a[2] + a[3]
+    out = {k: b / n for k, (n, b) in per.items()}
     out['note'] = ('mean dram__bytes_read.sum + dram__bytes_write.sum per launch over the launches of one steady-state bench step '
                    '(B=4 config 2), from the ncu launch list summarised in profiles/r02_launches_step.md')
     json.dump(out, open(sys.argv[2], 'w'), indent=1)
