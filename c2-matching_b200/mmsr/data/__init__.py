@@ -1,6 +1,8 @@
-"""Dataset / dataloader factories (reference: mmsr/data/__init__.py:25-93), test phase only."""
+"""Dataset / dataloader factories (reference: mmsr/data/__init__.py:25-93)."""
+import functools
 import importlib
 import os
+import random
 
 import torch.utils.data
 
@@ -235,13 +237,43 @@ class PairBatcher:
                 pass
 
 
-def create_dataloader(dataset, dataset_opt, num_gpu=1, dist=False, sampler=None):
+def _seed_worker(seed, rank, num_workers, worker_id):
+    """Each loader worker of each rank gets its own seed for `random` and numpy (the augmentations draw from
+    `random`), derived from `manual_seed` and the rank, so a run can be repeated."""
+    import numpy as np
+    s = seed + rank * num_workers + worker_id
+    random.seed(s)
+    np.random.seed(s % 2 ** 32)
+
+
+def create_train_dataloader(dataset, dataset_opt, seed=0, sampler=None):
+    """Train-phase loader (reference: data/__init__.py:67-86 with `DistIterSampler`): this rank's shard of the
+    shuffled, `dataset_enlarge_ratio`-times enlarged index set, `batch_size / world` samples per batch (the
+    option is the batch over all GPUs, as in the reference), `n_workers` loader workers per GPU, incomplete last
+    batch dropped.  The caller calls `loader.sampler.set_epoch(epoch)` before each pass."""
+    from .data_sampler import DistIterSampler
+    world = torch.distributed.get_world_size() if torch.distributed.is_initialized() else 1
+    rank = torch.distributed.get_rank() if torch.distributed.is_initialized() else 0
+    batch = int(dataset_opt['batch_size'])
+    if batch % world:
+        raise ValueError(f'batch_size {batch} is not divisible by the {world} GPUs')
+    if sampler is None:
+        sampler = DistIterSampler(dataset, world, rank, int(dataset_opt.get('dataset_enlarge_ratio') or 1))
+    workers = int(dataset_opt.get('n_workers') or 0)
+    return torch.utils.data.DataLoader(
+        dataset, batch_size=batch // world, sampler=sampler, num_workers=workers, drop_last=True,
+        pin_memory=torch.cuda.is_available(), persistent_workers=workers > 0,
+        worker_init_fn=functools.partial(_seed_worker, int(seed or 0), rank, workers))
+
+
+def create_dataloader(dataset, dataset_opt, num_gpu=1, dist=False, sampler=None, seed=0):
     """Test-phase loader (reference: data/__init__.py:86-93, batch 1 / 1 worker / every rank sees everything).
     Here: the pair list is sharded `rank::world` at the INDEX level (a rank decodes only its pairs), pairs of equal
     shape are batched (`batch_size`, default 1 = the reference's behaviour), several workers decode ahead — one PAIR
-    per worker task (`PairBatcher`; `per_sample_workers: false` restores one batch per worker task)."""
+    per worker task (`PairBatcher`; `per_sample_workers: false` restores one batch per worker task).
+    A train-phase dataset option gets `create_train_dataloader` (`seed`: the run's `manual_seed`)."""
     if dataset_opt.get('phase', 'test') == 'train':
-        raise NotImplementedError('training loaders are outside the H100 hot-path scope')
+        return create_train_dataloader(dataset, dataset_opt, seed, sampler)
     from .data_sampler import ShapeBucketBatchSampler, ShardedEvalSampler
     if sampler is None:
         sampler = ShardedEvalSampler(dataset) if dist else ShardedEvalSampler(dataset, 1, 0)

@@ -1,17 +1,23 @@
-"""Inference-side `RefRestorationModel` (reference: mmsr/models/ref_restoration_model.py,
-base_model.py, sr_model.py): owns net_extractor / net_map / net_g, loads the reference's
-checkpoints strictly, `feed_data` / `test` / `get_current_visuals` / `validation`.
+"""`RefRestorationModel` (reference: mmsr/models/ref_restoration_model.py, base_model.py, sr_model.py):
+owns net_extractor / net_map / net_g, loads the reference's checkpoints strictly, `feed_data` / `test` /
+`get_current_visuals` / `validation`, and with `is_train` the pixel-loss training of net_g (stage 3,
+options/train/stage3_restoration_mse.yml): Adam over the reference's four parameter groups, MultiStepLR with
+linear warm-up, L1 / MSE pixel loss, checkpoints and training states in the reference's layout.
 
 Execution differences from the reference (SURVEY.md §8f N1): one process per GPU instead of
-nn.DataParallel; no per-image `torch.cuda.empty_cache()`; validation can be rank-sharded with
-`torch.distributed` (the reference's dist validation is broken, sr_model.py:160-162) and metrics
-are all-gathered at the end.  Training methods are out of scope and raise."""
+nn.DataParallel (DistributedDataParallel around net_g when training with `dist`); no per-image
+`torch.cuda.empty_cache()`; validation can be rank-sharded with `torch.distributed` (the reference's dist
+validation is broken, sr_model.py:160-162) and metrics are all-gathered at the end.  In training the frozen
+extractor and net_map run under no_grad, and the reference's stage-3 model builds its schedulers before its
+generator optimizer exists (ref_restoration_model.py:44-87 after sr_model.py:38-39), so there `lr_steps`
+never take effect; here they do.  GAN / perceptual / style / texture options raise NotImplementedError."""
 import logging
 import os
 import os.path as osp
 from collections import OrderedDict
 
 import torch
+import torch.nn.functional as F
 
 from c2m_b200.dist import gather_rows
 from mmsr.models import networks
@@ -21,13 +27,99 @@ from mmsr.utils.util import tensor2img
 logger = logging.getLogger('base')
 
 
+# options of losses and networks this build does not train (the GAN stage, perceptual / style / texture losses)
+_OUT_OF_SCOPE = (('train', 'perceptual_opt'), ('train', 'style_opt'), ('train', 'texture_opt'), ('train', 'gan_type'),
+                 (None, 'network_d'), ('path', 'pretrain_model_d'))
+
+
+def check_train_scope(opt):
+    """Raise NotImplementedError naming the first option that needs a loss or network outside pixel-loss training."""
+    for section, key in _OUT_OF_SCOPE:
+        holder = opt if section is None else (opt.get(section) or {})
+        if holder.get(key):
+            name = key if section is None else f'{section}.{key}'
+            raise NotImplementedError(f'option {name} needs a loss or network outside pixel-loss training of net_g '
+                                      '(the GAN stage and the perceptual, style and texture losses are not built)')
+
+
+def param_groups(net_g):
+    """The reference's split of net_g's trainable parameters (ref_restoration_model.py:54-68): names containing
+    'offset' and 'small' -> relu3_offset, 'offset' and 'medium' -> relu2_offset, other 'offset' names -> offset,
+    the rest -> g.  Returns OrderedDict group -> [(name, parameter)] in the reference's optimizer order."""
+    groups = OrderedDict((k, []) for k in ('g', 'offset', 'relu3_offset', 'relu2_offset'))
+    for name, v in net_g.named_parameters():
+        if not v.requires_grad:
+            continue
+        if 'offset' in name:
+            groups['relu3_offset' if 'small' in name else 'relu2_offset' if 'medium' in name else 'offset'].append((name, v))
+        else:
+            groups['g'].append((name, v))
+    return groups
+
+
+def build_optimizer(net_g, train_opt):
+    """Adam over param_groups with lr_g / lr_offset / lr_relu3_offset / lr_relu2_offset, weight_decay_g, beta_g
+    (ref_restoration_model.py:70-85)."""
+    g = param_groups(net_g)
+    lrs = {'offset': train_opt['lr_offset'], 'relu3_offset': train_opt['lr_relu3_offset'],
+           'relu2_offset': train_opt['lr_relu2_offset']}
+    return torch.optim.Adam([{'params': [p for _, p in ps], **({'lr': float(lrs[k])} if k in lrs else {})}
+                             for k, ps in g.items()],
+                            lr=float(train_opt['lr_g']), weight_decay=float(train_opt.get('weight_decay_g') or 0),
+                            betas=tuple(float(b) for b in train_opt.get('beta_g') or (0.9, 0.999)))
+
+
+def build_scheduler(optimizer, train_opt):
+    """`lr_scheme: MultiStepLR` (base_model.py:77-86: MultiStepRestartLR without restarts, which is torch's
+    MultiStepLR): every group's lr times lr_gamma at each of lr_steps."""
+    scheme = train_opt.get('lr_scheme') or 'MultiStepLR'
+    if scheme != 'MultiStepLR':
+        raise NotImplementedError(f'lr_scheme {scheme} is not implemented (MultiStepLR is)')
+    return torch.optim.lr_scheduler.MultiStepLR(optimizer, list(train_opt.get('lr_steps') or []),
+                                                gamma=float(train_opt.get('lr_gamma') or 0.1))
+
+
+def update_learning_rate(optimizers, schedulers, current_iter, warmup_iter=-1):
+    """base_model.py:155-177: step the schedulers from the second iteration on; below warmup_iter every group's lr
+    is its initial lr x current_iter / warmup_iter.  As there, the scheduler steps from the lr it finds, so after a
+    warm-up the lr stays at the last warm-up value (initial x (warmup_iter - 1) / warmup_iter) until a step."""
+    if current_iter > 1:
+        for s in schedulers:
+            s.step()
+    if warmup_iter is not None and current_iter < warmup_iter:
+        for o in optimizers:
+            for g in o.param_groups:
+                g['lr'] = g['initial_lr'] / warmup_iter * current_iter
+
+
+class PixelLoss(torch.nn.Module):
+    """`pixel_criterion` L1Loss / MSELoss of losses.py:30-83 without element weights: loss_weight x the
+    elementwise loss reduced by 'mean' or 'sum'."""
+
+    def __init__(self, criterion, loss_weight=1.0, reduction='mean'):
+        super().__init__()
+        fns = {'L1Loss': F.l1_loss, 'MSELoss': F.mse_loss}
+        if criterion not in fns:
+            raise NotImplementedError(f'pixel_criterion {criterion} is not implemented (L1Loss, MSELoss are)')
+        if reduction not in ('mean', 'sum'):
+            raise ValueError(f"reduction must be 'mean' or 'sum', got {reduction!r}")
+        self.fn, self.loss_weight, self.reduction = fns[criterion], float(loss_weight), reduction
+
+    def forward(self, pred, target):
+        return self.loss_weight * self.fn(pred, target, reduction=self.reduction)
+
+
+def _bare(net):
+    return net.module if isinstance(net, torch.nn.parallel.DistributedDataParallel) else net
+
+
 class RefRestorationModel:
 
     def __init__(self, opt):
         self.opt = opt
-        if opt.get('is_train'):
-            raise NotImplementedError('the H100 build covers inference (restoration forward) only')
-        self.is_train = False
+        self.is_train = bool(opt.get('is_train'))
+        if self.is_train:
+            check_train_scope(opt)
         if not torch.cuda.is_available():
             raise RuntimeError('RefRestorationModel needs a CUDA device: the H100 hot path has no CPU fallback')
         self.device = torch.device('cuda', torch.cuda.current_device())
@@ -51,9 +143,87 @@ class RefRestorationModel:
             self.load_network(self.net_extractor, path['pretrain_model_feature_extractor'], strict)
         if path.get('pretrain_model_g'):
             self.load_network(self.net_g, path['pretrain_model_g'], strict)
+        if self.is_train:
+            self.init_training_settings()
+
+    # -- training (ref_restoration_model.py:44-110, 186-269, base_model.py:136-307)
+    def init_training_settings(self):
+        train_opt = self.opt['train']
+        if self.opt.get('use_tb_logger'):
+            logger.warning('use_tb_logger is set: TensorBoard logging is not built, the run logs to its text log only.')
+        for net in (self.net_extractor, self.net_map):
+            net.eval().requires_grad_(False)
+        self.net_g.train()
+        if self.opt.get('dist'):
+            self.net_g = torch.nn.parallel.DistributedDataParallel(self.net_g, device_ids=[self.device.index])
+        if not float(train_opt.get('pixel_weight') or 0) > 0:
+            raise ValueError('pixel_weight must be > 0: the pixel loss is the only loss trained here')
+        self.cri_pix = PixelLoss(train_opt.get('pixel_criterion') or 'L1Loss', train_opt['pixel_weight'],
+                                 train_opt.get('reduction') or 'mean')
+        self.net_g_pretrain_steps = int(train_opt.get('net_g_pretrain_steps') or 0)
+        self.net_d_steps = int(train_opt.get('net_d_steps') or 1)
+        self.net_d_init_steps = int(train_opt.get('net_d_init_steps') or 0)
+        self.optimizer_g = build_optimizer(_bare(self.net_g), train_opt)
+        self.optimizers = [self.optimizer_g]
+        self.schedulers = [build_scheduler(self.optimizer_g, train_opt)]
+        self.log_dict = OrderedDict()
+
+    def optimize_parameters(self, step):
+        """One step of net_g on the pixel loss (ref_restoration_model.py:192-269 without a discriminator): the
+        frozen extractor and net_map run forward under no_grad.  As in the reference the loss is logged as l_pix
+        up to net_g_pretrain_steps and as l_g_pix after, where net_d_steps / net_d_init_steps gate the update."""
+        with torch.no_grad():
+            self.features = self.net_extractor(self.match_img_in, self.img_ref)
+            self.pre_offset, self.img_ref_feat = self.net_map(self.features, self.img_ref)
+        pretrain = step <= self.net_g_pretrain_steps
+        k = step - self.net_g_pretrain_steps
+        if not pretrain and not (k % self.net_d_steps == 0 and k > self.net_d_init_steps):
+            return
+        self.output = self.net_g(self.img_in_lq, self.pre_offset, self.img_ref_feat)
+        self.optimizer_g.zero_grad()
+        l_pix = self.cri_pix(self.output, self.gt)
+        l_pix.backward()
+        self.optimizer_g.step()
+        self.log_dict['l_pix' if pretrain else 'l_g_pix'] = l_pix.detach()     # read on the host only when logged
+
+    def update_learning_rate(self, current_iter, warmup_iter=-1):
+        update_learning_rate(self.optimizers, self.schedulers, current_iter, warmup_iter)
+
+    def get_current_learning_rate(self):
+        return [g['lr'] for g in self.optimizer_g.param_groups]
+
+    def get_current_log(self):
+        return OrderedDict((k, float(v)) for k, v in self.log_dict.items())
+
+    def _rank0(self):
+        return not (torch.distributed.is_available() and torch.distributed.is_initialized()) or \
+            torch.distributed.get_rank() == 0
+
+    def save(self, epoch, current_iter):
+        """net_g_<iter>.pth (net_g_latest.pth for iter -1) and, for iter != -1, training_state/<iter>.state with the
+        epoch, the iteration and the optimizer and scheduler states (base_model.py:185-290); rank 0 writes."""
+        if not self._rank0():
+            return
+        self.save_network(self.net_g, 'net_g', 'latest' if current_iter == -1 else current_iter)
+        if current_iter != -1:
+            state = {'epoch': epoch, 'iter': current_iter, 'optimizers': [o.state_dict() for o in self.optimizers],
+                     'schedulers': [s.state_dict() for s in self.schedulers]}
+            torch.save(state, osp.join(self.opt['path']['training_state'], f'{current_iter}.state'))
+
+    def resume_training(self, resume_state):
+        """Load the optimizer and scheduler states of a training state (base_model.py:292-307); net_g's weights come
+        from its checkpoint (`path.pretrain_model_g`)."""
+        if len(resume_state['optimizers']) != len(self.optimizers) or \
+                len(resume_state['schedulers']) != len(self.schedulers):
+            raise ValueError('the training state holds a different number of optimizers or schedulers')
+        for o, sd in zip(self.optimizers, resume_state['optimizers']):
+            o.load_state_dict(sd)
+        for s, sd in zip(self.schedulers, resume_state['schedulers']):
+            s.load_state_dict(sd)
 
     # -- checkpoint I/O (base_model.py:245-265: strips DataParallel's `module.` prefix)
     def load_network(self, net, load_path, strict=True):
+        net = _bare(net)
         logger.info(f'Loading {net.__class__.__name__} model from {load_path}.')
         sd = torch.load(load_path, map_location='cpu')
         sd = OrderedDict((k[7:] if k.startswith('module.') else k, v) for k, v in sd.items())
@@ -61,7 +231,7 @@ class RefRestorationModel:
 
     def save_network(self, net, net_label, current_iter):
         save_path = osp.join(self.opt['path']['models'], f'{net_label}_{current_iter}.pth')
-        torch.save(OrderedDict((k, v.cpu()) for k, v in net.state_dict().items()), save_path)
+        torch.save(OrderedDict((k, v.cpu()) for k, v in _bare(net).state_dict().items()), save_path)
 
     # -- data / forward (ref_restoration_model.py:186-190, 271-287)
     def feed_data(self, data):
@@ -76,16 +246,15 @@ class RefRestorationModel:
     def test(self):
         self.features = self.net_extractor(self.match_img_in, self.img_ref)
         self.pre_offset, self.img_ref_feat = self.net_map(self.features, self.img_ref)
-        self.output = self.net_g(self.img_in_lq, self.pre_offset, self.img_ref_feat)
+        # the bare net_g: a forward through DistributedDataParallel would take part in its collectives, and the ranks
+        # of a sharded validation run different numbers of batches
+        self.output = _bare(self.net_g)(self.img_in_lq, self.pre_offset, self.img_ref_feat)
 
     def get_current_visuals(self):
         out = OrderedDict(img_in_lq=self.img_in_lq.detach().cpu(), rlt=self.output.detach().cpu())
         if hasattr(self, 'gt'):
             out['gt'] = self.gt.detach().cpu()
         return out
-
-    def optimize_parameters(self, step):
-        raise NotImplementedError('training is outside the H100 hot-path scope')
 
     # -- validation (ref_restoration_model.py:295-370): rank-sharded, batched, host work off the GPU's critical path
     # packed-split activations are fp16 pairs: |x * 2^sa| must stay below 65504 (c2m_b200.ops.PSA)

@@ -47,7 +47,8 @@ def parse(opt_path, is_train=True):
     root = osp.abspath(osp.join(osp.dirname(osp.abspath(__file__)), osp.pardir, osp.pardir))
     opt['path']['root'] = root
     if is_train:
-        exp = osp.join(root, 'experiments', opt['name'])
+        # `path.experiments_root` in the file moves a run's directory out of the package tree
+        exp = opt['path'].get('experiments_root') or osp.join(root, 'experiments', opt['name'])
         opt['path'].update(experiments_root=exp, models=osp.join(exp, 'models'),
                            training_state=osp.join(exp, 'training_state'), log=exp,
                            visualization=osp.join(exp, 'visualization'))
