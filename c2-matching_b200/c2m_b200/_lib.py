@@ -90,9 +90,6 @@ SYMBOLS = {
     'c2m_psa_to_f32': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 5 + [c_f32p, c_f32p] +
                        [ctypes.c_longlong] * 4 + [ctypes.c_void_p]),
     'c2m_conv3x3': (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
-    'c2m_grad_psa_from_f32': (ctypes.c_int, [c_f32p] + [ctypes.c_int] * 4 + [ctypes.c_longlong] * 4 +
-                              [ctypes.c_void_p] * 4),
-    'c2m_grad_unscale_f32': (ctypes.c_int, [c_f32p, ctypes.c_longlong, ctypes.c_void_p, ctypes.c_void_p]),
     'c2m_conv3x3_wgrad_workspace_bytes': (ctypes.c_size_t, [ctypes.c_int] * 5),
     'c2m_conv3x3_operand_f32': (ctypes.c_int, [c_f32p] + [ctypes.c_int] * 4 + [ctypes.c_longlong] * 4 +
                                 [ctypes.c_void_p] * 4),
@@ -153,7 +150,7 @@ class C2MError(RuntimeError):
     pass
 
 
-EXPECTED_ABI = 6      # c2m_abi_version() the ctypes structs above mirror (include/c2m_sm100.h)
+EXPECTED_ABI = 7      # c2m_abi_version() the ctypes structs above mirror (include/c2m_sm100.h)
 
 
 def lib():

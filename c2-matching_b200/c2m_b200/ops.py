@@ -494,19 +494,10 @@ def conv3x3_psa(x, weight, bias, act=None, residual=None, residual2=None, x2=Non
     return _one_or_both(ret_psa, ret_f32)
 
 
-def _grad_psa(gy):
-    """grad_output [B,C,H,W] fp32 (any strides) as PSA at the power-of-two scale 2^sg chosen on the device, and the
-    one-element amax buffer the kernels read sg from (c2m_grad_psa_from_f32).  Call with gy's device current."""
-    B, C, H, W = gy.shape
-    gp = PSA.empty(B, C, H, W, gy.device)
-    amax = torch.empty(1, dtype=torch.int32, device=gy.device)
-    _call('c2m_grad_psa_from_f32', gy, B, C, H, W, *gy.stride(), gp.hi, gp.lo, amax)
-    return gp, amax
-
-
 def _conv3x3_operand(x):
     """x [B,C,H,W] fp32 (any strides, any magnitude) as PSA image b times 2^sa_b, and the [B] amax buffer the kernels
-    read sa_b from (c2m_conv3x3_operand_f32).  Call with x's device current."""
+    read sa_b from (c2m_conv3x3_operand_f32).  The operand form of x in the convolution's forward and of grad_output in
+    both backwards.  Call with x's device current."""
     B, C, H, W = x.shape
     xp = PSA.empty(B, C, H, W, x.device)
     amax = torch.empty(B, dtype=torch.int32, device=x.device)
@@ -517,8 +508,8 @@ def _conv3x3_operand(x):
 class _Conv3x3(torch.autograd.Function):
     """Forward on conv3x3_wgmma_kernel from x at a power-of-two scale per image chosen on the device
     (c2m_conv3x3_operand_f32); backward: the activation's backward, dX on the same kernel with the rotated weights, dW
-    on conv3x3_wgrad_kernel, db as a torch sum.  grad_output enters the kernels as PSA at a power-of-two scale chosen on
-    the device (c2m_grad_psa_from_f32).  The results divide every scale back out on the device."""
+    on conv3x3_wgrad_kernel, db as a torch sum.  grad_output enters the kernels like x, as PSA at a power-of-two scale
+    per image chosen on the device.  The results divide every scale back out on the device, image by image."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, act):
@@ -542,11 +533,10 @@ class _Conv3x3(torch.autograd.Function):
         dev = gy.device
         dx = dw = db = None
         with torch.cuda.device(dev):
-            gp, amax = _grad_psa(gy)
+            gp, amax = _conv3x3_operand(gy)
             if need_x:
                 dx = conv3x3_psa(gp, weight.transpose(0, 1), None, psa_out=False, out_f32=True,
-                                 packed=conv3x3_pack_weights(weight, dgrad=True))
-                _call('c2m_grad_unscale_f32', dx, dx.numel(), amax)
+                                 packed=conv3x3_pack_weights(weight, dgrad=True), x_amax=amax)
             if need_w:
                 dw = torch.empty(cout, cin, 3, 3, dtype=torch.float32, device=dev)
                 nbytes = _size('c2m_conv3x3_wgrad_workspace_bytes', B, cin, cout, H, W)
@@ -562,8 +552,9 @@ def conv3x3(x, weight, bias=None, act=None):
     """Differentiable act(conv2d(x, weight, bias, stride 1, padding 1)) on the tensor cores, fp32-grade forward and
     backward (fp32 in, fp32 out).  x [B,Cin,H,W] with H >= 18 and W >= 10, weight [Cout,Cin,3,3], bias [Cout] or None,
     act None / 'relu' / 'lrelu' (LeakyReLU(0.1)).  Any fp32 magnitude: each image of x and grad_output enters the
-    kernels at a power-of-two scale chosen on the device from its largest finite value, so x * 2^k gives exactly 2^k
-    times the output and dW.  NaN / Inf propagate to the entries that depend on them, as in an fp32 convolution (the
+    kernels at its own power-of-two scale chosen on the device from its largest finite value, so an image's results do
+    not depend on the other images' magnitudes, x * 2^k gives exactly 2^k times the output and dW, and grad_output * 2^k
+    exactly 2^k times every gradient.  NaN / Inf propagate to the entries that depend on them, as in an fp32 convolution (the
     input gradient of a non-finite weight also reaches the map's border)."""
     _require_cuda('x', x)
     _require_cuda('weight', weight)
@@ -682,9 +673,10 @@ def _dcn_tc_pack_dgrad(weight, dg):
 
 class _DcnV2Tc(torch.autograd.Function):
     """Forward: the tensor-core launch of `_ext.dcn_v2_forward` (dcn_v2_fused_tc with the final mask).  Backward:
-    grad_output as PSA at a power-of-two scale chosen on the device (c2m_grad_psa_from_f32), then
+    grad_output as PSA at a power-of-two scale per image chosen on the device (c2m_conv3x3_operand_f32), then
     dcn_dgrad_kernel for grad_offset / grad_mask (and grad_input when x requires it) and dcn_wgrad_kernel for the
-    weight gradient; db is a torch sum."""
+    weight gradient; db is a torch sum.  Every gradient divides each image's scales back out, so an image's gradients
+    do not depend on the other images' magnitudes."""
 
     @staticmethod
     def forward(ctx, x, offset, mask, weight, bias, dg):
@@ -706,7 +698,7 @@ class _DcnV2Tc(torch.autograd.Function):
         dev = gy.device
         gx = goff = gmask = dw = db = None
         with torch.cuda.device(dev):
-            gp, gamax = _grad_psa(gy)
+            gp, gamax = _conv3x3_operand(gy)
             # the forward's operand, made again: x * 2^sa and mask * 2^sm per image
             x_il, x_amax, mask_amax = _dcn_tc_operand(x, dg, mask)
             a = _lib.DcnTcGradArgs()

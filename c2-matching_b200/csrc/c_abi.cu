@@ -122,12 +122,13 @@ static void carve(CorrWorkspace &ws, const CorrGeom &g, uint8_t *base) {
 
 using namespace c2m;
 
-// 6: no fp32 c2m_dcn_v2_* twins of c2m_deform_conv_*; 5: c2m_dcn_tc_args without x_hi / x_lo; 4: .x_il +
+// 7: gy_amax is [B] (one grad_output exponent per image), no c2m_grad_psa_from_f32 / c2m_grad_unscale_f32; 6: no fp32
+// c2m_dcn_v2_* twins of c2m_deform_conv_*; 5: c2m_dcn_tc_args without x_hi / x_lo; 4: .x_il +
 // c2m_psa_interleave; 3: .mask; 2: out_f32_octets / om_octets.  (c2m_dcn_tc_args has since gained x_amax / mask_amax at
 // its end and c2m_psa_interleave became c2m_dcn_tc_operand_psa; c2m_conv3x3_args gained x_amax at its end, with
 // c2m_conv3x3_operand_f32 and c2m_conv3x3_wgrad_scaled: the bindings resolve every declared symbol, so a library older
 // than those fails to load.)
-extern "C" int c2m_abi_version(void) { return 6; }
+extern "C" int c2m_abi_version(void) { return 7; }
 extern "C" const char *c2m_last_error(void) { return g_err; }
 extern "C" unsigned long long c2m_launch_count(void) { return g_launches.load(); }
 

@@ -171,8 +171,12 @@ conv3x3_wgmma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
             tile_at(g, b, y0, x0);
             const int y = y0 + e / T_C, x = x0 + e % T_C;
             const bool ok = y < p.H && x < p.W;
-            // per-image input exponents (ops.conv3x3): 2^-(sa_b + sw) for this tile's image
-            const float osc = q.x_amax ? ldexpf(1.f, -(grad_scale_exp(q.x_amax + b) + sw)) : out_scale;
+            // per-image input exponents (ops.conv3x3): 2^-(sa_b + sw) for this tile's image.  Past 2^-126 that factor
+            // is not a normal float (past 2^-149 it is 0): the accumulator is then first multiplied by 2^-ex, exactly
+            // while it stays normal, and the epilogue applies the rest, so an output of ~2^-120 still rounds once.
+            const int oe = q.x_amax ? grad_scale_exp(q.x_amax + b) + sw : 0;
+            const int ex = oe > 126 ? min(oe - 126, 126) : 0;
+            const float osc = q.x_amax ? ldexpf(1.f, ex - oe) : out_scale;
             ResRegs ra;
             if (has1 && c0 < N) {
                 if (full_blk) prefetch_residual_full(q.res_hi, q.res_lo, p, b, y, x, ok, o_base, c0, ra);
@@ -210,6 +214,11 @@ conv3x3_wgmma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
             float v[N / 2];
 #pragma unroll
             for (int i = 0; i < N / 2; ++i) v[i] = acc[i] + acc[i + N / 2];      // columns c and N + c
+            if (ex) {                                                            // uniform per tile
+                const float pre = ldexpf(1.f, -ex);
+#pragma unroll
+                for (int i = 0; i < N / 2; ++i) v[i] *= pre;
+            }
             asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");          // previous tile's epilogue is done
             acc_store(acc_s, wg * 64, v);
             asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
@@ -237,13 +246,13 @@ conv3x3_wgmma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_con
 // ------------------------------------------------------------------------------------------
 __global__ void psa_from_f32_kernel(const float *__restrict__ x, int C, int C8, int H, int W, long long xs_b,
                                     long long xs_c, long long xs_y, long long xs_x, int sa,
-                                    const unsigned *__restrict__ amax, int amax_step, __half *__restrict__ hi,
+                                    const unsigned *__restrict__ amax, __half *__restrict__ hi,
                                     __half *__restrict__ lo) {
     // one thread = one (octet, pixel); pixel fastest -> coalesced NCHW reads and 16 B stores
     const long long HW = (long long)H * W;
     const long long n = (long long)C8 * HW;
     const int b = blockIdx.y;
-    const float S = ldexpf(1.f, amax ? grad_scale_exp(amax + b * amax_step) : sa);
+    const float S = ldexpf(1.f, amax ? grad_scale_exp(amax + b) : sa);
     for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x) {
         const int oct = (int)(e / HW);
         const long long pix = e % HW;
@@ -385,7 +394,7 @@ extern "C" int c2m_psa_from_f32(const float *x, int B, int C, int H, int W, long
     int bx = (int)((n + 255) / 256);
     if (bx > 4096) bx = 4096;
     psa_from_f32_kernel<<<dim3(bx, B), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-        x, C, C8, H, W, xs_b, xs_c, xs_y, xs_x, sa, nullptr, 0, reinterpret_cast<__half *>(hi),
+        x, C, C8, H, W, xs_b, xs_c, xs_y, xs_x, sa, nullptr, reinterpret_cast<__half *>(hi),
         reinterpret_cast<__half *>(lo));
     C2M_LAUNCH_CHECK("psa_from_f32_kernel");
     return C2M_OK;

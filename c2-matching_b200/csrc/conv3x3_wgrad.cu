@@ -5,9 +5,11 @@
 // in Cin / Cout and rotated by 180 degrees, so it runs on conv3x3_wgmma_kernel with a second packed weight blob.
 //
 // Loss gradients are tiny (an L1 mean over a 9 x 3 x 160 x 160 batch gives ~2^-19 per element) and would lose their lo
-// halves to fp16 subnormals at scale exponent 0.  c2m_grad_psa_from_f32 therefore stores grad_output * 2^sg, where
-// sg = 14 - exponent(largest finite |grad_output|) is computed on the device; the results divide 2^sg back out on the
-// device, so no host synchronisation is needed and grad_output * 2^k gives exactly 2^k times the gradients.
+// halves to fp16 subnormals at scale exponent 0.  grad_output therefore enters as the forward's x does
+// (c2m_conv3x3_operand_f32): image b is stored as grad_output * 2^sg_b, sg_b = 14 - exponent(largest finite |grad_output|
+// of image b), computed on the device.  The results divide 2^sg_b back out on the device, image by image, so no host
+// synchronisation is needed, an image's gradients do not depend on the other images' magnitudes, and grad_output * 2^k
+// gives exactly 2^k times the gradients.
 //
 // Weight gradient, dW[co][ci][tap] = sum over (b, y, x) of gY[b,co,y,x] * X[b,ci,(y,x) + delta_tap]: a GEMM with
 // M = Cout, N = Cin x 9 taps and K = every pixel of the batch.  Both operands are PSA tensors, fp16 [B][C/8][H][W][8]:
@@ -44,6 +46,7 @@ struct WgradGeom {
     int nslice, nchunk, ksplit;
     int tiles_x, tiles_y;
     long long ntiles;
+    const unsigned *gy_amax;    // [B]: image b of gY is stored as gy * 2^grad_scale_exp(gy_amax + b)
     const unsigned *x_amax;     // [B] or null: image b of X is stored as x * 2^grad_scale_exp(x_amax + b)
 };
 
@@ -83,12 +86,6 @@ __global__ void grad_amax_kernel(const float *__restrict__ g, int C, int H, int 
     if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(amax + b * amax_step, __float_as_uint(m));
 }
 
-__global__ void grad_unscale_kernel(float *__restrict__ x, long long n, const unsigned *__restrict__ amax) {
-    const int s = -grad_scale_exp(amax);
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-        x[i] = ldexpf(x[i], s);
-}
-
 // Consumer warpgroup of conv3x3_wgrad_kernel: taps [T0, T0 + NT) of every K step of tiles [t0, t1), then the 64 x 32 x NT
 // partial into the CTA's workspace slot `dst` ([co_pad][tap][ci_pad] fp32, see wgrad_flush).
 template <int T0, int NT>
@@ -102,15 +99,11 @@ __device__ __forceinline__ void wgrad_consume(uint8_t *smem, uint64_t *full, uin
     const int ci_pad = p.nchunk * WG_CI, ncol = 9 * ci_pad;
     float *blk = dst + (size_t)slice * WG_CO * ncol + T0 * ci_pad + chunk * WG_CI;
     bool first = true;
-    // each accumulator run holds one image: the flush divides its input exponent back out.  |exponent| <= 120, so
-    // the scale is a normal float and the product rounds like ldexpf (one multiply instead of ldexpf per register).
+    // each accumulator run holds one image: the flush divides its two operand exponents back out (their sum can reach
+    // +-240, see wgrad_flush)
     auto flush = [&](int b) {
-        const float sc = ldexpf(1.f, p.x_amax && b >= 0 ? -grad_scale_exp(p.x_amax + b) : 0);
-#pragma unroll
-        for (int t = 0; t < NT; ++t)
-#pragma unroll
-            for (int i = 0; i < 16; ++i) acc[t][i] *= sc;
-        wgrad_flush<false>(acc, blk, ncol, ci_pad, first, 0);
+        const int e = b < 0 ? 0 : -(grad_scale_exp(p.gy_amax + b) + (p.x_amax ? grad_scale_exp(p.x_amax + b) : 0));
+        wgrad_flush(acc, blk, ncol, ci_pad, first, e);
         first = false;
     };
     int stage = 0, phase = 0, n = 0, cur_b = -1;
@@ -223,8 +216,7 @@ conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tg_hi, const __grid_con
 }
 
 __global__ void wgrad_reduce_kernel(const float *__restrict__ ws, int nslots, int C, int Cout, int cpg, int co_pad,
-                                    int ncol, const unsigned *__restrict__ gy_amax, float *__restrict__ dw) {
-    const int s = -grad_scale_exp(gy_amax);
+                                    int ncol, float *__restrict__ dw) {
     const long long n = (long long)Cout * ncol;
     const size_t slot = (size_t)co_pad * ncol;
     for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x) {
@@ -233,13 +225,13 @@ __global__ void wgrad_reduce_kernel(const float *__restrict__ ws, int nslots, in
         if (c >= C) continue;                                             // padding column
         float v = 0.f;
         for (int j = 0; j < nslots; ++j) v += ws[e + j * slot];
-        dw[((size_t)co * C + c) * 9 + pair % 9] = ldexpf(v, s);
+        dw[((size_t)co * C + c) * 9 + pair % 9] = v;
     }
 }
 
 static int wgrad_geom(int B, int Cin, int Cout, int H, int W, WgradGeom &g) {
     g.B = B; g.H = H; g.W = W; g.Cin = Cin; g.Cout = Cout;
-    g.x_amax = nullptr;
+    g.gy_amax = g.x_amax = nullptr;
     g.C8i = (Cin + 7) / 8; g.C8o = (Cout + 7) / 8;
     g.nslice = ceil_div(Cout, WG_CO);
     g.nchunk = ceil_div(Cin, WG_CI);
@@ -253,47 +245,22 @@ static int wgrad_geom(int B, int Cin, int Cout, int H, int W, WgradGeom &g) {
 
 using namespace c2m;
 
-namespace c2m {
-// g [B,C,H,W] fp32 -> PSA g * 2^grad_scale_exp(amax), with the largest finite |g| of the batch in amax[0]
-// (per_image 0) or of each image in amax[b] (1)
-static int scaled_psa_from_f32(const float *g, int B, int C, int H, int W, long long gs_b, long long gs_c,
-                               long long gs_y, long long gs_x, void *hi, void *lo, unsigned *amax, int per_image,
-                               c2m_stream_t stream) {
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    C2M_CUDA(cudaMemsetAsync(amax, 0, (per_image ? B : 1) * sizeof(unsigned), st));
-    const long long n = (long long)C * H * W;
-    const int ba = (int)((n + 255) / 256 < 1024 ? (n + 255) / 256 : 1024);
-    grad_amax_kernel<<<dim3(ba, B), 256, 0, st>>>(g, C, H, W, gs_b, gs_c, gs_y, gs_x, amax, per_image);
-    C2M_LAUNCH_CHECK("grad_amax_kernel");
-    const int C8 = (C + 7) / 8;
-    const long long np = (long long)C8 * H * W;
-    const int bx = (int)((np + 255) / 256 < 4096 ? (np + 255) / 256 : 4096);
-    psa_from_f32_kernel<<<dim3(bx, B), 256, 0, st>>>(g, C, C8, H, W, gs_b, gs_c, gs_y, gs_x, 0, amax, per_image,
-                                                     reinterpret_cast<__half *>(hi), reinterpret_cast<__half *>(lo));
-    C2M_LAUNCH_CHECK("psa_from_f32_kernel");
-    return C2M_OK;
-}
-
-}  // namespace c2m
-
-extern "C" int c2m_grad_psa_from_f32(const float *g, int B, int C, int H, int W, long long gs_b, long long gs_c,
-                                     long long gs_y, long long gs_x, void *hi, void *lo, unsigned *amax,
-                                     c2m_stream_t stream) {
-    C2M_CHECK_ARG(g && hi && lo && amax && B > 0 && C > 0 && H > 0 && W > 0, "grad_psa_from_f32: bad argument");
-    return scaled_psa_from_f32(g, B, C, H, W, gs_b, gs_c, gs_y, gs_x, hi, lo, amax, 0, stream);
-}
-
 extern "C" int c2m_conv3x3_operand_f32(const float *x, int B, int C, int H, int W, long long xs_b, long long xs_c,
                                        long long xs_y, long long xs_x, void *hi, void *lo, unsigned *amax,
                                        c2m_stream_t stream) {
     C2M_CHECK_ARG(x && hi && lo && amax && B > 0 && C > 0 && H > 0 && W > 0, "conv3x3_operand_f32: bad argument");
-    return scaled_psa_from_f32(x, B, C, H, W, xs_b, xs_c, xs_y, xs_x, hi, lo, amax, 1, stream);
-}
-
-extern "C" int c2m_grad_unscale_f32(float *x, long long n, const unsigned *amax, c2m_stream_t stream) {
-    C2M_CHECK_ARG(x && amax && n > 0, "grad_unscale_f32: bad argument");
-    grad_unscale_kernel<<<grid_blocks(n), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(x, n, amax);
-    C2M_LAUNCH_CHECK("grad_unscale_kernel");
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    C2M_CUDA(cudaMemsetAsync(amax, 0, B * sizeof(unsigned), st));
+    const long long n = (long long)C * H * W;
+    const int ba = (int)((n + 255) / 256 < 1024 ? (n + 255) / 256 : 1024);
+    grad_amax_kernel<<<dim3(ba, B), 256, 0, st>>>(x, C, H, W, xs_b, xs_c, xs_y, xs_x, amax, 1);
+    C2M_LAUNCH_CHECK("grad_amax_kernel");
+    const int C8 = (C + 7) / 8;
+    const long long np = (long long)C8 * H * W;
+    const int bx = (int)((np + 255) / 256 < 4096 ? (np + 255) / 256 : 4096);
+    psa_from_f32_kernel<<<dim3(bx, B), 256, 0, st>>>(x, C, C8, H, W, xs_b, xs_c, xs_y, xs_x, 0, amax,
+                                                     reinterpret_cast<__half *>(hi), reinterpret_cast<__half *>(lo));
+    C2M_LAUNCH_CHECK("psa_from_f32_kernel");
     return C2M_OK;
 }
 
@@ -316,6 +283,7 @@ static int conv3x3_wgrad(const void *gy_hi, const void *gy_lo, const unsigned *g
     C2M_CHECK_ARG(H >= X_R && W >= X_C, "conv3x3_wgrad: map %dx%d smaller than one halo tile (18x10)", H, W);
     WgradGeom g;
     if (const int rc = wgrad_geom(B, Cin, Cout, H, W, g)) return rc;
+    g.gy_amax = gy_amax;
     g.x_amax = x_amax;
     const int co_pad = g.nslice * WG_CO, ci_pad = g.nchunk * WG_CI;
     const size_t need = wgrad_ws_bytes(g.ksplit, co_pad, 9 * ci_pad);
@@ -341,7 +309,7 @@ static int conv3x3_wgrad(const void *gy_hi, const void *gy_lo, const unsigned *g
     C2M_LAUNCH_CHECK("conv3x3_wgrad_kernel");
     prof_end(ph, st);
     wgrad_reduce_kernel<<<grid_blocks((long long)Cout * 9 * ci_pad), 256, 0, st>>>(part, g.ksplit, Cin, Cout, ci_pad,
-                                                                                co_pad, 9 * ci_pad, gy_amax, dw);
+                                                                                co_pad, 9 * ci_pad, dw);
     C2M_LAUNCH_CHECK("wgrad_reduce_kernel");
     return C2M_OK;
 }

@@ -2,8 +2,10 @@
 // 3x3 / stride 1 / pad 1 / dilation 1, one conv group) on the sm_90a tensor cores, fp32-grade (split fp16 x 3).
 //
 // Both kernels work on the forward's 16x8-pixel tiles and its column order K = (deformable group g, tap, channel in
-// group).  grad_output enters as PSA at the power-of-two scale 2^sg of c2m_grad_psa_from_f32; x enters as the forward's
-// interleaved operand x_il (x * 2^sa_b per image) and the final mask as mask * 2^sm_b (c2m_dcn_tc_operand_f32).
+// group).  grad_output enters as PSA at the per-image power-of-two scale 2^sg_b of c2m_conv3x3_operand_f32; x enters as
+// the forward's
+// interleaved operand x_il (x * 2^sa_b per image) and the final mask as mask * 2^sm_b (c2m_dcn_tc_operand_f32).  Every
+// result is divided by its own image's exponents, so an image's gradients do not depend on the other images.
 //
 // dcn_dgrad_kernel: gcol = W^T gY, M = the tile's 128 pixels, N = a chunk of columns, K = Cout.  gY arrives by TMA as
 // the forward's K-major activation layout [octet][128 px][8], the weights as a second packed blob (K = Cout octets,
@@ -18,7 +20,7 @@
 // warps build mask * bilinear(x) for a tile in the forward's [octet][px][8] layout, which is an MN-major operand along
 // K = pixels; gY is the MN-major operand of the same tile by TMA (as in conv3x3_wgrad.cu).  The accumulator is added
 // into the CTA's fp32 workspace slot every WG_FLUSH tiles and whenever the image changes, divided by that image's
-// operand scale 2^(sa_b + sm_b); wgrad_reduce_kernel sums the slots in one fixed order and divides 2^sg out
+// operand scales 2^(sa_b + sm_b + sg_b); wgrad_reduce_kernel sums the slots in one fixed order
 // (umma_conv_common.cuh).
 #include "dcn_sampling.cuh"
 #include "umma_conv_common.cuh"
@@ -155,7 +157,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) dcn_dgrad_kernel(const __grid_c
         const int e = (threadIdx.x - 256) >> 7, m = threadIdx.x & 127;
         const float *buf = stg + e * (acc_stage_bytes(DG_NMAX) / 4) + m;
         const size_t plane = (size_t)d.H * d.W;
-        const int sgw = grad_scale_exp(d.gy_amax) + *reinterpret_cast<const int *>(d.wblob);   // gcol = 2^sgw W^T gY
+        const int sw_blob = *reinterpret_cast<const int *>(d.wblob);
         int got = 0;
         float sh = 0.f, sw = 0.f, sm = 0.f;                 // running sums of the current (pixel, g, tap)
         for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
@@ -163,6 +165,7 @@ __global__ void __launch_bounds__(DG_THREADS, 1) dcn_dgrad_kernel(const __grid_c
             const int y = (tt / d.tiles_x) * T_R + m / T_C, x = (tt % d.tiles_x) * T_C + m % T_C;
             const bool ok = y < d.H && x < d.W;
             const int p = y * d.W + x;
+            const int sgw = grad_scale_exp(d.gy_amax + b) + sw_blob;    // gcol = 2^sgw W^T gY of image b
             // unscaled as one ldexpf of the result: 2^-(sgw + sa_b) alone can be below fp32's range
             const int out_exp = -(sgw + operand_exp(d.x_amax, b));
             const float *offb = d.off + (size_t)b * 2 * d.dg * 9 * plane;
@@ -315,8 +318,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) dcn_wgrad_kernel(const __grid_con
         float *blk = d.ws + ((size_t)kr * d.ncs * WG_NCO + cs * WG_NCO) * ncol + kc * 32;
         bool first = true;
         auto flush = [&](int b) {
-            wgrad_flush<true>(acc, blk, ncol, 64 * ncol, first,
-                        -(operand_exp(d.x_amax, b) + mask_exp(d.mask_amax, b)));
+            wgrad_flush(acc, blk, ncol, 64 * ncol, first,
+                        -(operand_exp(d.x_amax, b) + mask_exp(d.mask_amax, b) + grad_scale_exp(d.gy_amax + b)));
             first = false;
         };
         int ys = 0, yph = 0, gs = 0, gph = 0, n = 0, cur_b = -1;
@@ -565,7 +568,7 @@ extern "C" int c2m_dcn_tc_wgrad(const c2m_dcn_tc_grad_args *a, c2m_stream_t stre
     }
     C2M_LAUNCH_CHECK("dcn_wgrad_kernel");
     wgrad_reduce_kernel<<<grid_blocks((long long)a->Cout * d.nkc * 32), 256, 0, st>>>(
-        d.ws, d.ksplit, a->C, a->Cout, d.cpg, d.ncs * WG_NCO, d.nkc * 32, a->gy_amax, a->grad_weight);
+        d.ws, d.ksplit, a->C, a->Cout, d.cpg, d.ncs * WG_NCO, d.nkc * 32, a->grad_weight);
     C2M_LAUNCH_CHECK("wgrad_reduce_kernel");
     prof_end(ph, st);
     return C2M_OK;

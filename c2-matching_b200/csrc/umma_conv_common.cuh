@@ -93,9 +93,9 @@ __host__ __device__ __forceinline__ int amax_exp(unsigned bits, int top) {
     const int s = top - e;
     return s < -120 ? -120 : s > 120 ? 120 : s;
 }
-// Gradient scale exponent: sg = 14 - floor(log2 amax) (amax * 2^sg in [2^14, 2^15)), from the bits of the largest finite
-// |grad_output|; 0 for an all-zero gradient, clamped to +-120 so that 2^sg and 2^-sg are normal floats.  The plain
-// convolution's per-image input exponents (c2m_conv3x3_operand_f32) are the same function of each image's amax.
+// Per-image exponent of the plain convolution's operands (c2m_conv3x3_operand_f32: x in the forward, grad_output in
+// both backwards): sg = 14 - floor(log2 amax) (amax * 2^sg in [2^14, 2^15)), from the bits of the image's largest
+// finite |value|; 0 for an all-zero image, clamped to +-120 so that 2^sg and 2^-sg are normal floats.
 __host__ __device__ __forceinline__ int grad_scale_exp(const unsigned *amax) { return amax_exp(*amax, 14); }
 
 // ---- Split-K weight gradients (conv3x3_wgrad.cu, dcn_tc_bwd.cu).  dW is a GEMM with M = Cout and K = every pixel of
@@ -116,22 +116,29 @@ inline int wgrad_ksplit(int ctas, long long ntiles, int &ksplit) {
 
 inline size_t wgrad_ws_bytes(int ksplit, int co_pad, int ncol) { return (size_t)ksplit * co_pad * ncol * sizeof(float); }
 
-// Adds the calling warpgroup's NA m64n32 fp32 wgmma accumulators into a slot and restarts them (`first` stores instead
-// of adding); SCALED multiplies them by 2^e first.  Accumulator a covers rows [0, 64) x columns [0, 32) from
-// blk + a * stride, row pitch ncol.  Register i of thread (warp w, lane l) holds row 16 w + l / 4 + 8 ((i / 2) % 2),
-// column 8 (i / 4) + 2 (l % 4) + i % 2.  The kernels flush every few tiles because the tensor cores' fp32 accumulation
-// error grows with the number of MMAs into one accumulator (linearly, not as a random walk); the slot adds are fp32.
-template <bool SCALED, int NA>
+// Adds the calling warpgroup's NA m64n32 fp32 wgmma accumulators, times 2^e, into a slot and restarts them (`first`
+// stores instead of adding).  Accumulator a covers rows [0, 64) x columns [0, 32) from blk + a * stride, row pitch ncol.
+// Register i of thread (warp w, lane l) holds row 16 w + l / 4 + 8 ((i / 2) % 2), column 8 (i / 4) + 2 (l % 4) + i % 2.
+// The kernels flush every few tiles because the tensor cores' fp32 accumulation error grows with the number of MMAs
+// into one accumulator (linearly, not as a random walk); the slot adds are fp32.
+// e sums up to three clamped operand exponents, so 2^e need not be a float: it is one multiply by a normal power of two
+// when |e| <= 126 (the common case), else two or three of the same sign.  Each partial product then lies between the
+// accumulator and the result, so only the last rounds, as ldexpf would (unless the result is below fp32's normal range).
+template <int NA>
 __device__ __forceinline__ void wgrad_flush(float (&acc)[NA][16], float *blk, int ncol, int stride, bool first,
                                             int e) {
     const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
     float *out = blk + (16 * w + (l >> 2)) * ncol + 2 * (l & 3);
+    const int e1 = max(-126, min(126, e)), e2 = max(-126, min(126, e - e1));
+    const float s1 = ldexpf(1.f, e1), s2 = ldexpf(1.f, e2), s3 = ldexpf(1.f, e - e1 - e2);
+    const bool more = e1 != e;
 #pragma unroll
     for (int a = 0; a < NA; ++a) {
         float *o0 = out + a * stride, *o1 = o0 + 8 * ncol;
 #pragma unroll
         for (int i = 0; i < 16; ++i) {
-            const float v = SCALED ? ldexpf(acc[a][i], e) : acc[a][i];
+            float v = acc[a][i] * s1;
+            if (more) v = v * s2 * s3;
             float &d = ((i >> 1) & 1 ? o1 : o0)[8 * (i >> 2) + (i & 1)];
             d = first ? v : d + v;
             acc[a][i] = 0.f;
@@ -139,20 +146,20 @@ __device__ __forceinline__ void wgrad_flush(float (&acc)[NA][16], float *blk, in
     }
 }
 
-// dW [Cout][C][3][3] = 2^-sg * (slot 0 + slot 1 + ...), always in that order; one thread per slot column, so the reads
+// dW [Cout][C][3][3] = slot 0 + slot 1 + ..., always in that order (the kernels' flushes have divided every operand
+// exponent out); one thread per slot column, so the reads
 // are coalesced (conv3x3_wgrad.cu; grid-stride over Cout * ncol)
 __global__ void wgrad_reduce_kernel(const float *__restrict__ ws, int nslots, int C, int Cout, int cpg, int co_pad,
-                                    int ncol, const unsigned *__restrict__ gy_amax, float *__restrict__ dw);
+                                    int ncol, float *__restrict__ dw);
 
 __device__ __forceinline__ int operand_exp(const unsigned *amax, int b) { return amax ? amax_exp(amax[b], 11) : 0; }
 __device__ __forceinline__ int mask_exp(const unsigned *amax, int b) { return amax ? amax_exp(amax[b], 0) : 0; }
 
 // fp32 [B,C,H,W] (element strides) -> PSA x * 2^sa, or, when amax is not null, image b times
-// 2^grad_scale_exp(amax + b * amax_step): one exponent for the batch (amax_step 0) or one per image (1)
-// (conv3x3_umma.cu; grid (blocks, B))
+// 2^grad_scale_exp(amax + b) (conv3x3_umma.cu; grid (blocks, B))
 __global__ void psa_from_f32_kernel(const float *__restrict__ x, int C, int C8, int H, int W, long long xs_b,
                                     long long xs_c, long long xs_y, long long xs_x, int sa,
-                                    const unsigned *__restrict__ amax, int amax_step, __half *__restrict__ hi,
+                                    const unsigned *__restrict__ amax, __half *__restrict__ hi,
                                     __half *__restrict__ lo);
 // Largest finite |g| of a strided [B,C,H,W] tensor as fp32 bits (NaN and Inf do not set the scale), of the whole batch
 // into amax[0] (amax_step 0) or image by image into amax[b] (1); the outputs start at 0 (conv3x3_wgrad.cu; grid

@@ -50,7 +50,9 @@ enum {
     C2M_ERR_UNSUPPORTED = 4   /* no sm_90 device / driver entry point missing */
 };
 
-int c2m_abi_version(void);      /* 6 since the fp32 c2m_dcn_v2_* twins of c2m_deform_conv_* are gone (5: c2m_dcn_tc_args
+int c2m_abi_version(void);      /* 7 since grad_output takes one exponent per image: gy_amax holds [B] values,
+                                 * c2m_grad_psa_from_f32 and c2m_grad_unscale_f32 are gone (6: the fp32 c2m_dcn_v2_*
+                                 * twins of c2m_deform_conv_* are gone; 5: c2m_dcn_tc_args
                                  * takes only x_il; 4: .x_il / c2m_psa_interleave; 3: .mask; 2: out_f32_octets /
                                  * om_octets).  Later additions (c2m_dcn_tc_args.x_amax / .mask_amax,
                                  * c2m_dcn_tc_operand_*, c2m_conv3x3_args.x_amax with c2m_conv3x3_operand_f32 and
@@ -191,31 +193,25 @@ int c2m_psa_from_f32(const float *x, int B, int C, int H, int W, long long xs_b,
 int c2m_psa_to_f32(const void *hi, const void *lo, int B, int C, int H, int W, int sa, const float *add, float *out,
                    long long os_b, long long os_c, long long os_y, long long os_x, c2m_stream_t stream);
 int c2m_conv3x3(const c2m_conv3x3_args *args, c2m_stream_t stream);
-/* Operand of the differentiable convolution: x [B,C,H,W] fp32 (element strides) of any magnitude -> PSA hi / lo holding
+/* Operand of the differentiable convolution, for x and for grad_output: x [B,C,H,W] fp32 (element strides) of any magnitude -> PSA hi / lo holding
  * image b times 2^sa_b, sa_b = 14 - floor(log2 amax[b]), where amax[b], the largest finite |x| of image b (NaN and Inf
  * do not count; 0 gives sa_b = 0; sa_b is clamped to +-120), is computed on the device and its fp32 bits stored in
  * amax[0, B) (device memory).  Pass amax as c2m_conv3x3_args.x_amax and to c2m_conv3x3_wgrad_scaled.  Scaling an image by
- * 2^k leaves its PSA planes bit for bit the same, so the output and dW scale by exactly 2^k while in range. */
+ * 2^k leaves its PSA planes bit for bit the same, so the output and the gradients scale by exactly 2^k while in range. */
 int c2m_conv3x3_operand_f32(const float *x, int B, int C, int H, int W, long long xs_b, long long xs_c, long long xs_y,
                             long long xs_x, void *hi, void *lo, unsigned *amax, c2m_stream_t stream);
 /* Backward of the convolution above (3x3 / stride 1 / pad 1, one input), fp32-grade, no host synchronisation.
- * c2m_grad_psa_from_f32: grad_output g [B,C,H,W] fp32 (element strides) -> PSA hi / lo holding g * 2^sg, where
- *   sg = 14 - floor(log2 amax) and amax, the largest finite |g| (NaN and Inf do not count; 0 gives sg = 0; sg is
- *   clamped to +-120), is computed on the device and its fp32 bits stored in *amax (device memory, 4 bytes).  Scaling
- *   g by 2^k leaves the PSA planes bit for bit the same, so the gradients below scale by exactly 2^k while in range.
- * Input gradient: c2m_conv3x3 of that PSA tensor (sa_in = 0, Cin = the forward's Cout, Cout = the forward's Cin) with
- *   the weights W'[ci][co][ky][kx] = W[co][ci][2-ky][2-kx] packed by c2m_conv3x3_pack_weights_f32, fp32 output, then
- *   c2m_grad_unscale_f32 on that output: x[i] *= 2^-sg for n elements.
+ * grad_output g [B,C,H,W] enters as c2m_conv3x3_operand_f32(g, ..., hi, lo, gy_amax): one exponent per image, so an
+ * image's gradients do not depend on the other images' magnitudes.
+ * Input gradient: c2m_conv3x3 of that PSA tensor with x_amax = gy_amax (Cin = the forward's Cout, Cout = the forward's
+ *   Cin) and the weights W'[ci][co][ky][kx] = W[co][ci][2-ky][2-kx] packed by c2m_conv3x3_pack_weights_f32, fp32 output.
  * c2m_conv3x3_wgrad: dW[co][ci][ky][kx] = sum over b, y, x of g[b,co,y,x] * x[b,ci,y+ky-1,x+kx-1] (zero outside the
- *   map), written to dw [Cout,Cin,3,3] fp32.  gy_* / gy_amax: the output of c2m_grad_psa_from_f32; x_*: the forward's
+ *   map), written to dw [Cout,Cin,3,3] fp32.  gy_* / gy_amax ([B]): the output of c2m_conv3x3_operand_f32; x_*: the forward's
  *   input as PSA at scale exponent 0 (c2m_conv3x3_wgrad) or, with x_amax, the output of c2m_conv3x3_operand_f32
  *   (c2m_conv3x3_wgrad_scaled).  Only pixels inside the map contribute, also next to a non-finite x.  Split-K over CTAs with per-CTA partials in `ws` (at least
  *   c2m_conv3x3_wgrad_workspace_bytes(B, Cin, Cout, H, W) bytes, which depends on the device's SM count), summed in one
  *   fixed order: the same bits on every run on a given device.  Needs H >= 18 and W >= 10, like c2m_conv3x3.
  */
-int c2m_grad_psa_from_f32(const float *g, int B, int C, int H, int W, long long gs_b, long long gs_c, long long gs_y,
-                          long long gs_x, void *hi, void *lo, unsigned *amax, c2m_stream_t stream);
-int c2m_grad_unscale_f32(float *x, long long n, const unsigned *amax, c2m_stream_t stream);
 size_t c2m_conv3x3_wgrad_workspace_bytes(int B, int Cin, int Cout, int H, int W);   /* 0 on a bad shape */
 int c2m_conv3x3_wgrad(const void *gy_hi, const void *gy_lo, const unsigned *gy_amax, const void *x_hi, const void *x_lo,
                       int B, int Cin, int Cout, int H, int W, float *dw, void *ws, size_t ws_bytes,
@@ -277,7 +273,8 @@ int c2m_dcn_tc_operand_f32(const float *x, int B, int C, int H, int W, long long
 
 /* --- Backward of the tensor-core DCN (the `_ext` contract: final offsets and final mask) -------------------------
  * Same shapes as c2m_dcn_v2_fused_tc (c2m_dcn_tc_supported), maps of at least 16 x 8.  Inputs:
- *   gy_hi / gy_lo / gy_amax   grad_output [B,Cout,H,W] as PSA at the scale of c2m_grad_psa_from_f32
+ *   gy_hi / gy_lo / gy_amax   grad_output [B,Cout,H,W] as c2m_conv3x3_operand_f32 writes it: PSA image b times
+ *                             2^sg_b, gy_amax [B]
  *   x_il, x_amax, mask_amax   the forward's operand: c2m_dcn_tc_operand_f32(x, ..., mask, x_il, amax) with
  *                             x_amax = amax, mask_amax = amax + B
  *   offset, mask              final offsets [B,2*dg*9,H,W] and final mask [B,dg*9,H,W], contiguous fp32
@@ -289,7 +286,7 @@ int c2m_dcn_tc_operand_f32(const float *x, int B, int C, int H, int W, long long
  * c2m_dcn_tc_wgrad_workspace_bytes(B, C, H, W, Cout, dg) bytes (0 on bad arguments; it queries the current device). */
 typedef struct {
     const void *gy_hi, *gy_lo;
-    const unsigned *gy_amax;
+    const unsigned *gy_amax;     /* [B] */
     const void *x_il;
     const unsigned *x_amax, *mask_amax;
     const float *offset, *mask;

@@ -7,6 +7,7 @@ the same case).  The activation's mask is the op's own forward output (y > 0): t
 pre-activation within rounding of 0 that changes sign is not a backward error.  Also: exact 2^k scaling, bitwise
 repeatability, sentinel guards around every buffer the new entry points write, non-finite propagation, and one
 RestorationNet training step on both paths."""
+import ctypes
 import math
 
 import pytest
@@ -147,10 +148,11 @@ def _guards_intact(buf, dtype):
 
 @pytest.mark.parametrize('case', [(2, 40, 72, 19, 11, None), (1, 64, 64, 130, 70, None), (3, 3, 3, 18, 10, None)],
                          ids=_ids)
-def test_backward_with_image_exponents_writes_stay_in_bounds(case):
-    """Every buffer the backward's entry points write (the PSA gradient, its amax, dW from the forward's per-image
-    operand through c2m_conv3x3_wgrad_scaled, the workspace, the unscaled dX) sits between sentinel guards that must
-    come back untouched; the results must equal the op's."""
+def test_backward_with_per_image_grad_exponents_writes_stay_in_bounds(case):
+    """Every buffer the backward's entry points write (the PSA gradient and its per-image amax from
+    c2m_conv3x3_operand_f32, dW from the forward's per-image operand through c2m_conv3x3_wgrad_scaled, the workspace,
+    dX from c2m_conv3x3 with the gradient's exponents) sits between sentinel guards that must come back untouched; the
+    results must equal the op's."""
     from c2m_b200 import _lib, ops
     B, cin, cout, H, W, _ = case
     x, w, b, gy = _inputs(case, 400)
@@ -159,11 +161,11 @@ def test_backward_with_image_exponents_writes_stay_in_bounds(case):
     c8o, c8i = (cout + 7) // 8, (cin + 7) // 8
     npsa = B * c8o * H * W * 8
     ghi, glo = _guarded(npsa, torch.float16), _guarded(npsa, torch.float16)
-    amax = _guarded(1, torch.float32)
+    amax = _guarded(B, torch.float32)
     st = torch.cuda.current_stream().cuda_stream
-    rc = L.c2m_grad_psa_from_f32(gy.data_ptr(), B, cout, H, W, *gy.stride(), ghi[GUARD:].data_ptr(),
-                                 glo[GUARD:].data_ptr(), amax[GUARD:].data_ptr(), st)
-    _lib.check(rc, 'c2m_grad_psa_from_f32')
+    rc = L.c2m_conv3x3_operand_f32(gy.data_ptr(), B, cout, H, W, *gy.stride(), ghi[GUARD:].data_ptr(),
+                                   glo[GUARD:].data_ptr(), amax[GUARD:].data_ptr(), st)
+    _lib.check(rc, 'c2m_conv3x3_operand_f32')
     xp, x_amax = ops._conv3x3_operand(x)
     assert xp.hi.numel() == B * c8i * H * W * 8
     nws = L.c2m_conv3x3_wgrad_workspace_bytes(B, cin, cout, H, W)
@@ -175,18 +177,17 @@ def test_backward_with_image_exponents_writes_stay_in_bounds(case):
                              ws[GUARD:].data_ptr(), nws, st)
     _lib.check(rc, 'c2m_conv3x3_wgrad_scaled')
     dxs = _guarded(x.numel(), torch.float32)
-    gp = ops.PSA(ghi[GUARD:GUARD + npsa].view(B, c8o, H, W, 8), glo[GUARD:GUARD + npsa].view(B, c8o, H, W, 8),
-                 B, cout, H, W)
-    dx_scaled = ops.conv3x3_psa(gp, w.transpose(0, 1), None, psa_out=False, out_f32=True,
-                                packed=ops.conv3x3_pack_weights(w, dgrad=True))
-    dxs[GUARD:GUARD + x.numel()].copy_(dx_scaled.flatten())
-    rc = L.c2m_grad_unscale_f32(dxs[GUARD:].data_ptr(), x.numel(), amax[GUARD:].data_ptr(), st)
-    _lib.check(rc, 'c2m_grad_unscale_f32')
+    a = _lib.ConvArgs()
+    a.in_hi, a.in_lo, a.Cin, a.B, a.H, a.W = ghi[GUARD:].data_ptr(), glo[GUARD:].data_ptr(), cout, B, H, W
+    a.packed_w, a.Cout = ops.conv3x3_pack_weights(w, dgrad=True).data_ptr(), cin
+    a.out_f32, a.x_amax = dxs[GUARD:].data_ptr(), amax[GUARD:].data_ptr()
+    a.os_b, a.os_c, a.os_y, a.os_x = cin * H * W, H * W, W, 1
+    _lib.check(L.c2m_conv3x3(ctypes.addressof(a), st), 'c2m_conv3x3')
     torch.cuda.synchronize()
     for buf, dt in ((ghi, torch.float16), (glo, torch.float16), (dw, torch.float32), (ws, torch.float32),
                     (dxs, torch.float32)):
         assert _guards_intact(buf, dt)
-    assert bool(amax[:GUARD].isnan().all()) and bool(amax[GUARD + 1:].isnan().all())
+    assert bool(amax[:GUARD].isnan().all()) and bool(amax[GUARD + B:].isnan().all())
     assert torch.equal(dw[GUARD:GUARD + dw_op.numel()].view_as(dw_op), dw_op)
     assert torch.equal(dxs[GUARD:GUARD + x.numel()].view_as(dx_op), dx_op)
 

@@ -307,7 +307,7 @@ def _guards_intact(buf, n):
 
 
 @pytest.mark.parametrize('shape', [(2, 40, 72, 19, 11), (3, 3, 48, 21, 13)], ids=['40to72_19x11', '3to48_21x13'])
-def test_operand_and_kernels_write_inside_their_buffers(shape):
+def test_operand_and_kernels_write_inside_their_buffers_per_image_grad(shape):
     """c2m_conv3x3_operand_f32 (the PSA operand and its per-image amax), the forward with those exponents (fp32 output)
     and c2m_conv3x3_wgrad_scaled with them (dW, workspace) write only inside their buffers, between sentinel guards, and give
     the op's results bit for bit."""
@@ -331,7 +331,7 @@ def test_operand_and_kernels_write_inside_their_buffers(shape):
     a.out_f32, a.x_amax = y[GUARD:].data_ptr(), amax[GUARD:].data_ptr()
     a.os_b, a.os_c, a.os_y, a.os_x = cout * H * W, H * W, W, 1
     _lib.check(L.c2m_conv3x3(ctypes.addressof(a), st), 'c2m_conv3x3')
-    gp, gamax = ops._grad_psa(gy)
+    gp, gamax = ops._conv3x3_operand(gy)
     nws = L.c2m_conv3x3_wgrad_workspace_bytes(B, cin, cout, H, W)
     ws, dw = _guarded(nws // 4, torch.float32), _guarded(cout * cin * 9, torch.float32)
     _lib.check(L.c2m_conv3x3_wgrad_scaled(gp.hi.data_ptr(), gp.lo.data_ptr(), gamax.data_ptr(), xp.hi.data_ptr(),

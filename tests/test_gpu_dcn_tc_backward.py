@@ -175,8 +175,9 @@ def test_nonfinite_pattern_matches_oracle(where):
         assert torch.equal(torch.isfinite(m).cpu(), torch.isfinite(r)), where
 
 
-def test_no_writes_outside_buffers():
-    """Sentinels around grad_offset, grad_mask, grad_input and grad_weight of both entry points."""
+def test_no_writes_outside_buffers_per_image_grad():
+    """Sentinels around grad_output's per-image amax, and around grad_offset, grad_mask, grad_input and grad_weight of
+    both entry points."""
     from c2m_b200 import _lib, ops
     L = _lib.lib()
     case = (2, 64, 40, 19, 11, 8, 'small', 'sig')
@@ -184,9 +185,10 @@ def test_no_writes_outside_buffers():
     B, C, H, W, cout, dg = 2, 64, 19, 11, 40, 8
     pad = 4096
     gp = ops.PSA.empty(B, cout, H, W, DEV)
-    gamax = torch.empty(1, dtype=torch.int32, device=DEV)
-    _lib.check(L.c2m_grad_psa_from_f32(gy.data_ptr(), B, cout, H, W, *gy.stride(), gp.hi.data_ptr(), gp.lo.data_ptr(),
-                                       gamax.data_ptr(), ops._stream()), 'psa')
+    gamax_full = torch.full((B + 2 * pad,), -12345, dtype=torch.int32, device=DEV)
+    gamax = gamax_full[pad:pad + B]
+    _lib.check(L.c2m_conv3x3_operand_f32(gy.data_ptr(), B, cout, H, W, *gy.stride(), gp.hi.data_ptr(),
+                                         gp.lo.data_ptr(), gamax.data_ptr(), ops._stream()), 'psa')
     x_il = torch.empty(L.c2m_dcn_tc_operand_bytes(B, C, H, W, dg) // 2, dtype=torch.float16, device=DEV)
     amax = torch.empty(2 * B, dtype=torch.int32, device=DEV)
     _lib.check(L.c2m_dcn_tc_operand_f32(x.data_ptr(), B, C, H, W, *x.stride(), dg, mask.data_ptr(), x_il.data_ptr(),
@@ -214,6 +216,7 @@ def test_no_writes_outside_buffers():
     for k, (full, _) in bufs.items():
         assert bool((full[:pad] == 12345.0).all()) and bool((full[-pad:] == 12345.0).all()), k
     assert bool((ws_full[:pad] == 12345.0).all()) and bool((ws_full[pad + n // 4:] == 12345.0).all())
+    assert bool((gamax_full[:pad] == -12345).all()) and bool((gamax_full[pad + B:] == -12345).all())
 
 
 def _training_setup():

@@ -29,7 +29,7 @@ def _header_functions():
     return sorted(set(re.findall(r'\b(c2m_[a-z0-9_]+)\s*\(', src)))
 
 
-def test_library_exports_every_declared_symbol_of_abi_6(built):
+def test_library_exports_every_declared_symbol_of_abi_7(built):
     declared = _header_functions()
     assert 'c2m_corr_argmax_f32' in declared and 'c2m_deform_conv_forward_f32' in declared
     out = subprocess.run(['nm', '-D', '--defined-only', built.LIB_PATH], capture_output=True, text=True, check=True).stdout
@@ -37,7 +37,7 @@ def test_library_exports_every_declared_symbol_of_abi_6(built):
     assert set(declared) <= exported, set(declared) - exported
     assert set(built.SYMBOLS) == set(declared)          # the ctypes table binds all of them
     lib = built.lib()
-    assert lib.c2m_abi_version() == 6
+    assert lib.c2m_abi_version() == 7
 
 
 def test_sass_is_hopper_native(built):

@@ -73,7 +73,7 @@ def shape_times(cin, cout, H, iters, warmup):
     st = torch.cuda.current_stream().cuda_stream
     xp, x_amax = ops._conv3x3_operand(x)
     gp = ops.PSA.empty(B, cout, H, H, dev)
-    amax = torch.empty(1, dtype=torch.int32, device=dev)
+    amax = torch.empty(B, dtype=torch.int32, device=dev)
     wt = w.transpose(0, 1)
     blob = ops.conv3x3_pack_weights(w, dgrad=True)
     nws = L.c2m_conv3x3_wgrad_workspace_bytes(B, cin, cout, H, H)
@@ -81,13 +81,12 @@ def shape_times(cin, cout, H, iters, warmup):
     dw = torch.empty_like(w)
 
     def convert():
-        _lib.check(L.c2m_grad_psa_from_f32(gy.data_ptr(), B, cout, H, H, *gy.stride(), gp.hi.data_ptr(),
-                                           gp.lo.data_ptr(), amax.data_ptr(), st), 'grad_psa')
+        _lib.check(L.c2m_conv3x3_operand_f32(gy.data_ptr(), B, cout, H, H, *gy.stride(), gp.hi.data_ptr(),
+                                             gp.lo.data_ptr(), amax.data_ptr(), st), 'grad_psa')
 
     def tc_dx():
         convert()
-        dx = ops.conv3x3_psa(gp, wt, None, psa_out=False, out_f32=True, packed=blob)
-        _lib.check(L.c2m_grad_unscale_f32(dx.data_ptr(), dx.numel(), amax.data_ptr(), st), 'unscale')
+        ops.conv3x3_psa(gp, wt, None, psa_out=False, out_f32=True, packed=blob, x_amax=amax)
 
     def tc_dw():
         _lib.check(L.c2m_conv3x3_wgrad_scaled(gp.hi.data_ptr(), gp.lo.data_ptr(), amax.data_ptr(), xp.hi.data_ptr(),

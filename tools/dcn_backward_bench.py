@@ -85,14 +85,14 @@ def conversion(x, mask, gy, reps, dg=8):
     L = _lib.lib()
     B, C, H, W = x.shape
     gp = ops.PSA.empty(B, C, H, W, x.device)
-    gamax = torch.empty(1, dtype=torch.int32, device=x.device)
+    gamax = torch.empty(B, dtype=torch.int32, device=x.device)
     x_il = torch.empty(L.c2m_dcn_tc_operand_bytes(B, C, H, W, dg) // 2, dtype=torch.float16, device=x.device)
     amax = torch.empty(2 * B, dtype=torch.int32, device=x.device)
     st = ops._stream()
 
     def run():
-        _lib.check(L.c2m_grad_psa_from_f32(gy.data_ptr(), B, C, H, W, *gy.stride(), gp.hi.data_ptr(),
-                                           gp.lo.data_ptr(), gamax.data_ptr(), st), 'grad_psa_from_f32')
+        _lib.check(L.c2m_conv3x3_operand_f32(gy.data_ptr(), B, C, H, W, *gy.stride(), gp.hi.data_ptr(),
+                                             gp.lo.data_ptr(), gamax.data_ptr(), st), 'conv3x3_operand_f32')
         _lib.check(L.c2m_dcn_tc_operand_f32(x.data_ptr(), B, C, H, W, *x.stride(), dg, mask.data_ptr(),
                                             x_il.data_ptr(), amax.data_ptr(), st), 'dcn_tc_operand_f32')
     return _time(run, reps)
