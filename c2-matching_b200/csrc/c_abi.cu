@@ -110,11 +110,18 @@ static void carve(CorrWorkspace &ws, const CorrGeom &g, uint8_t *base) {
     ws.ovf = (CorrOverflow *)take((size_t)g.B * g.NQ * sizeof(CorrOverflow));
     ws.best = (unsigned long long *)take((size_t)g.B * g.NQ * 8);
     ws.qnorm = (float *)take((size_t)g.B * g.NQ * 4);
-    ws.amax_bits = (unsigned *)take(256);            // zeroed at the start of every call
-    ws.sexp = (int *)(ws.amax_bits ? ws.amax_bits + 8 : nullptr);
-    ws.ovf_count = ws.amax_bits ? ws.amax_bits + 16 : nullptr;
-    ws.max_pn_bits = ws.amax_bits ? ws.amax_bits + 17 : nullptr;
-    ws.rinv_max_bits = ws.amax_bits ? ws.amax_bits + 18 : nullptr;
+    ws.qnorm_s = (float *)take((size_t)g.B * g.NQ * 4);
+    ws.flag_ref = (int *)take((size_t)g.B * g.NR * 4);
+    // control block, zeroed at the start of every call: amax [2B], sexp [2B], ovf_count [2], pr_max [B], rinv_max [B],
+    // flag_count [B]
+    ws.ctl_bytes = (size_t)(7 * g.B + 2) * 4;
+    unsigned *ctl = (unsigned *)take(ws.ctl_bytes);
+    ws.amax_bits = ctl;
+    ws.sexp = ctl ? (int *)(ctl + 2 * g.B) : nullptr;
+    ws.ovf_count = ctl ? ctl + 4 * g.B : nullptr;
+    ws.pr_max_bits = ctl ? ctl + 4 * g.B + 2 : nullptr;
+    ws.rinv_max_bits = ctl ? ctl + 5 * g.B + 2 : nullptr;
+    ws.flag_count = ctl ? ctl + 6 * g.B + 2 : nullptr;
     ws.total_bytes = off;
 }
 
@@ -155,7 +162,7 @@ extern "C" int c2m_corr_argmax_f32(const float *fin, const float *fref, int B, i
         return C2M_ERR_WORKSPACE;
     }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    C2M_CUDA(cudaMemsetAsync(ws.amax_bits, 0, 256, st));
+    C2M_CUDA(cudaMemsetAsync(ws.amax_bits, 0, ws.ctl_bytes, st));
 
     const bool use_umma = !(flags & 1u) && corr_umma_supported(g);
     CorrChunkGeom cg;
@@ -173,17 +180,18 @@ extern "C" int c2m_corr_argmax_f32(const float *fin, const float *fref, int B, i
         }
         ws.nchunk = corr_umma_pick_nchunk(g, sms);
         corr_umma_chunk_geom(g, ws.nchunk, cg);
-        // DESIGN.md K2: the search scores (q_hi + q_lo) . r_hi.  |approx - exact| <= E = [2^-11 + 2^-22 (K/16 + 3)] ||P_q||
-        // ||P_r|| rinv_r + E_sub: 2^-11 = fp16 rounding of the Ref operand (Cauchy-Schwarz over the patch), K/16 wgmma
-        // instructions feed each score with 1 fp32 ulp of (|acc| + sum|products|) each, + the query's 2^-22 split.
-        // Window = 2E for the rounding part (best and candidate both err; 1 % margin) and 4E for the accumulation part
-        // (x2 of slack for the tensor core's internal alignment).
-        // E_sub: one scale exponent per map and call (|x| 2^sexp <= 1024 for the largest |x| of the whole batch) puts
+        // DESIGN.md K2, everything in search units (scores times 2^u, operands times their image's 2^sexp, rinv_r the
+        // column scale; corr_internal.cuh): the search scores (q_hi + q_lo) . r_hi.  |approx - exact| <= E =
+        // [2^-11 + 2^-22 (K/16 + 3)] ||P_q|| ||P_r|| rinv_r + E_sub: 2^-11 = fp16 rounding of the Ref operand
+        // (Cauchy-Schwarz over the patch), K/16 wgmma instructions feed each score with 1 fp32 ulp of
+        // (|acc| + sum|products|) each, + the query's 2^-22 split.  Window = 2E for the rounding part (best and candidate
+        // both err; 1 % margin) and 4E for the accumulation part (x2 of slack for the tensor core's internal alignment).
+        // E_sub: one scale exponent per map and image (|x| 2^sexp <= 1024 for the image's largest finite |x|) puts
         // elements far below that maximum into the fp16 subnormals, whose rounding is absolute: up to 2^-25 per element
-        // of r_hi and of q_hi + q_lo, i.e. sqrt(K) 2^-25 over a patch.  E_sub = sqrt(K) 2^-25 [2^-sexp_in ||P_r|| rinv_r
-        // + ||P_q|| 2^-sexp_ref rinv_r], with ||P_r|| rinv_r <= 1 (max ||P_r|| for raw scores) and rinv_r <= the largest
-        // rinv of a nonzero Ref patch (an all-zero patch rounds exactly).  With l2norm (sexp = 10, pixel norms 1 or 0)
-        // it is ~1e-6 of the window.
+        // of r_hi and of q_hi + q_lo, i.e. sqrt(K) 2^-25 over a patch.  E_sub = sqrt(K) 2^-25 [||P_r|| rinv_r
+        // + ||P_q|| rinv_r], with ||P_r|| rinv_r <= P (the image's largest ||P_r|| rinv_r, <= 1 when normalised) and
+        // rinv_r <= R (the image's largest rinv of a nonzero Ref patch; an all-zero patch rounds exactly).  With l2norm
+        // (sexp = 10, pixel norms 1 or 0) it is ~1e-6 of the window.
         window_coef = 1.01f * ldexpf(1.f, -10) + ldexpf(1.f, -20) * (float)((K + 15) / 16 + 3);
         sub_coef = 1.01f * ldexpf(1.f, -24) * sqrtf((float)(g.Cp * g.patch * g.patch));
     } else {
@@ -194,7 +202,8 @@ extern "C" int c2m_corr_argmax_f32(const float *fin, const float *fref, int B, i
         if (n < 1) n = 1;
         ws.nchunk = n;
         corr_generic_chunk_geom(g, ws.nchunk, cg);
-        // sequential fp32 FMA chain of K terms: |approx - exact| <= K * 2^-24 * ||P_q|| * ||P_r|| * rinv_r (+ the final scale)
+        // sequential fp32 FMA chain of K terms on the scaled operands: |approx - exact| <= K * 2^-24 * ||P_q|| * ||P_r||
+        // * rinv_r (+ the final scale) in search units, + the underflow floor that corr_rescore_launch adds to both searches
         window_coef = ldexpf(1.f, -23) * (float)(K + 4);
     }
 

@@ -3,16 +3,25 @@
 // Data layout in HBM (per feature map of one call, all images b of the batch):
 //   p32   [B][HW][Cp]        fp32, pixel-major ("NHWC"), Cp = C rounded up to 8, pad = 0.
 //                            Exact values the search is defined on (optionally L2-normalised).
-//   hi,lo [B][Cp/8][HW][8]   fp16 split operands of x * 2^sexp:  hi = rn(x*S), lo = rn(x*S - hi).
+//   hi,lo [B][Cp/8][HW][8]   fp16 split operands of x * 2^sexp[b] (one exponent per map and image):  hi = rn(x*S),
+//                            lo = rn(x*S - hi); a non-finite element is written as 0 (its pixel is flagged by ss).
 //                            One 16-byte element per (channel-octet, pixel): a (W*8)-wide row of
 //                            one image row is contiguous, so a TMA box of (cols*8, rows, octets)
 //                            lands in shared memory as [octet][pixel][8 halfs] = the wgmma
 //                            K-major no-swizzle core-matrix layout with rows 16 B apart.
-//   ss    [B][HW]            fp32 per-pixel sum of squares of p32 (for the patch norms).
-//   rinv  [B][NR]            fp32 1 / (sqrt(sum_{patch} ss) + 1e-5)   (1 when !is_norm)
+//   ss    [B][HW]            fp32 per-pixel sum of squares of p32 * 2^sexp[b]: non-finite iff the pixel holds a
+//                            non-finite element (the scaled finite elements are <= 1024, their squares cannot overflow).
+//   rinv  [B][NR]            fp32 Ref column scale in SEARCH UNITS (see below): 1 / (||P_r|| 2^sexp_ref + 1e-5 2^sexp_ref)
+//                            when is_norm, 1 otherwise; NaN for a Ref patch holding a non-finite element (those are
+//                            listed in flag_ref and scored exactly for every query by the rescoring).
+//   Search units: both searches score s~ * 2^u, u = sexp_in[b] (+ sexp_ref[b] for raw scores), from the scaled operands,
+//   so no product of scales can leave the fp32 range.  u is constant per query, so the ranking is that of s~; the
+//   rescoring window is formed in the same units from the scaled norms.
 //   part  [B][nchunk][NQ]    Candidate: approximate top-8 (tensor cores) / top-4 (FFMA) of each query over one Ref chunk (nchunk <= 32).
 //   ovf   [B*NQ]             (query, chunk bit mask) of the (query, chunk) pairs whose top-2 list may be incomplete:
-//                            the exhaustive pass re-scans those chunks exactly (see corr_aux.cu).
+//                            the exhaustive pass re-scans those chunks exactly (see corr_aux.cu).  Filled from the
+//                            front (subject to the re-scan budget) and, for queries whose patch holds a non-finite
+//                            element (every chunk, always re-scanned), from the back.
 #pragma once
 #include "c2m_common.cuh"
 
@@ -59,11 +68,16 @@ struct CorrWorkspace {
     CorrOverflow *ovf;       // [B*NQ] overflow list
     unsigned long long *best;   // [B*NQ] packed (exact score, index) of the best candidate so far (best_key)
     float *qnorm;            // [B*NQ] ||P_query|| (exact, deterministic)
-    unsigned *amax_bits;     // [2]
-    int *sexp;               // [2] scale exponents for (in, ref)
-    unsigned *ovf_count;     // [1] entries in ovf
-    unsigned *max_pn_bits;   // [1] max over Ref patches of ||P_ref|| (float bits) — window scale when !is_norm
-    unsigned *rinv_max_bits; // [1] max of rinv over Ref patches with nonzero norm (float bits)
+    float *qnorm_s;          // [B*NQ] ||P_query|| 2^sexp_in (the window's query scale in search units)
+    int *flag_ref;           // [B][NR] Ref patches holding a non-finite element (the first flag_count[b] entries)
+    // control block, zeroed at the start of every call (ctl .. ctl + ctl_bytes):
+    unsigned *amax_bits;     // [2][B] largest finite |x| per (map, image) (float bits)
+    int *sexp;               // [2][B] scale exponents per (map, image): in, ref
+    unsigned *ovf_count;     // [2] entries in ovf: [0] from the front, [1] from the back
+    unsigned *pr_max_bits;   // [B] max over finite Ref patches of ||P_ref|| 2^sexp_ref rinv (float bits): the window's Ref factor
+    unsigned *rinv_max_bits; // [B] max of rinv over finite Ref patches with nonzero norm (float bits)
+    unsigned *flag_count;    // [B] entries in flag_ref
+    size_t ctl_bytes;
     int nchunk;
     size_t total_bytes;
 };
@@ -109,14 +123,17 @@ __device__ __forceinline__ Candidate cand_pack(const float (&v)[K], const int (&
     c.pad[0] = c.pad[1] = c.pad[2] = 0.f;
     return c;
 }
-__device__ __forceinline__ bool cand_better(float s, int r, float v, int i) {   // exact scores: lower index wins ties
-    return s > v || (s == v && r < i);
+// exact scores, torch's max rule: NaN is the maximum, then larger; the lower index wins ties (and among NaNs)
+__device__ __forceinline__ bool cand_better(float s, int r, float v, int i) {
+    if (s != s) return v == v || r < i;
+    return s > v || (s == v && r < i);          // v NaN: both false
 }
 
-// (score, index) packed so that an unsigned 64-bit max is the lexicographic "better": larger score, then LOWER index
+// (score, index) packed so that an unsigned 64-bit max is cand_better: NaN (one key, whatever its sign and payload)
+// above everything, then larger score (-0 as +0), then LOWER index
 __device__ __forceinline__ unsigned long long best_key(float s, int r) {
-    const unsigned b = __float_as_uint(s);
-    const unsigned ord = (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+    const unsigned b = __float_as_uint(s == 0.f ? 0.f : s);
+    const unsigned ord = s != s ? 0xffffffffu : (b & 0x80000000u) ? ~b : (b | 0x80000000u);
     return ((unsigned long long)ord << 32) | (unsigned long long)(0xffffffffu - (unsigned)r);
 }
 __device__ __forceinline__ void best_unkey(unsigned long long k, float &s, int &r) {
@@ -135,7 +152,7 @@ bool corr_umma_supported(const CorrGeom &g);
 int corr_umma_pick_nchunk(const CorrGeom &g, int sms);
 void corr_umma_chunk_geom(const CorrGeom &g, int nchunk, CorrChunkGeom &cg);
 void corr_generic_chunk_geom(const CorrGeom &g, int nchunk, CorrChunkGeom &cg);
-// window_coef: rigorous bound on 2 x |approximate - exact score| per unit of ||P_query|| (see corr_aux.cu);
+// window_coef: rigorous bound on 2 x |approximate - exact score| per unit of ||P_query|| (search units, see corr_aux.cu);
 // sub_coef: the same for the absolute rounding of fp16-subnormal operand elements (0 for the fp32 search, see c_abi.cu)
 int corr_rescore_launch(const CorrGeom &g, const CorrWorkspace &ws, const CorrChunkGeom &cg, float window_coef,
                         float sub_coef, int is_norm, int norm_input, int64_t *idx, float *val, cudaStream_t st);

@@ -17,7 +17,7 @@
 // row, so a warp's 32 threads are exactly two 16-px block rows and the diagonal sum is two __shfl_down per score.
 // Tile efficiency (14/16)^2 = 0.77, i.e. 2.3x fewer MMA cycles per score than issuing all nine taps.
 //
-// Precision.  Operands are split fp16 pairs of x*2^sexp (hi + lo, 22 mantissa bits); each K step
+// Precision.  Operands are split fp16 pairs of x*2^sexp[b] (hi + lo, 22 mantissa bits); each K step
 // issues q_hi*r_hi + q_lo*r_hi into the same fp32 accumulator (M=128, N=128).  The scores
 // only RANK candidates: the epilogue keeps a top-8 per (query, Ref chunk) and the exact rescoring kernel
 // (corr_aux.cu) decides, so tensor-core rounding cannot leak into the index map; corr_aux.cu states the error
@@ -66,7 +66,7 @@ struct UmmaParams {
 __global__ void __launch_bounds__(512, 1)
 corr_umma_kernel(const __grid_constant__ CUtensorMap tm_in_hi, const __grid_constant__ CUtensorMap tm_in_lo,
                  const __grid_constant__ CUtensorMap tm_ref_hi,
-                 const float *__restrict__ rinv, const int *__restrict__ sexp, Candidate *__restrict__ part,
+                 const float *__restrict__ rinv, Candidate *__restrict__ part,
                  const UmmaParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -169,7 +169,6 @@ corr_umma_kernel(const __grid_constant__ CUtensorMap tm_in_hi, const __grid_cons
         // left behind; the rescoring pass re-scans the chunk exhaustively when `dropped` reaches its window.
         const int e = threadIdx.x - 128;                    // 0..127 = accumulator row m = 16 * block row + block column
         const int yy = e >> 4, xx = e & 15;
-        const float sinv = ldexpf(1.f, -(sexp[0] + sexp[1]));
         const float *acc_row = acc_s + e;
         int acc = 0;
         uint32_t tphase = 0;
@@ -184,14 +183,16 @@ corr_umma_kernel(const __grid_constant__ CUtensorMap tm_in_hi, const __grid_cons
             float dropped = -INFINITY;
             for (int rt = rt_b; rt < rt_e; ++rt) {
                 const int ry0 = (rt / p.rt_x) * TR_R, rx0 = (rt % p.rt_x) * TV;
-                float2 *rc = rcol + acc * UN;               // per column: score = V * scale + bias (bias = -inf: no such patch)
+                // per column: score = V * scale + bias, in search units (corr_internal.cuh); bias = -inf: no such patch,
+                // or one holding NaN / Inf (rinv NaN; its operands read as 0, so V is finite), which the rescoring scores
+                float2 *rc = rcol + acc * UN;
 #pragma unroll
                 for (int k = 0; k < UN / 128; ++k) {
                     const int n = e + k * 128;
                     const int uu = n >> 4, vv = n & 15;
                     const int ry = ry0 + uu, rx = rx0 + vv;
-                    const bool ok = vv < TV && ry < p.rh && rx < p.rw;
-                    rc[n] = ok ? make_float2(rinvb[ry * p.rw + rx] * sinv, 0.f) : make_float2(0.f, -INFINITY);
+                    const float ri = vv < TV && ry < p.rh && rx < p.rw ? rinvb[ry * p.rw + rx] : __int_as_float(0x7fffffff);
+                    rc[n] = ri == ri ? make_float2(ri, 0.f) : make_float2(0.f, -INFINITY);
                 }
                 asm volatile("bar.sync 1, 128;" ::: "memory");
                 mbar_wait(tfull, tphase);
@@ -318,7 +319,7 @@ int corr_search_umma_launch(const CorrGeom &g, const CorrWorkspace &ws, cudaStre
     C2M_CUDA(sm_count(sms));
     const int n_items = g.B * p.qt_x * p.qt_y * p.nchunk;
     const int grid = n_items < sms ? n_items : sms;
-    corr_umma_kernel<<<grid, 512, SMEM_BYTES, st>>>(tih, til, trh, ws.rinv, ws.sexp, ws.part, p);
+    corr_umma_kernel<<<grid, 512, SMEM_BYTES, st>>>(tih, til, trh, ws.rinv, ws.part, p);
     C2M_LAUNCH_CHECK("corr_umma_kernel");
     return C2M_OK;
 }

@@ -26,6 +26,10 @@
  *     score(q, r) = < P_in(q), P_ref(r) / (||P_ref(r)||_2 + 1e-5) >        (:62-67)
  *     idx(q) = argmax_r score, lowest r on ties (first max within a chunk :69, strict '>'
  *              across chunks :74-76  =>  globally the lowest index among equal maxima)
+ *              with torch's `max` rule for NaN: a NaN score is the maximum, the lowest-index NaN
+ *              wins and val is NaN; +Inf is an ordinary maximum.  (The reference's strict '>'
+ *              merge across chunks of 2^29 / (h*w) Ref patches makes NaN chunk-dependent once
+ *              NR*h*w > 2^29; this oracle is the single-chunk rule.)
  *     val(q) = max_r score, divided by (||P_in(q)||_2 + 1e-5) if norm_input  (:78-84)
  *
  * Arithmetic: the reference normalises the Ref patches in fp32 BEFORE the dot product
@@ -88,7 +92,8 @@ int oracle_corr_argmax(const float *fin, const float *fref, int C, int h, int w,
                 double acc = 0.0;
                 for (int k = 0; k < K; ++k) acc += (double)pq[k] * (double)p[k];
                 const float s = (float)acc;
-                if (s > best) { best = s; besti = r; }          /* strict '>' => lowest index */
+                /* torch's max: NaN is the maximum (the first NaN wins), otherwise strict '>' => lowest index */
+                if (!isnan(best) && (isnan(s) || s > best)) { best = s; besti = r; }
                 if (acc > best_d) { second_d = best_d; best_d = acc; }
                 else if (acc > second_d) second_d = acc;
             }

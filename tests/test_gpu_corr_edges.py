@@ -20,8 +20,8 @@ and items (`_over_sms` when CTAs run several).  What each case pins:
 - `below_10x15`: one column short of the threshold, so the generic search runs; it must give the same answer.
 Each runs with `l2norm` off and on (on: checked against `F.normalize` + the oracle).
 
-Dynamic range (`dyn_*`): the prep scales each map by one power of two chosen from its largest |x| over the whole
-batch, so elements far below it fall into the fp16 subnormals, where the rounding error of the operands is absolute
+Dynamic range (`dyn_*`): the prep scales each map of each image by one power of two chosen from its largest finite
+|x|, so elements far below it fall into the fp16 subnormals, where the rounding error of the operands is absolute
 rather than relative.  A query map at 1e-7 / 1e-8 with one element at 1.0, a Ref map at 1e-5 / 1e-6 with one
 element at 1e3, and a batch whose second image is the first times 1e-8 must still give the exact argmax.
 
